@@ -1,9 +1,9 @@
 """The reference arm of bench.py: the UNMODIFIED reference (EDAPINENUT/CBGBench) run through its own public API.
 
-``stage()``   copies the reference's Python package (``/root/reference/repo``) into the git-ignored ``baseline/_ref/``
-              so that it travels to the GPU box with the repo snapshot (the reference is pure Python and not
+``stage()``   installs the reference's Python package (``$CBG_REFERENCE/repo``, default ``/root/reference``) into the
+              git-ignored ``oracle/_ref/`` by the recipe ``oracle/stage_ref.py`` (the reference is pure Python and not
               pip-installable: this copy IS the install; nothing of it enters the git history).
-``install()`` puts the staged (or the live ``/root/reference``) tree on ``sys.path`` behind the shims of SURVEY.md
+``install()`` puts the staged tree on ``sys.path`` behind the shims of SURVEY.md
               Appendix C: fake ``easydict`` / ``rdkit``, ``torch_scatter`` + ``torch_geometric.nn.knn_graph`` restated with
               plain torch ops (those two packages are un-vendored third-party dependencies of the reference), empty
               package shells so the heavy ``__init__``s (lmdb, BioPython, real rdkit) are not executed.
@@ -17,7 +17,6 @@ Nothing of this repo's kernels, models or engine is on that path.  The scatter p
 the neighbour search has a batched on-device variant here so that the eager-GPU arm is not throttled by a host loop.
 """
 import os
-import shutil
 import sys
 import time
 import types
@@ -25,38 +24,14 @@ from unittest.mock import MagicMock
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
-STAGED = os.path.join(HERE, '_ref')
-LIVE = '/root/reference'
-
-
-def stage(force=False):
-    """Copy the reference's ``repo`` package (``*.py`` and the size-prior table) to baseline/_ref/.  Returns the path,
-    or None when /root/reference is absent (GPU box: the staged copy ships with the snapshot)."""
-    if not os.path.isdir(os.path.join(LIVE, 'repo')):
-        return STAGED if os.path.isdir(os.path.join(STAGED, 'repo')) else None
-    marker = os.path.join(STAGED, '.staged')
-    if os.path.exists(marker) and not force:
-        return STAGED
-    if os.path.isdir(STAGED):
-        shutil.rmtree(STAGED)
-    keep = ('.py', '.npy')
-    for dirpath, dirnames, filenames in os.walk(os.path.join(LIVE, 'repo')):
-        rel = os.path.relpath(dirpath, LIVE)
-        for fn in filenames:
-            if fn.endswith(keep):
-                os.makedirs(os.path.join(STAGED, rel), exist_ok=True)
-                shutil.copy2(os.path.join(dirpath, fn), os.path.join(STAGED, rel, fn))
-    with open(marker, 'w') as f:
-        f.write('staged from /root/reference (EDAPINENUT/CBGBench); git-ignored, ships to the GPU box with the snapshot\n')
-    return STAGED
+if ROOT not in sys.path:
+    sys.path.insert(0, ROOT)
+from oracle.stage_ref import STAGED, stage  # noqa: E402,F401
 
 
 def ref_root():
-    if os.path.isdir(os.path.join(STAGED, 'repo')):
-        return STAGED
-    if os.path.isdir(os.path.join(LIVE, 'repo')):
-        return LIVE
-    return None
+    """The staged reference (oracle/_ref), or None when build() found no reference to stage."""
+    return STAGED if os.path.isdir(os.path.join(STAGED, 'repo')) else None
 
 
 class EasyDict(dict):
@@ -125,7 +100,7 @@ def install(device_knn=True):
     """Make ``from repo.models.diffusion.targetdiff import TargetDiff`` importable.  Returns the root used."""
     root = ref_root()
     if root is None:
-        raise FileNotFoundError('no reference: neither baseline/_ref (run baseline/ref_runner.py stage) nor /root/reference')
+        raise FileNotFoundError('no staged reference: run oracle/stage_ref.py where the reference checkout is available')
     if 'repo.models.diffusion.targetdiff' in sys.modules:
         return root
     if ROOT not in sys.path:

@@ -4,6 +4,7 @@
 
     python bench.py --gpus N --steps K --warmup W            # this repo (CUDA path)
     python bench.py --impl reference --gpus N --steps K ...  # the reference's CPU path (oracle port)
+    python bench.py ... --dump-outputs DIR                   # + the last timed step's outputs as DIR/<name>.npy
     torchrun --nproc-per-node N ... bench.py --gpus N ...    # N > 1: one rank per GPU, weak scaling
 
 A "step" is ONE denoise step of the whole batch: ligand embedding -> device kNN -> edge gate ->
@@ -52,6 +53,11 @@ def parse_args():
                     help="weak: every rank gets the workload's pockets (default for c2/c3/c1); strong: ONE global batch is "
                          'partitioned over the ranks by atom count (default for c5: 256 ragged pockets over the box)')
     ap.add_argument('--global-graphs', type=int, default=None, help='pockets of the global batch for --scaling strong')
+    ap.add_argument('--dump-outputs', default=None, metavar='DIR',
+                    help='write what the timed path computed last (ligand coordinates and atom-type log-probabilities: of the '
+                         'last timed step, or the final state of the timed sample() call of the reference arms) as '
+                         'DIR/<name>.npy (float32; with --gpus N one file pair per rank, <name>.rank<r>.npy, each '
+                         "holding that rank's pockets); inputs are seeded, so two builds compare output for output")
     return ap.parse_args()
 
 
@@ -113,12 +119,19 @@ class ClockSampler:
                 'reasons': sorted(self.reasons), 'samples': len(self.samples)}
 
 
-def measured_peaks():
-    path = os.path.join(ROOT, 'MEASURED_PEAKS.json')
-    if os.path.exists(path):
-        with open(path) as f:
-            return json.load(f), 'measured'
-    return {'hbm_gbs': 6650.0, 'bf16_tflops': 1590.0}, 'fallback'
+def data_sheet_peaks():
+    """NVIDIA's data-sheet figures of the H100 SXM at its 700 W limit (dense f16 tensor rate, HBM3 bandwidth): an upper
+    bound, not a rate this card was seen to reach - a power-limited card sustains less."""
+    return {'hbm_gbs': 3350.0, 'f16_tflops': 989.0}, 'H100 SXM data sheet'
+
+
+def dump_outputs(out_dir, rank, world, pos, logp):
+    """--dump-outputs: the two arrays a caller of the timed path receives, float32."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    tag = f'.rank{rank}' if world > 1 else ''
+    np.save(os.path.join(out_dir, f'ligand_pos{tag}.npy'), pos.detach().float().cpu().numpy())
+    np.save(os.path.join(out_dir, f'ligand_type_logprob{tag}.npy'), logp.detach().float().cpu().numpy())
 
 
 def workload_batch(name, rank, n_graphs=None):
@@ -135,7 +148,7 @@ def workload_batch(name, rank, n_graphs=None):
 
 # ---------------------------------------------------------------------------------------------
 # Reference legs.  What is timed is the UNMODIFIED reference: TargetDiff.sample(batch) (repo/models/diffusion/
-# targetdiff.py:127-184) imported from baseline/_ref (staged copy of /root/reference, see baseline/ref_runner.py) with the
+# targetdiff.py:127-184) imported from oracle/_ref (staged copy of the reference, see baseline/ref_runner.py) with the
 # bench's seeded weights, on the FULL batch of the workload.  One sample() call with T = n steps is n denoise steps.
 def reference_enc(workload):
     """Encoder overrides the reference can run: its radius branch is dead code (unitransformer.py:76-77), so the c3
@@ -181,7 +194,7 @@ def run_reference(args):
     import torch
     from baseline import ref_runner
     if ref_runner.ref_root() is None:
-        print(json.dumps({'impl': args.impl, 'unavailable': 'baseline/_ref missing and /root/reference absent'}), flush=True)
+        print(json.dumps({'impl': args.impl, 'unavailable': 'no staged reference (oracle/_ref)'}), flush=True)
         return
     B, n_prot, n_lig, _, _, desc = WORKLOADS[args.workload]
     enc, note = reference_enc(args.workload)
@@ -192,7 +205,8 @@ def run_reference(args):
         torch.cuda.set_device(dev)
         warm_steps = max(2, args.warmup)
         ref_runner.time_sample(batch, enc, warm_steps, dev)                      # warm-up call (allocator, kernels)
-        sec, _ = ref_runner.time_sample(batch, enc, max(2, args.steps), dev)
+        torch.manual_seed(2024)
+        sec, traj = ref_runner.time_sample(batch, enc, max(2, args.steps), dev)
         threads, tried = torch.get_num_threads(), None
         kind = 'reference eager PyTorch on one GPU (unmodified TargetDiff.sample, torch-op shims for pyg/scatter)'
     else:
@@ -200,8 +214,11 @@ def run_reference(args):
         while warm_steps < args.warmup:                                         # top up to the requested warm-up
             ref_runner.time_sample(batch, enc, 2, 'cpu', threads=threads)
             warm_steps += 2
-        sec, _ = ref_runner.time_sample(batch, enc, max(2, args.steps), 'cpu', threads=threads)
+        torch.manual_seed(2024)
+        sec, traj = ref_runner.time_sample(batch, enc, max(2, args.steps), 'cpu', threads=threads)
         kind = 'reference CPU path (unmodified TargetDiff.sample, torch CPU fp32)'
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, 0, 1, traj[-1][0], traj[-1][1])      # final state of the timed sample() call
     n_timed = max(2, args.steps)
     sec_step = sec / n_timed
     value = B / (T_STEPS * sec_step)
@@ -285,7 +302,7 @@ def run_b200(args):
     Cc = torch.empty((T_STEPS + 1, n_lig_tot, K), device=dev)
     X[T_STEPS].copy_(state['x_lig'])
     Cc[T_STEPS].copy_(state['c_lig'])
-    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)   # > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)   # > 50 MB L2
     t_seq = list(reversed(range(T_STEPS)))
     model.run_steps(state, t_seq[:args.warmup], X, Cc)
     barrier()
@@ -300,6 +317,10 @@ def run_b200(args):
             ends[i].record()
         barrier()
     gpu_launches = L.cbg_launch_count() - launches0
+    if args.dump_outputs:
+        # what a caller of run_steps receives from the last timed step: the ligand state it wrote at index t
+        t_last = t_seq[args.warmup + args.steps - 1]
+        dump_outputs(args.dump_outputs, rank, world, X[t_last], Cc[t_last])
     step_ms = [s.elapsed_time(e) for s, e in zip(starts, ends)]
     ms_per_step = sum(step_ms) / len(step_ms)
     t = torch.tensor([ms_per_step], device=dev, dtype=torch.float64)
@@ -317,7 +338,7 @@ def run_b200(args):
         model.run_steps(state, t_seq[p0:p0 + args.profile_steps], X, Cc)
         prof = _lib.profile_collect()
         L.cbg_profile_enable(0)
-    peaks, peak_kind = measured_peaks()
+    peaks, peak_kind = data_sheet_peaks()
     roofline, kernels = None, None
     if prof:
         kernels = {k: {'ms_per_step': v[0] / args.profile_steps, 'launches_per_step': v[1] / args.profile_steps}
@@ -336,43 +357,33 @@ def run_b200(args):
             rows_src = sum(cnt[l] for l in range(n_layers)) / n_layers          # rows whose Pj plane a launch may gather
         else:
             rows_src = rows
-        traffic, ncu_info = None, None
-        tpath = os.path.join(ROOT, 'profiles', 'ncu_traffic.json')      # dram bytes/launch from the last ncu --set full capture
-        if os.path.exists(tpath):
-            with open(tpath) as f:
-                rec = json.load(f).get(dom + '_tc') or {}
-            traffic = rec.get('dram_bytes_per_launch')
-            ncu_info = rec.get('ncu')
-        # The fused X2H kernels (csrc/x2h_tc.cu) are TENSOR-bound, not HBM-bound (DESIGN.md section 5): per 128-edge tile
-        # they issue 17 + 48 tcgen05 MMAs, nothing of size [E, 128] crosses HBM.
-        #   executed tensor FLOPs per tile = 17 x (128 x 128 x 16 x 2) + 48 x (128 x 64 x 16 x 2); the (hi, lo) f16 split
+        # The fused X2H kernels (csrc/x2h_tc.cu) are bounded on the compute side, not by HBM (DESIGN.md section 5): per
+        # 128-edge tile they issue 2 x (17 + 24) wgmma m64n128k16, nothing of size [E, 128] crosses HBM.
+        #   executed tensor FLOPs per tile = (17 + 24) x (128 x 128 x 16 x 2); the (hi, lo) f16 split
         #   runs three f16 products per fp32 product and pads K = 84 to 96
         #   algorithmic (fp32-equivalent) FLOPs per edge and kernel = (84 + 128) x 128 x 2   (first-Linear RBF part + second Linear)
         #   algorithmic HBM bytes per launch: node planes read once + per-row neighbour / gate / coordinate rows + w / h
         tiles = rows / 4.0
-        exec_flops = tiles * (17 * 128 * 128 * 16 * 2 + 48 * 128 * 64 * 16 * 2)
+        exec_flops = tiles * (17 + 24) * 128 * 128 * 16 * 2
         alg_flops = rows * 32 * (84 + 128) * 128 * 2
         per_row = {'x2h_k': 512 + 512 + 128 + 128 + 16 + 2048, 'x2h_v': 512 + 128 + 16 + 2048 + 1024}[dom]
         alg_bytes = per_row * rows + 512 * rows_src
-        tf_peak = peaks.get('bf16_tflops_sustained') or peaks.get('bf16_tflops')
+        tf_peak = peaks['f16_tflops']
         ach_exec = exec_flops / (dom_ms * 1e-3) / 1e12
         ach_alg = alg_flops / (dom_ms * 1e-3) / 1e12
         hbm = alg_bytes / (dom_ms * 1e-3) / 1e9
         roofline = {'kernel': dom + ' (x2h_tc_kernel)', 'bound': 'tensor', 'achieved': ach_alg, 'peak': tf_peak / 3.0, 'unit': 'TFLOP/s',
-                    'frac': ach_alg / (tf_peak / 3.0), 'traffic': traffic,
-                    'peak_source': f'{peak_kind} bf16 cuBLAS TFLOP/s sustained (MEASURED_PEAKS.json: {tf_peak}) / 3: the fp32-accurate '
+                    'frac': ach_alg / (tf_peak / 3.0),
+                    'peak_source': f'{peak_kind} dense f16 TFLOP/s ({tf_peak}, not a measured rate) / 3: the fp32-accurate '
                                    '(hi, lo) f16 split needs three tensor-core products per algorithmic product',
+                    'device': torch.cuda.get_device_name(dev),
                     'algorithmic_flops_per_launch': alg_flops, 'launch_ms': dom_ms, 'rows_per_launch': rows,
                     'executed': {'tflops': ach_exec, 'peak_tflops': tf_peak, 'frac': ach_exec / tf_peak,
-                                 'note': 'tcgen05 FLOPs actually issued (3 products, K padded 84 -> 96)'},
+                                 'note': 'wgmma FLOPs actually issued (3 products, K padded 84 -> 96)'},
                     'hbm': {'algorithmic_bytes_per_launch': alg_bytes, 'achieved_gbs': hbm, 'peak_gbs': peaks['hbm_gbs'],
                             'frac': hbm / peaks['hbm_gbs'],
-                            'note': "the north-star's 60 % HBM target assumed per-edge k/v tensors crossing HBM (9.9 GB/step); they are "
-                                    'never materialised, the kernel moves ~4 KB per node and is bounded on the compute side'},
-                    # what shares the SM with the tensor pipe (DESIGN.md section 5.2): LSU wavefronts of the last ncu capture of
-                    # this kernel (unpruned launch, 5184 tiles) and the B-operand bytes the 41 MMAs of a tile read from shared memory
-                    'shared_memory': {'ncu_capture': ncu_info, 'mma_b_operand_bytes_per_tile': 41 * 128 * 16 * 2,
-                                      'note': 'static evidence from profiles/ncu_traffic.json (ncu --set full), not measured in this run'}}
+                            'note': 'per-edge k/v tensors are never materialised: the kernel moves ~4 KB per node and is bounded '
+                                    'on the compute side'}}
 
     # ---- end to end through the public API: host batch -> model.sample() -> host trajectory -------
     e2e = None

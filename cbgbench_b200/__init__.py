@@ -1,7 +1,7 @@
-"""cbgbench_b200 - B200-native implementation of CBGBench's diffusion-sampling hot path.
+"""cbgbench_b200 - H100-native (sm_90a) implementation of CBGBench's diffusion-sampling hot path.
 
 Only what the path needs (DESIGN.md):
-  csrc/         hand-written sm_100a CUDA kernels + the C-ABI (include/cbg_b200.h)
+  csrc/         hand-written sm_90a CUDA kernels + the C-ABI (include/cbg_b200.h)
   modules.py    nn.Module mirror of the reference denoiser (same signatures / state-dict keys)
   targetdiff.py TargetDiff.sample drop-in (outer diffusion loop in Python, one C call per step)
   diffsbdd.py   DiffSBDD.sample drop-in (row f2: variational schedule + COM projection on the same denoiser)

@@ -1,6 +1,6 @@
-"""Build libcbg_b200.so in-tree with nvcc for sm_100a (cross-compiles without a GPU).
+"""Build libcbg_b200.so in-tree with nvcc for sm_90a (H100; cross-compiles without a GPU).
 
-The shared library is git-ignored but travels to the GPU box with the repo snapshot.
+The shared library is a build product and git-ignored.
 """
 import os
 import subprocess
@@ -11,7 +11,7 @@ CSRC = os.path.join(HERE, 'csrc')
 LIB_PATH = os.path.join(HERE, 'libcbg_b200.so')
 SOURCES = ['api.cu', 'graph.cu', 'node_gemm.cu', 'node_gemm_tc.cu', 'node_gemm_f16.cu', 'edge.cu', 'x2h_tc.cu', 'misc.cu', 'batch.cu', 'ipa.cu']
 HEADERS = ['cbg_common.cuh', 'cbg_kernels.cuh', 'cbg_layout.h', 'cbg_tc.cuh', '../../include/cbg_b200.h']
-NVCC_FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a', '-lineinfo', '-O3', '-std=c++17',
+NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-O3', '-std=c++17',
               '-Xcompiler', '-fPIC', '-shared']
 
 

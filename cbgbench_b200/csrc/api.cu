@@ -73,7 +73,7 @@ struct Workspace {
   int* cnt;
   float* ew;
   float* dx;
-  float* hw;                   // H2X on the tcgen05 kernel: alpha * e_w of the generated nodes' edges, compact [n_gen,32,16]
+  float* hw;                   // H2X on the wgmma tile kernel: alpha * e_w of the generated nodes' edges, compact [n_gen,32,16]
   int* tickets;                // 64 work counters of the X2H launches of one step (dynamic node scheduling)
   unsigned char* fstat;        // per node: all 32 in-edges static this step (written by the edge gate when an R-cache is used)
   StepIO* io;                  // per-step pointers / coefficients of a graph-replayed step (cbg_sample_step_graph_f32)
@@ -118,7 +118,7 @@ int check_ws(const void* workspace, size_t have, long long n_nodes, long long n_
   return 0;
 }
 
-// node GEMM implementation: tcgen05 kind::f16 with the (hi, lo) split (default), CBG_NODE_GEMM=tf32 the 3xTF32
+// node GEMM implementation: wgmma f16 with the (hi, lo) split (default), CBG_NODE_GEMM=tf32 the 3xTF32
 // kernel, CBG_NODE_GEMM=simt the fp32 SIMT kernel
 int node_gemm_impl() {
   static int impl = -1;
@@ -598,7 +598,7 @@ int32_t cbg_sample_begin_f32(const cbg_sample_plan* plan, const float* x_nodes, 
     if (int rc = cbg_launch_edge_gate(plan->blob, ws.x4, ws.snbr, plan->n_nodes, nullptr, nullptr, ws.sew, st)) return rc;
   }
   if (plan->rcache) {
-    // step-invariant first-Linear terms of the static edges, for the legacy (non-tcgen05) X2H kernels
+    // step-invariant first-Linear terms of the static edges, for the fp32 SIMT X2H kernels
     const int64_t need = cbg_rcache_bytes(plan->n_nodes, plan->num_layers);
     if ((int64_t)plan->rcache_bytes < need) { cbg_set_error("rcache too small: have %zu bytes, need %lld", plan->rcache_bytes, (long long)need); return 1; }
     if (int rc = cbg_launch_rcache(plan->blob + cbg_layout::kGlobalFloats, plan->num_layers, ws.x4, ws.snbr,

@@ -1,4 +1,4 @@
-// Shared device helpers for the cbg_b200 kernels (sm_100a).
+// Shared device helpers for the cbg_b200 kernels (sm_90a).
 #pragma once
 #include <stdlib.h>
 #include <cuda_runtime.h>
@@ -48,10 +48,10 @@ void cbg_prof_mark(int family, int is_end, cudaStream_t st);
 
 // Launch with (or without) programmatic stream serialization: the kernel may be scheduled before the previous kernel of
 // the stream has finished; it must execute griddepcontrol.wait (cbg_tc.cuh: pdl_wait) before touching anything that
-// kernel produces or still reads.  Off unless CBG_PDL=1 (measured at c2 / c1 under graph replay: no gain, DESIGN.md section 5.3).
+// kernel produces or still reads.  Off unless CBG_PDL=1 (DESIGN.md section 5.3).
 inline bool cbg_pdl_enabled() {
   static int on = -1;
-  if (on < 0) { const char* e = getenv("CBG_PDL"); on = (e && e[0] == '1') ? 1 : 0; }      // opt-in: measured neutral under graph replay
+  if (on < 0) { const char* e = getenv("CBG_PDL"); on = (e && e[0] == '1') ? 1 : 0; }
   return on != 0;
 }
 template <typename... KArgs, typename... Args>
@@ -95,38 +95,42 @@ __device__ __forceinline__ float4 ld4(const float* p) { return *reinterpret_cast
 __device__ __forceinline__ float4 ldg4(const float* p) { return __ldg(reinterpret_cast<const float4*>(p)); }
 __device__ __forceinline__ void st4(float* p, float4 v) { *reinterpret_cast<float4*>(p) = v; }
 
-// Blackwell packed fp32: FFMA2 / FMUL2 / FADD2 execute two IEEE-rn operations per issued instruction
-// (sm_100a; a scalar second operand is broadcast by the hardware).  Bit-identical to the scalar forms,
-// half the issue slots - the edge kernels are issue-limited, not FMA-pipe-limited.
+// Pairwise fp32 helpers: two IEEE-rn operations on the halves of a float2 (Hopper has no packed fp32 instruction:
+// these compile to two scalar FFMA / FMUL / FADD and are bit-identical to the scalar forms).
+__device__ __forceinline__ float2 ffma2(const float2 a, const float2 b, const float2 c) {
+  return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
+}
+__device__ __forceinline__ float2 fmul2(const float2 a, const float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 fadd2(const float2 a, const float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
 __device__ __forceinline__ void fma4(float4& acc, const float4 w, const float s) {
   const float2 ss = make_float2(s, s);
-  const float2 lo = __ffma2_rn(make_float2(w.x, w.y), ss, make_float2(acc.x, acc.y));
-  const float2 hi = __ffma2_rn(make_float2(w.z, w.w), ss, make_float2(acc.z, acc.w));
+  const float2 lo = ffma2(make_float2(w.x, w.y), ss, make_float2(acc.x, acc.y));
+  const float2 hi = ffma2(make_float2(w.z, w.w), ss, make_float2(acc.z, acc.w));
   acc = make_float4(lo.x, lo.y, hi.x, hi.y);
 }
 __device__ __forceinline__ float4 add4(const float4 a, const float4 b) {
-  const float2 lo = __fadd2_rn(make_float2(a.x, a.y), make_float2(b.x, b.y));
-  const float2 hi = __fadd2_rn(make_float2(a.z, a.w), make_float2(b.z, b.w));
+  const float2 lo = fadd2(make_float2(a.x, a.y), make_float2(b.x, b.y));
+  const float2 hi = fadd2(make_float2(a.z, a.w), make_float2(b.z, b.w));
   return make_float4(lo.x, lo.y, hi.x, hi.y);
 }
 __device__ __forceinline__ float4 add4s(const float4 a, const float s) {
   const float2 ss = make_float2(s, s);
-  const float2 lo = __fadd2_rn(make_float2(a.x, a.y), ss);
-  const float2 hi = __fadd2_rn(make_float2(a.z, a.w), ss);
+  const float2 lo = fadd2(make_float2(a.x, a.y), ss);
+  const float2 hi = fadd2(make_float2(a.z, a.w), ss);
   return make_float4(lo.x, lo.y, hi.x, hi.y);
 }
 // a.x*b.x + a.y*b.y + a.z*b.z + a.w*b.w as (x,z | y,w) packed partial sums
 __device__ __forceinline__ float dot4(const float4 a, const float4 b) {
-  float2 t = __fmul2_rn(make_float2(a.x, a.y), make_float2(b.x, b.y));
-  t = __ffma2_rn(make_float2(a.z, a.w), make_float2(b.z, b.w), t);
+  float2 t = fmul2(make_float2(a.x, a.y), make_float2(b.x, b.y));
+  t = ffma2(make_float2(a.z, a.w), make_float2(b.z, b.w), t);
   return t.x + t.y;
 }
 // relu((a * rstd) * gamma + beta)
 __device__ __forceinline__ float4 ln_relu4(const float4 a, const float rstd, const float4 gamma, const float4 beta) {
   const float2 rr = make_float2(rstd, rstd);
-  float2 lo = __fmul2_rn(make_float2(a.x, a.y), rr), hi = __fmul2_rn(make_float2(a.z, a.w), rr);
-  lo = __ffma2_rn(lo, make_float2(gamma.x, gamma.y), make_float2(beta.x, beta.y));
-  hi = __ffma2_rn(hi, make_float2(gamma.z, gamma.w), make_float2(beta.z, beta.w));
+  float2 lo = fmul2(make_float2(a.x, a.y), rr), hi = fmul2(make_float2(a.z, a.w), rr);
+  lo = ffma2(lo, make_float2(gamma.x, gamma.y), make_float2(beta.x, beta.y));
+  hi = ffma2(hi, make_float2(gamma.z, gamma.w), make_float2(beta.z, beta.w));
   return make_float4(fmaxf(lo.x, 0.f), fmaxf(lo.y, 0.f), fmaxf(hi.x, 0.f), fmaxf(hi.y, 0.f));
 }
 

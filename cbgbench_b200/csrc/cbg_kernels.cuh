@@ -52,9 +52,9 @@ struct NodeGemmArgs {
   long long* trace;        // debug: globaltimer stamps of CTA 0 (cbg_debug_node_gemm_trace)
 };
 int cbg_launch_node_gemm(const NodeGemmArgs& a, cudaStream_t st);      // fp32 SIMT
-// tcgen05 3xTF32; cluster = 1/2/4 CTAs sharing weight chunks by multicast, 0 = default (env CBG_GEMM_CLUSTER)
+// wgmma 3xTF32; cluster = 1/2/4 CTAs sharing weight chunks by multicast, 0 = default (env CBG_GEMM_CLUSTER)
 int cbg_launch_node_gemm_tc(const NodeGemmArgs& a, cudaStream_t st, int cluster = 0);
-// tcgen05 kind::f16 with the (hi, lo) split: default
+// wgmma f16 with the (hi, lo) split: default
 int cbg_launch_node_gemm_f16(const NodeGemmArgs& a, cudaStream_t st);
 void cbg_node_gemm_f16_set_trace(long long* buf_dev);
 
@@ -79,19 +79,19 @@ struct EdgeArgs {
   const float* rc_v;
   int* ticket;           // x2h: optional work counter (zeroed by the caller) for dynamic node scheduling; k uses ticket[0], v ticket[1]
   const unsigned char* fstat;  // x2h with an R-cache: 1 = all 32 in-edges of the node are static (nbr row == its static list)
-  long long* trace;      // x2h_tc debugging: per-tile SM-clock stamps of CTA 0 ([tile][16 events]) or nullptr
+  long long* trace;      // x2h_tc debugging: per-tile SM-clock stamps of CTA 0 ([tile][16 event slots]) or nullptr
   int trace_tiles;
   int w_compact;         // x2h_tc: 1 = w is indexed by the position in node_idx ([n_nodes,32,16], H2X), 0 = by node id
 };
 int cbg_launch_rcache(const float* layers, int num_layers, const float4* x4, const int* snbr, int n_nodes,
                       float* rcache, cudaStream_t st);
 int cbg_launch_x2h(const EdgeArgs& a, cudaStream_t st);
-// x2h_tc.cu: both X2H kernels on tcgen05 (A operands in TMEM, f16 hi/lo split); edge order of w = neighbour-table order
+// x2h_tc.cu: both X2H kernels on wgmma (activations as register A fragments, f16 hi/lo split); edge order of w = neighbour-table order
 int cbg_launch_x2h_tc(const EdgeArgs& a, cudaStream_t st);
-// hardware self-test of the tcgen05 operand conventions (tests): d[128][128] = a[128][32] * b[128][32]^T, f16 inputs
+// hardware self-test of the wgmma operand conventions (tests): d[128][128] = a[128][32] * b[128][32]^T, f16 inputs
 // debugging: x2h_tc kernels of later launches stamp CTA 0's pipeline events into buf ([max_tiles][16] int64; nullptr = off)
 void cbg_x2h_tc_set_trace(long long* buf, int max_tiles);
-// H2X on the same tcgen05 kernel (generated nodes only): a.w = compact [n_nodes,32,16] scratch, a.dx = [n_nodes,4] out
+// H2X on the same wgmma kernel (generated nodes only): a.w = compact [n_nodes,32,16] scratch, a.dx = [n_nodes,4] out
 int cbg_launch_h2x_tc(const EdgeArgs& a, cudaStream_t st);
 int cbg_launch_umma_selftest(const void* a, const void* b, float* d, int a_from_smem, cudaStream_t st);
 int cbg_launch_h2x(const EdgeArgs& a, cudaStream_t st);

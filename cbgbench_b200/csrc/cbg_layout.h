@@ -45,8 +45,8 @@
   X(X2H_V_W1, 128 * 128)     /* hv_func.net.3.weight natural [f_out][f_in] */            \
   X(X2H_V_B1, 128)           /* hv_func.net.3.bias */                                    \
   X(X2H_V_RBF, 32)                                                                       \
-  /* X2H node GEMM weights for the tcgen05 path: 6 planes [Pj_k,Pj_v,Pi_k,Pi_v,q_hidden,q_out],   \
-     each = 4 K-chunks x (hi | lo) x [128 n][32 k] tf32 in UMMA canonical K-major layout */       \
+  /* X2H node GEMM weights for the 3xTF32 wgmma path: 6 planes [Pj_k,Pj_v,Pi_k,Pi_v,q_hidden,q_out],   \
+     each = 4 K-chunks x (hi | lo) x [128 n][32 k] tf32 in the canonical K-major layout  */       \
   X(X2H_NODE_TC, 6 * 32768)                                                              \
   /* H2X node GEMM */                                                                    \
   X(H2X_NODE_WT, 128 * 640)                                                              \
@@ -66,18 +66,18 @@
   X(H2X_V_W1, 16 * 128)      /* xv_func.net.3.weight [head][f_in] */                     \
   X(H2X_V_B1, 32)            /* xv_func.net.3.bias[16], zero padded */                   \
   X(H2X_RBF, 32)                                                                         \
-  /* tcgen05 X2H kernels (x2h_tc.cu): f16 (hi | lo) operand images in the UMMA canonical K-major layout.        \
+  /* wgmma X2H kernels (x2h_tc.cu): f16 (hi | lo) operand images in the canonical K-major no-swizzle layout.   \
      TCW1 = 64 * W1 [128 n][128 k]; TCWG = [128 n][96 k] with k < 80: 16 * Wrf[t][m] at k = 20 t + m,           \
-     k = 80 + t: 16 * c[t], k >= 84: zero (the kernel writes the tile's Pi rows there).  Sizes in floats. */    \
+     k = 80 + t: 16 * c[t], k >= 84: zero padding to K = 96.  Sizes in floats. */                       \
   X(X2H_K_TCW1, 2 * 128 * 128 / 2)                                                       \
   X(X2H_K_TCWG, 2 * 128 * 96 / 2)                                                        \
   X(X2H_V_TCW1, 2 * 128 * 128 / 2)                                                       \
   X(X2H_V_TCWG, 2 * 128 * 96 / 2)                                                        \
-  /* node GEMM weights for the f16 tcgen05 path (node_gemm_f16.cu): the 6 planes of X2H_NODE_TC / H2X_NODE_TC, each as   \
-     2 K-chunks x (hi | lo) x [128 n][64 k] f16 of 256 * W in the UMMA canonical K-major layout.  Sizes in floats. */   \
+  /* node GEMM weights for the f16 wgmma path   (node_gemm_f16.cu): the 6 planes of X2H_NODE_TC / H2X_NODE_TC, each as   \
+     2 K-chunks x (hi | lo) x [128 n][64 k] f16 of 256 * W in the canonical K-major layout.  Sizes in floats. */        \
   X(X2H_NODE_TCH, 6 * 2 * 2 * 128 * 64 / 2)                                              \
   X(H2X_NODE_TCH, 6 * 2 * 2 * 128 * 64 / 2)                                              \
-  /* tcgen05 H2X kernels (x2h_tc.cu, modes H2X-k / H2X-v): same images for the xk / xv edge MLPs of H2XAttention; the    \
+  /* wgmma   H2X kernels (x2h_tc.cu, modes H2X-k / H2X-v): same images for the xk / xv edge MLPs of H2XAttention; the    \
      second Linear of xv has 16 outputs (one per head): TCW1 = 64 * W1xv as a [16 n][128 k] (hi | lo) image */          \
   X(H2X_K_TCW1, 2 * 128 * 128 / 2)                                                       \
   X(H2X_K_TCWG, 2 * 128 * 96 / 2)                                                        \

@@ -294,10 +294,10 @@ struct ULeaf {
   __device__ __forceinline__ void eval2(float (&lo)[4], float (&hi)[4]) const {
 #pragma unroll
     for (int ee = 0; ee < 4; ++ee) {
-      float2 t = __fmul2_rn(make_float2(U[0][HP], U[0][HP + 1]), make_float2(a[ee].x, a[ee].x));
-      t = __ffma2_rn(make_float2(U[1][HP], U[1][HP + 1]), make_float2(a[ee].y, a[ee].y), t);
-      t = __ffma2_rn(make_float2(U[2][HP], U[2][HP + 1]), make_float2(a[ee].z, a[ee].z), t);
-      t = __ffma2_rn(make_float2(U[3][HP], U[3][HP + 1]), make_float2(a[ee].w, a[ee].w), t);
+      float2 t = fmul2(make_float2(U[0][HP], U[0][HP + 1]), make_float2(a[ee].x, a[ee].x));
+      t = ffma2(make_float2(U[1][HP], U[1][HP + 1]), make_float2(a[ee].y, a[ee].y), t);
+      t = ffma2(make_float2(U[2][HP], U[2][HP + 1]), make_float2(a[ee].z, a[ee].z), t);
+      t = ffma2(make_float2(U[3][HP], U[3][HP + 1]), make_float2(a[ee].w, a[ee].w), t);
       lo[ee] = t.x;
       hi[ee] = t.y;
     }
@@ -663,7 +663,7 @@ __global__ void __launch_bounds__(256) rcache_kernel(const float* __restrict__ l
 int g_num_sms = 0;
 int g_edge_warps = 12;
 int g_h2x_impl = -1;       // -1: follow g_edge_impl; CBG_H2X_IMPL=simt|tc overrides
-int g_edge_impl = 6;       // 6 (default): tcgen05 kernels (x2h_tc.cu); 0: the fp32 SIMT kernels above (tested alternative, R-cache capable)
+int g_edge_impl = 6;       // 6 (default): wgmma tile kernels (x2h_tc.cu); 0: the fp32 SIMT kernels above (tested alternative, R-cache capable)
 int g_h2x_warps = 12;
 
 template <int W>
@@ -753,7 +753,7 @@ int cbg_launch_rcache(const float* layers, int num_layers, const float4* x4, con
 int cbg_launch_x2h(const EdgeArgs& a, cudaStream_t st) {
   if (a.n_nodes <= 0) return 0;
   if (int rc = cbg_edge_init()) return rc;
-  if (g_edge_impl == 6) return cbg_launch_x2h_tc(a, st);       // tcgen05 kernels (x2h_tc.cu)
+  if (g_edge_impl == 6) return cbg_launch_x2h_tc(a, st);       // wgmma tile kernels (x2h_tc.cu)
   switch (g_edge_warps) {
     case 8: return launch_x2h<8>(a, st);
     case 16: return launch_x2h<16>(a, st);
@@ -764,7 +764,7 @@ int cbg_launch_x2h(const EdgeArgs& a, cudaStream_t st) {
 int cbg_launch_h2x(const EdgeArgs& a, cudaStream_t st) {
   if (a.n_nodes <= 0) return 0;
   if (int rc = cbg_edge_init()) return rc;
-  // default: the tcgen05 tile kernel (x2h_tc.cu, needs the compact w scratch); the fp32 SIMT kernel below stays as the
+  // default: the wgmma tile kernel (x2h_tc.cu, needs the compact w scratch); the fp32 SIMT kernel below stays as the
   // independent cross-check (cbg_set_edge_impl(0) or CBG_H2X_IMPL=simt)
   if ((g_h2x_impl < 0 ? g_edge_impl : g_h2x_impl) == 6 && a.w != nullptr) return cbg_launch_h2x_tc(a, st);
   switch (g_h2x_warps) {
@@ -777,7 +777,7 @@ int cbg_launch_h2x(const EdgeArgs& a, cudaStream_t st) {
 // testing hook (include/cbg_b200.h): pick the X2H edge-kernel implementation and the SIMT kernels' warps per CTA
 int cbg_edge_set_impl(int impl, int warps) {
   if (int rc = cbg_edge_init()) return rc;
-  if (impl != 0 && impl != 6) { cbg_set_error("edge impl must be 6 (tcgen05, default) or 0 (fp32 SIMT)"); return 1; }
+  if (impl != 0 && impl != 6) { cbg_set_error("edge impl must be 6 (wgmma, default) or 0 (fp32 SIMT)"); return 1; }
   if (warps != 0 && warps != 8 && warps != 12 && warps != 16) { cbg_set_error("warps per CTA must be 8, 12 or 16"); return 1; }
   g_edge_impl = impl;
   if (warps && impl == 0) g_edge_warps = warps;

@@ -6,7 +6,7 @@
 // Same algebra as the 128-wide denoiser (DESIGN.md section 3): the first Linear of the edge MLPs is split into node planes
 // (Pj, Pi), a type-dependent RBF mat-vec and a type bias, [E, 2H + 84] is never formed, the key bias cancels in the
 // softmax.  The kernels here are width-generic fp32 SIMT kernels (one CTA per destination node, thread = feature): this
-// row is built to the parity bar; the tcgen05 tile kernels (x2h_tc.cu) are specialised for H = 128 (TMEM budget).
+// row is built to the parity bar; the wgmma tile kernels (x2h_tc.cu) are specialised for H = 128 (register budget of the accumulator fragments).
 // Graph construction (kNN) and the edge gate are the hot path's own kernels (graph.cu).
 #include <math.h>
 #include "cbg_kernels.cuh"

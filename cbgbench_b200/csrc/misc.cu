@@ -414,7 +414,7 @@ int cbg_launch_classifier(const float* blob_global, const float* h, const int* r
     attr_set = true;
   }
   int grid = (n_rows + 7) / 8;
-  if (grid > 2 * 148) grid = 2 * 148;
+  if (grid > 2 * 132) grid = 2 * 132;
   CBG_PROF_BEGIN(CBG_K_CLASSIFIER, st);
   classifier_kernel<<<grid, 256, kClsFloats * 4, st>>>(blob_global + cbg_layout::global_offset(CBG_GF_CLS_W0T), h,
                                                        row_idx, n_rows, num_classes, logits);

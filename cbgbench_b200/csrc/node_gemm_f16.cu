@@ -1,17 +1,16 @@
-// Node-level projections on tcgen05 with the f16 (hi, lo) split (kind::f16, three products per K step, fp32 accumulate
-// in TMEM): same contract as node_gemm_tc.cu (planes Pj_k, Pj_v, Pi_k, Pi_v, q of one attention sub-layer; reference:
-// x2h_attention.py:58-83, h2x_attention.py:42-62, common.py:151-171), half the tensor-core time and half the operand
-// bytes of the 3xTF32 version at the same accuracy class (cbg_tc.cuh).
+// Node-level projections on the Hopper tensor cores (wgmma) with the f16 (hi, lo) split (three products per K step, fp32
+// accumulate in registers): same contract as node_gemm_tc.cu (planes Pj_k, Pj_v, Pi_k, Pi_v, q of one attention
+// sub-layer; reference: x2h_attention.py:58-83, h2x_attention.py:42-62, common.py:151-171), half the tensor-core time
+// and half the operand bytes of the 3xTF32 version at the same accuracy class (cbg_tc.cuh).
 //
-// One CTA = one 128-row tile.  A (rows of h, scaled by 16) is split once per CTA into hi/lo f16 tiles in shared memory
-// (UMMA canonical K-major layout); the weight planes (scaled by 256) are pre-split and pre-laid-out by the packer in
-// 64-wide K chunks (hi | lo = 32 KB) and stream through a 2-stage ring with cp.async.bulk + mbarrier; warp-specialised:
-// 8 staging/epilogue warps, a copy thread, an MMA thread, four TMEM accumulators (plane g+1 accumulates while plane g
-// drains).  LayerNorm + ReLU of the q MLP is done out of TMEM and fed back as the A operand of its second Linear.
-// Epilogue: a thread owns one accumulator ROW (tcgen05.ld 32x32b), but a plane row is 512 contiguous bytes in global
-// memory, so each warp transposes its 32 x 32 block through a swizzled shared-memory tile and stores full 128-byte
-// lines (4 rows per instruction).  Storing straight from the TMEM layout (16 B per lane into 32 different rows, half a
-// sector each) made the epilogue, not the MMAs, the per-plane cost: 3.2 us against 0.9 us of tensor time.
+// One CTA = one 128-row tile = two consumer warpgroups of 64 rows (wgmma M = 64) + a copy warp.  A (rows of h, scaled by
+// 16) is split once per CTA into hi/lo f16 tiles in shared memory (canonical K-major layout, read through wgmma
+// descriptors); the weight planes (scaled by 256) are pre-split and pre-laid-out by the packer in 64-wide K chunks
+// (hi | lo = 32 KB) and stream through a 3-stage ring with cp.async.bulk + mbarrier.  Each warpgroup holds the
+// 64 x 128 fp32 accumulator of its rows in registers and runs the epilogue from them: a quad of lanes owns 8 consecutive
+// columns of a row, so the plane rows go to global memory as full 32-byte sectors with no staging.  LayerNorm + ReLU
+// of the q MLP is done in registers (row sums over the quad) and written to a second (hi | lo) A tile for the second
+// Linear; only the owning warpgroup reads those rows back, so that hand-over is a warpgroup barrier.
 #include "cbg_kernels.cuh"
 #include "cbg_tc.cuh"
 
@@ -19,11 +18,10 @@ using namespace cbg_tc;
 
 namespace {
 
-constexpr int TM = 128;                        // rows per CTA (UMMA M)
+constexpr int TM = 128;                        // rows per CTA (2 x wgmma M)
 constexpr int KC = 64;                         // K elements per weight chunk
 constexpr int NKC = CBG_H / KC;                // 2 chunks per plane
-constexpr int STAGES = 2;
-constexpr int NACC = 4;                        // TMEM accumulators (128 columns each)
+constexpr int STAGES = 3;
 constexpr uint32_t A_TILE = TM * CBG_H * 2;                // 32 KB per (hi | lo)
 constexpr uint32_t B_CHUNK = 128 * KC * 2;                 // 16 KB per (hi | lo)
 constexpr uint32_t B_STAGE = 2 * B_CHUNK;
@@ -31,13 +29,9 @@ constexpr uint32_t SM_A_HI = 0;                            // rows of h (hi at +
 constexpr uint32_t SM_Q = 2 * A_TILE;                      // relu(LN(q hidden)), same (hi | lo) layout
 constexpr uint32_t SM_B0 = 4 * A_TILE;
 constexpr uint32_t SM_BARS = SM_B0 + STAGES * B_STAGE;
-constexpr uint32_t SM_RED = SM_BARS + 256;                 // [2 passes][2 halves][128 rows] floats
-constexpr uint32_t SM_STG = SM_RED + 2 * 2 * TM * 4;      // epilogue transpose: [8 warps][32 rows][32 cols] fp32, 16-byte groups XOR-swizzled by row
-constexpr uint32_t SM_TOTAL = SM_STG + 8 * 32 * 32 * 4;
+constexpr uint32_t SM_TOTAL = SM_BARS + 64;
 static_assert(SM_TOTAL <= 232448, "shared memory budget");
 constexpr uint32_t A_SBO = (CBG_H / 8) * 128, B_SBO = (KC / 8) * 128, LBO = 128;
-constexpr uint32_t TMEM_COLS = 512;
-constexpr uint32_t IDESC = idesc_f16(128);
 constexpr float kScaleA = 16.f;                // h (and the LayerNorm'ed q hidden) in the A tiles
 constexpr float kInvAcc = 1.f / 4096.f;        // weights are scaled by 256 (packer): accumulator at 2^12
 
@@ -94,7 +88,12 @@ __device__ __forceinline__ void stamp(long long* trace, int slot) {
   }
 }
 
-__global__ void __launch_bounds__(320, 1) node_gemm_f16_kernel(const __grid_constant__ NodeGemmArgs p) {
+__device__ __forceinline__ float quad_sum(float v) {
+  v += __shfl_xor_sync(CBG_FULL, v, 1);
+  return v + __shfl_xor_sync(CBG_FULL, v, 2);
+}
+
+__global__ void __launch_bounds__(288, 1) node_gemm_f16_kernel(const __grid_constant__ NodeGemmArgs p) {
   extern __shared__ __align__(1024) uint8_t smem[];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   int n_rows = p.n_rows;
@@ -108,27 +107,19 @@ __global__ void __launch_bounds__(320, 1) node_gemm_f16_kernel(const __grid_cons
   if (sc.n_gemm == 0) return;
   const uint32_t sbase = smem_u32(smem);
   const uint32_t bar_full = sbase + SM_BARS;                  // [STAGES]
-  const uint32_t bar_empty = bar_full + 8 * STAGES;           // [STAGES]
-  const uint32_t bar_acc_full = bar_empty + 8 * STAGES;       // [NACC]
-  const uint32_t bar_acc_free = bar_acc_full + 8 * NACC;      // [NACC]
-  const uint32_t bar_a_ready = bar_acc_free + 8 * NACC;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + SM_BARS + 8 * (2 * STAGES + 2 * NACC + 2));
+  const uint32_t bar_empty = bar_full + 8 * STAGES;           // [STAGES]: one arrival per consumer warpgroup
   const int total_chunks = sc.n_gemm * NKC;
   if (tid == 0) stamp(p.trace, 0);
 
-  if (warp == 0) tmem_alloc(smem_u32(tmem_slot), TMEM_COLS);
-  if (tid == 288) {
+  if (tid == 256) {
     // barriers + the first weight chunks: nothing here depends on the A tile, so the copies fly during its staging
-    for (int s = 0; s < STAGES; ++s) { mbar_init(bar_full + 8 * s, 1); mbar_init(bar_empty + 8 * s, 1); }
-    for (int b = 0; b < NACC; ++b) { mbar_init(bar_acc_full + 8 * b, 1); mbar_init(bar_acc_free + 8 * b, 8); }
-    mbar_init(bar_a_ready, 8);
+    for (int s = 0; s < STAGES; ++s) { mbar_init(bar_full + 8 * s, 1); mbar_init(bar_empty + 8 * s, 2); }
     fence_mbar_init();
     for (int i = 0; i < STAGES && i < total_chunks; ++i) {
       mbar_expect_tx(bar_full + 8 * i, B_STAGE);
       bulk_g2s(sbase + SM_B0 + i * B_STAGE, chunk_src(p, sc, i), B_STAGE, bar_full + 8 * i);
     }
   }
-
   if (warp < 8) {
     // A tile: rows of h -> (hi, lo) f16 tiles; lane <-> row keeps the 16-byte shared stores conflict free
     const int r = tid & (TM - 1);
@@ -136,26 +127,21 @@ __global__ void __launch_bounds__(320, 1) node_gemm_f16_kernel(const __grid_cons
     const bool live = row < n_rows;
     const float* arow = p.a + (size_t)(live ? (p.row_idx ? p.row_idx[row] : row) : 0) * CBG_H;
     const float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
-    {                                              // thread handles k8 = (tid >> 7) + 2 * j, j < 8: all 16 loads in flight
-      float4 v[16];
+    float4 v[16];                                  // thread handles k8 = (tid >> 7) + 2 * j, j < 8: all 16 loads in flight
 #pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const int k8 = (tid >> 7) + 2 * j;
-        v[2 * j] = live ? ldg4(arow + 8 * k8) : z;
-        v[2 * j + 1] = live ? ldg4(arow + 8 * k8 + 4) : z;
-      }
-#pragma unroll
-      for (int j = 0; j < 8; ++j) store_split8(smem + SM_A_HI, r, (tid >> 7) + 2 * j, v[2 * j], v[2 * j + 1]);
+    for (int j = 0; j < 8; ++j) {
+      const int k8 = (tid >> 7) + 2 * j;
+      v[2 * j] = live ? ldg4(arow + 8 * k8) : z;
+      v[2 * j + 1] = live ? ldg4(arow + 8 * k8 + 4) : z;
     }
+#pragma unroll
+    for (int j = 0; j < 8; ++j) store_split8(smem + SM_A_HI, r, (tid >> 7) + 2 * j, v[2 * j], v[2 * j + 1]);
     fence_proxy_async();
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
   if (tid == 0) stamp(p.trace, 1);
 
-  if (warp == 9) {
+  if (warp == 8) {
     // ===== weight-chunk producer (chunks 0 .. STAGES-1 are already in flight) =====
     if (lane == 0) {
       for (int i = STAGES; i < total_chunks; ++i) {
@@ -165,142 +151,105 @@ __global__ void __launch_bounds__(320, 1) node_gemm_f16_kernel(const __grid_cons
         bulk_g2s(sbase + SM_B0 + s * B_STAGE, chunk_src(p, sc, i), B_STAGE, bar_full + 8 * s);
       }
     }
-  } else if (warp == 8) {
-    // ===== MMA issuer =====
-    if (lane == 0) {
-      for (int g = 0; g < sc.n_gemm; ++g) {
-        const int buf = g & (NACC - 1);
-        const bool q2 = sc.kind(g) == 2;
-        if (g >= NACC) mbar_wait(bar_acc_free + 8 * buf, (uint32_t)(((g / NACC) - 1) & 1));   // epilogue drained this accumulator
-        if (q2) mbar_wait(bar_a_ready, 0u);                                                  // relu(LN(q hidden)) is staged
-        tc_fence_after();
-        const uint32_t a_base = sbase + (q2 ? SM_Q : SM_A_HI);
-        const uint64_t da_hi = smem_desc(a_base, LBO, A_SBO), da_lo = smem_desc(a_base + A_TILE, LBO, A_SBO);
-        const uint32_t d_tmem = tmem + (uint32_t)(buf * 128);
+    return;
+  }
+  // ===== consumer warpgroups: MMAs and epilogue of rows 64 wg .. 64 wg + 63 =====
+  const int wg = warp >> 2, qg = lane >> 2, qt = lane & 3;
+  const int r_lo = 64 * wg + 16 * (warp & 3) + qg;            // this thread's accumulator rows: r_lo and r_lo + 8
+  int node[2];
 #pragma unroll
-        for (int c = 0; c < NKC; ++c) {
-          const int i = g * NKC + c, s = i % STAGES;
-          mbar_wait(bar_full + 8 * s, (uint32_t)((i / STAGES) & 1));
-          tc_fence_after();
-          const uint64_t db_hi = smem_desc(sbase + SM_B0 + s * B_STAGE, LBO, B_SBO);
-          const uint64_t db_lo = smem_desc(sbase + SM_B0 + s * B_STAGE + B_CHUNK, LBO, B_SBO);
+  for (int h = 0; h < 2; ++h) {
+    const int grow = row0 + r_lo + 8 * h;
+    node[h] = (grow < n_rows) ? (p.row_idx ? p.row_idx[grow] : grow) : -1;
+  }
+  for (int g = 0; g < sc.n_gemm; ++g) {
+    const int kind = sc.kind(g), rel = sc.rel(p, g);
+    const uint32_t a_base = sbase + (kind == 2 ? SM_Q : SM_A_HI) + (uint32_t)(8 * wg) * A_SBO;
+    const uint64_t da_hi = smem_desc(a_base, LBO, A_SBO), da_lo = smem_desc(a_base + A_TILE, LBO, A_SBO);
+    float d[64];
 #pragma unroll
-          for (int ks = 0; ks < KC / 16; ++ks) {
-            const uint64_t ka = (uint64_t)(16 * (c * (KC / 16) + ks)), kb = (uint64_t)(16 * ks);   // 256 bytes per K step
-            umma_f16_ss(d_tmem, da_lo + ka, db_hi + kb, IDESC, (c == 0 && ks == 0) ? 0u : 1u);    // small terms first
-            umma_f16_ss(d_tmem, da_hi + ka, db_lo + kb, IDESC, 1u);
-            umma_f16_ss(d_tmem, da_hi + ka, db_hi + kb, IDESC, 1u);
-          }
-          umma_commit(bar_empty + 8 * s);
-        }
-        umma_commit(bar_acc_full + 8 * buf);
+    for (int c = 0; c < NKC; ++c) {
+      const int i = g * NKC + c, s = i % STAGES;
+      mbar_wait(bar_full + 8 * s, (uint32_t)((i / STAGES) & 1));
+      const uint64_t db_hi = smem_desc(sbase + SM_B0 + s * B_STAGE, LBO, B_SBO);
+      const uint64_t db_lo = smem_desc(sbase + SM_B0 + s * B_STAGE + B_CHUNK, LBO, B_SBO);
+      wgmma_fence();
+#pragma unroll
+      for (int ks = 0; ks < KC / 16; ++ks) {
+        const uint64_t ka = (uint64_t)(16 * (c * (KC / 16) + ks)), kb = (uint64_t)(16 * ks);   // 256 bytes per K step
+        wgmma_f16_ss(d, da_lo + ka, db_hi + kb, (c == 0 && ks == 0) ? 0u : 1u);                // small terms first
+        wgmma_f16_ss(d, da_hi + ka, db_lo + kb, 1u);
+        wgmma_f16_ss(d, da_hi + ka, db_hi + kb, 1u);
       }
+      wgmma_commit();
+      wgmma_wait0();
+      if ((tid & 127) == 0) mbar_arrive(bar_empty + 8 * s);      // this warpgroup is done with the ring stage
     }
-  } else {
-    // ===== epilogue warps: thread = (row, 64-column half) =====
-    const int q4 = warp & 3, chalf = warp >> 2;
-    const int my_row = 32 * q4 + lane;
-    const int grow = row0 + my_row;
-    const int node = (grow < n_rows) ? (p.row_idx ? p.row_idx[grow] : grow) : -1;
-    float* red = reinterpret_cast<float*>(smem + SM_RED);
-    float* stg = reinterpret_cast<float*>(smem + SM_STG) + warp * (32 * 32);
-    // store phase of the transpose: lane = (row lane / 8 + 4 i, 16-byte column group lane % 8)
-    const int c4s = lane & 7;
-    int node_s[8];
+    wgmma_settle(d);
+    if (tid == 0) stamp(p.trace, 2 + g);
+    if (kind != 1) {
+      const float* bias = kind == 2 ? p.q_b1 : p.bias + rel * CBG_H;
+      float* out = kind == 2 ? p.out_q : p.out[rel];
+      // destination planes / q of a merged launch stop at n_dst
+      const bool dst_plane = kind == 2 || p.tc_first_plane + rel >= CBG_NODE_SRC_PLANES;
+      const int row_lim = dst_plane ? n_dst : n_rows;      // rows of this tile that exist for this plane
 #pragma unroll
-    for (int i = 0; i < 8; ++i) node_s[i] = __shfl_sync(CBG_FULL, node, (lane >> 3) + 4 * i);
-    for (int g = 0; g < sc.n_gemm; ++g) {
-      const int buf = g & (NACC - 1);
-      const int kind = sc.kind(g), rel = sc.rel(p, g);
-      mbar_wait(bar_acc_full + 8 * buf, (uint32_t)((g / NACC) & 1));
-      tc_fence_after();
-      if (warp == 0 && lane == 0) stamp(p.trace, 2 + g);
-      const uint32_t t_lane = tmem + ((uint32_t)(32 * q4) << 16) + (uint32_t)(buf * 128 + chalf * 64);
-      uint32_t ra[32], rb[32];
-      tmem_ld32_nowait(t_lane, ra);
-      tmem_ld32_nowait(t_lane + 32u, rb);
-      tmem_wait_ld();
-#define RR(i) __uint_as_float((i) < 32 ? ra[(i) & 31] : rb[(i) & 31])
-      if (kind != 1) {
-        const float* bias = (kind == 2 ? p.q_b1 : p.bias + rel * CBG_H) + chalf * 64;
-        float* out = kind == 2 ? p.out_q : p.out[rel];
-        // destination planes / q of a merged launch stop at n_dst
-        const bool dst_plane = kind == 2 || p.tc_first_plane + rel >= CBG_NODE_SRC_PLANES;
-        const int row_lim = dst_plane ? n_dst : n_rows;      // rows of this tile that exist for this plane
-#pragma unroll
-        for (int piece = 0; piece < 2; ++piece) {             // 32 columns at a time through the warp's staging tile
-#pragma unroll
-          for (int c4 = 0; c4 < 8; ++c4) {
-            const int j = 8 * piece + c4;
-            const float4 b = ldg4(bias + 4 * j);
-            *reinterpret_cast<float4*>(stg + lane * 32 + ((c4 ^ (lane & 7)) << 2)) =
-                make_float4(fmaf(RR(4 * j), kInvAcc, b.x), fmaf(RR(4 * j + 1), kInvAcc, b.y),
-                            fmaf(RR(4 * j + 2), kInvAcc, b.z), fmaf(RR(4 * j + 3), kInvAcc, b.w));
-          }
-          __syncwarp();
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const int rr = (lane >> 3) + 4 * i;
-            const float4 v = *reinterpret_cast<const float4*>(stg + rr * 32 + ((c4s ^ (rr & 7)) << 2));
-            if (node_s[i] >= 0 && row0 + 32 * q4 + rr < row_lim)
-              st4(out + (size_t)node_s[i] * CBG_H + chalf * 64 + piece * 32 + 4 * c4s, v);
-          }
-          __syncwarp();
-        }
-      } else {
-        // q hidden: + bias, LayerNorm over the row (two halves meet through shared memory; mean first, then the squared
-        // deviations), ReLU, (hi, lo) split into the A tile of the second Linear
-        const float* bias = p.bias + rel * CBG_H + chalf * 64;
-        float v[64];
-        float s = 0.f;
+      for (int h = 0; h < 2; ++h) {
+        if (node[h] < 0 || row0 + r_lo + 8 * h >= row_lim) continue;
+        float* o = out + (size_t)node[h] * CBG_H + 2 * qt;
 #pragma unroll
         for (int j = 0; j < 16; ++j) {
-          const float4 b = ldg4(bias + 4 * j);
-          v[4 * j] = fmaf(RR(4 * j), kInvAcc, b.x);
-          v[4 * j + 1] = fmaf(RR(4 * j + 1), kInvAcc, b.y);
-          v[4 * j + 2] = fmaf(RR(4 * j + 2), kInvAcc, b.z);
-          v[4 * j + 3] = fmaf(RR(4 * j + 3), kInvAcc, b.w);
-          s += (v[4 * j] + v[4 * j + 1]) + (v[4 * j + 2] + v[4 * j + 3]);
+          const float2 b = __ldg(reinterpret_cast<const float2*>(bias + 8 * j + 2 * qt));
+          *reinterpret_cast<float2*>(o + 8 * j) = make_float2(fmaf(d[4 * j + 2 * h], kInvAcc, b.x), fmaf(d[4 * j + 2 * h + 1], kInvAcc, b.y));
         }
-        red[chalf * TM + my_row] = s;
-        asm volatile("bar.sync %0, 64;" ::"r"(1 + q4) : "memory");
-        const float mean = (red[my_row] + red[TM + my_row]) * (1.f / 128.f);
-        float q = 0.f;
-#pragma unroll
-        for (int j = 0; j < 64; ++j) { v[j] -= mean; q = fmaf(v[j], v[j], q); }
-        red[2 * TM + chalf * TM + my_row] = q;
-        asm volatile("bar.sync %0, 64;" ::"r"(1 + q4) : "memory");
-        const float rstd = 1.f / sqrtf((red[2 * TM + my_row] + red[3 * TM + my_row]) * (1.f / 128.f) + 1e-5f);
-        const float* gam = p.q_ln + chalf * 64;
-        const float* bet = p.q_ln + 128 + chalf * 64;
-#pragma unroll
-        for (int k8 = 0; k8 < 8; ++k8) {
-          float a[8];
-#pragma unroll
-          for (int e = 0; e < 8; e += 4) {
-            const float4 gm = ldg4(gam + 8 * k8 + e), bt = ldg4(bet + 8 * k8 + e);
-            a[e] = fmaxf(fmaf(v[8 * k8 + e] * rstd, gm.x, bt.x), 0.f);
-            a[e + 1] = fmaxf(fmaf(v[8 * k8 + e + 1] * rstd, gm.y, bt.y), 0.f);
-            a[e + 2] = fmaxf(fmaf(v[8 * k8 + e + 2] * rstd, gm.z, bt.z), 0.f);
-            a[e + 3] = fmaxf(fmaf(v[8 * k8 + e + 3] * rstd, gm.w, bt.w), 0.f);
-          }
-          store_split8(smem + SM_Q, my_row, chalf * 8 + k8, make_float4(a[0], a[1], a[2], a[3]), make_float4(a[4], a[5], a[6], a[7]));
-        }
-        fence_proxy_async();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(bar_a_ready);
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_acc_free + 8 * buf);
-      if (warp == 0 && lane == 0) stamp(p.trace, 10 + g);
-#undef RR
+    } else {
+      // q hidden: + bias, LayerNorm over the row (a row's 128 columns live in the 4 lanes of a quad; mean first, then
+      // the squared deviations), ReLU, (hi, lo) split into the A tile of the second Linear
+      const float* bias = p.bias + rel * CBG_H;
+      float s0 = 0.f, s1 = 0.f;
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        const float2 b = __ldg(reinterpret_cast<const float2*>(bias + 8 * j + 2 * qt));
+        d[4 * j] = fmaf(d[4 * j], kInvAcc, b.x);
+        d[4 * j + 1] = fmaf(d[4 * j + 1], kInvAcc, b.y);
+        d[4 * j + 2] = fmaf(d[4 * j + 2], kInvAcc, b.x);
+        d[4 * j + 3] = fmaf(d[4 * j + 3], kInvAcc, b.y);
+        s0 += d[4 * j] + d[4 * j + 1];
+        s1 += d[4 * j + 2] + d[4 * j + 3];
+      }
+      const float mean0 = quad_sum(s0) * (1.f / 128.f), mean1 = quad_sum(s1) * (1.f / 128.f);
+      float q0 = 0.f, q1 = 0.f;
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        d[4 * j] -= mean0; d[4 * j + 1] -= mean0; d[4 * j + 2] -= mean1; d[4 * j + 3] -= mean1;
+        q0 = fmaf(d[4 * j], d[4 * j], q0); q0 = fmaf(d[4 * j + 1], d[4 * j + 1], q0);
+        q1 = fmaf(d[4 * j + 2], d[4 * j + 2], q1); q1 = fmaf(d[4 * j + 3], d[4 * j + 3], q1);
+      }
+      const float rstd0 = 1.f / sqrtf(quad_sum(q0) * (1.f / 128.f) + 1e-5f);
+      const float rstd1 = 1.f / sqrtf(quad_sum(q1) * (1.f / 128.f) + 1e-5f);
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        const float2 gm = __ldg(reinterpret_cast<const float2*>(p.q_ln + 8 * j + 2 * qt));
+        const float2 bt = __ldg(reinterpret_cast<const float2*>(p.q_ln + 128 + 8 * j + 2 * qt));
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const float rs = h ? rstd1 : rstd0;
+          const float a0 = fmaxf(fmaf(d[4 * j + 2 * h] * rs, gm.x, bt.x), 0.f);
+          const float a1 = fmaxf(fmaf(d[4 * j + 2 * h + 1] * rs, gm.y, bt.y), 0.f);
+          uint32_t hi, lo;
+          split_pair(a0 * kScaleA, a1 * kScaleA, hi, lo);
+          const uint32_t off = a_off8(r_lo + 8 * h, j) + 4u * (uint32_t)qt;
+          *reinterpret_cast<uint32_t*>(smem + SM_Q + off) = hi;
+          *reinterpret_cast<uint32_t*>(smem + SM_Q + A_TILE + off) = lo;
+        }
+      }
+      fence_proxy_async();
+      warpgroup_sync(wg);      // the second Linear of this warpgroup reads exactly the rows it has just written
     }
+    if (tid == 0) stamp(p.trace, 10 + g);
   }
-  tc_fence_before();
-  __syncthreads();
   if (tid == 0) stamp(p.trace, 20);
-  if (warp == 0) tmem_dealloc(tmem, TMEM_COLS);
 }
 
 }  // namespace
@@ -320,7 +269,7 @@ int cbg_launch_node_gemm_f16(const NodeGemmArgs& a, cudaStream_t st) {
   NodeGemmArgs args = a;
   args.trace = g_trace_buf;
   CBG_PROF_BEGIN(CBG_K_NODE_GEMM, st);
-  node_gemm_f16_kernel<<<(a.n_rows + TM - 1) / TM, 320, SM_TOTAL, st>>>(args);
+  node_gemm_f16_kernel<<<(a.n_rows + TM - 1) / TM, 288, SM_TOTAL, st>>>(args);
   CBG_LAUNCHED(CBG_K_NODE_GEMM, st);
   return 0;
 }

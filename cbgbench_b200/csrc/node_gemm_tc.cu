@@ -1,122 +1,43 @@
-// Node-level projections on the 5th-generation tensor cores (tcgen05 / UMMA, sm_100a).
+// Node-level projections on the Hopper tensor cores (wgmma, sm_90a) in 3xTF32.
 //
 // Same contract as node_gemm.cu (planes Pj_k, Pj_v, Pi_k, Pi_v, q of one attention sub-layer;
 // reference: x2h_attention.py:58-83, h2x_attention.py:42-62, common.py:151-171), but the
-// [rows,128] x [128,128] products run as tcgen05.mma kind::tf32 with the 3xTF32 error-compensated
+// [rows,128] x [128,128] products run as wgmma m64n128k8 tf32 with the 3xTF32 error-compensated
 // split  a*b ~= a_hi*b_hi + a_hi*b_lo + a_lo*b_hi  (a_hi = rna_tf32(a), a_lo = rna_tf32(a - a_hi)),
-// fp32 accumulation in TMEM => fp32-class accuracy (needed for the 1e-4 parity bar; single-pass
+// fp32 accumulation in registers => fp32-class accuracy (needed for the 1e-4 parity bar; single-pass
 // TF32 is ~1e-3 after 9 residual layers, SURVEY.md section 7 hard part 1).
 //
-// One CTA = one 128-row tile.  A (rows of h) is converted once per CTA into hi/lo tf32 tiles in
-// shared memory in the UMMA canonical K-major SWIZZLE_NONE layout (8x16B core matrices);
+// One CTA = one 128-row tile = two consumer warpgroups of 64 rows + a copy warp.  A (rows of h) is converted once
+// per CTA into hi/lo tf32 tiles in shared memory in the canonical K-major no-swizzle layout (8 x 16 B core matrices);
 // B (the weight plane) is pre-split and pre-laid-out on the host (packer) so a plain 1-D bulk
-// async copy (cp.async.bulk + mbarrier complete_tx) stages each 32 KB K-chunk into a 3-stage ring
-// (optionally multicast across a thread-block cluster of row tiles).  One thread issues copies and MMAs,
-// tcgen05.commit signals the mbarriers, all 8 warps drain the 128x128 fp32 accumulator from TMEM
-// (tcgen05.ld 32x32b) for the epilogue (+bias -> global, or LayerNorm+ReLU -> A tiles for the
-// second Linear of the q MLP).
-#include <stdlib.h>
+// async copy (cp.async.bulk + mbarrier complete_tx) stages each 32 KB K-chunk into a 3-stage ring,
+// optionally multicast across a thread-block cluster of CL row tiles: every CTA copies 1/CL of a chunk into all CL
+// shared memories, and a ring stage is refilled once the consumers of all CL CTAs have released it.
+// Each warpgroup keeps the 64 x 128 fp32 accumulator in registers for the epilogue (+bias -> global, or
+// LayerNorm+ReLU -> A tiles for the second Linear of the q MLP).
 #include "cbg_kernels.cuh"
+#include "cbg_tc.cuh"
+
+using namespace cbg_tc;
 
 namespace {
 
-constexpr int TM = 128;                        // rows per CTA (UMMA M)
+constexpr int TM = 128;                        // rows per CTA (2 x wgmma M)
 constexpr int KC = 32;                         // K elements per weight chunk
 constexpr int NKC = CBG_H / KC;                // 4 chunks per plane
-constexpr int MAX_STAGE = 3;                   // weight-chunk ring depth is a template parameter (2 or 3)
+constexpr int NSTAGE = 3;                      // weight-chunk ring depth
 constexpr uint32_t A_TILE_BYTES = TM * CBG_H * 4;          // 64 KB per (hi | lo)
 constexpr uint32_t B_CHUNK_BYTES = 128 * KC * 4;           // 16 KB per (hi | lo)
 constexpr uint32_t B_STAGE_BYTES = 2 * B_CHUNK_BYTES;      // hi + lo, contiguous in the blob
 constexpr uint32_t SMEM_A_HI = 0;
 constexpr uint32_t SMEM_A_LO = A_TILE_BYTES;
 constexpr uint32_t SMEM_B0 = 2 * A_TILE_BYTES;
-constexpr uint32_t smem_total(int nstage) { return SMEM_B0 + nstage * B_STAGE_BYTES + 128; }  // + mbarriers, tmem slot
+constexpr uint32_t SMEM_BAR = SMEM_B0 + NSTAGE * B_STAGE_BYTES;
+constexpr uint32_t SMEM_TOTAL = SMEM_BAR + 64;
+static_assert(SMEM_TOTAL <= 232448, "shared memory budget");
 constexpr uint32_t A_SBO = (CBG_H / 4) * 128;   // byte stride between 8-row groups of an A tile
 constexpr uint32_t B_SBO = (KC / 4) * 128;      // same for a B chunk
 constexpr uint32_t LBO = 128;                   // byte stride between core matrices along K
-constexpr uint32_t TMEM_COLS = 128;
-
-// instruction descriptor: D=f32, A=B=tf32, K-major both, N=128, M=128 (cute::UMMA::InstrDescriptor)
-constexpr uint32_t IDESC = (1u << 4) | (2u << 7) | (2u << 10) | ((128u >> 3) << 17) | ((128u >> 4) << 24);
-
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t sbo_bytes) {
-  // cute::UMMA::SmemDescriptor: start>>4 [0,14) | LBO>>4 [16,30) | SBO>>4 [32,46) | version=1 [46,48) | layout NONE
-  return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)(LBO >> 4) << 16) | ((uint64_t)(sbo_bytes >> 4) << 32) |
-         (1ull << 46);
-}
-
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  uint32_t done = 0, spins = 0;
-  while (!done) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(done)
-        : "r"(bar), "r"(parity)
-        : "memory");
-    if (!done && ++spins > (1u << 24)) __trap();   // never hang the GPU: fail loudly instead
-  }
-}
-__device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst),
-               "l"(src), "r"(bytes), "r"(bar)
-               : "memory");
-}
-// each CTA of a cluster copies its 1/CL slice of the chunk into the same offset of EVERY CTA's smem
-__device__ __forceinline__ void bulk_g2s_mcast(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar, uint16_t mask) {
-  asm volatile(
-      "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1], %2, [%3], %4;" ::"r"(dst),
-      "l"(src), "r"(bytes), "r"(bar), "h"(mask)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit_mcast(uint32_t bar, uint16_t mask) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar),
-               "h"(mask)
-               : "memory");
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ uint32_t cluster_rank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void umma_tf32(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(IDESC), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float (&v)[32]) {
-  uint32_t r[32];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
-}
 
 __device__ __forceinline__ float to_tf32(float x) {
   uint32_t r;
@@ -134,10 +55,11 @@ __device__ __forceinline__ void store_split(uint8_t* smem, int row, int k4, floa
   *reinterpret_cast<float4*>(smem + SMEM_A_HI + off) = hi;
   *reinterpret_cast<float4*>(smem + SMEM_A_LO + off) = lo;
 }
+__device__ __forceinline__ float quad_sum(float v) {
+  v += __shfl_xor_sync(CBG_FULL, v, 1);
+  return v + __shfl_xor_sync(CBG_FULL, v, 2);
+}
 
-// CL = CTAs per cluster sharing every weight chunk through multicast bulk copies (1 = no cluster).
-// The kernel is bound by L2->SM weight traffic (every CTA needs all 6 x 128 KB of weight images), so a
-// cluster of CL row tiles cuts that traffic by CL.
 // weight chunk i lives at: plane(i / NKC) -> tc plane index, chunk (i % NKC)
 __device__ __forceinline__ const float* chunk_src_ptr(const NodeGemmArgs& p, int i) {
   const int g = i / NKC, c = i % NKC;
@@ -145,9 +67,10 @@ __device__ __forceinline__ const float* chunk_src_ptr(const NodeGemmArgs& p, int
   return p.tc_planes + (size_t)plane * (NKC * 2 * 128 * KC) + (size_t)c * (2 * 128 * KC);
 }
 
-template <int CL, int NSTAGE>
-__global__ void __launch_bounds__(256, 1) node_gemm_tc_kernel(NodeGemmArgs p) {
-  constexpr uint32_t SMEM_BAR = SMEM_B0 + NSTAGE * B_STAGE_BYTES;
+// CL = CTAs per cluster sharing every weight chunk through multicast bulk copies (1 = no cluster).
+// Every CTA needs all 6 x 128 KB of weight images, so a cluster of CL row tiles cuts the L2 -> SM weight traffic by CL.
+template <int CL>
+__global__ void __launch_bounds__(288, 1) node_gemm_tc_kernel(NodeGemmArgs p) {
   constexpr uint16_t kMask = (uint16_t)((1u << CL) - 1u);
   const uint32_t crank = (CL > 1) ? cluster_rank() : 0u;
   if (p.n_rows_dev) {                 // list length lives on the device (receptive-field pruning)
@@ -160,22 +83,14 @@ __global__ void __launch_bounds__(256, 1) node_gemm_tc_kernel(NodeGemmArgs p) {
   const int row0 = blockIdx.x * TM;
   const uint32_t sbase = smem_u32(smem);
   const uint32_t bar_full = sbase + SMEM_BAR;                 // [NSTAGE]
-  const uint32_t bar_empty = bar_full + 8 * NSTAGE;           // [NSTAGE]
-  const uint32_t bar_acc = bar_empty + 8 * NSTAGE;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + SMEM_BAR + 8 * (2 * NSTAGE + 1));
+  const uint32_t bar_empty = bar_full + 8 * NSTAGE;           // [NSTAGE]: one arrival per consumer warpgroup of every CTA
 
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)),
-                 "r"(TMEM_COLS));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
+  if (tid == 256) {
+    for (int s = 0; s < NSTAGE; ++s) { mbar_init(bar_full + 8 * s, 1); mbar_init(bar_empty + 8 * s, 2 * CL); }
+    fence_mbar_init();
   }
-  if (tid == 32) {
-    for (int s = 0; s < NSTAGE; ++s) { mbar_init(bar_full + 8 * s, 1); mbar_init(bar_empty + 8 * s, CL); }
-    mbar_init(bar_acc, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  // A tile: rows of h -> (hi, lo) tf32 tiles; lanes <-> rows keeps the 16 B shared stores conflict free
-  {
+  if (warp < 8) {
+    // A tile: rows of h -> (hi, lo) tf32 tiles; lanes <-> rows keeps the 16 B shared stores conflict free
     const int r = tid & (TM - 1);
     const int row = row0 + r;
     const bool live = row < p.n_rows;
@@ -189,359 +104,139 @@ __global__ void __launch_bounds__(256, 1) node_gemm_tc_kernel(NodeGemmArgs p) {
 #pragma unroll
       for (int j = 0; j < 8; ++j) store_split(smem, r, (tid >> 7) + 2 * (it + j), v[j]);
     }
+    fence_proxy_async();
   }
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  if (CL > 1) cluster_sync_all();      // every CTA's barriers exist before any peer copy / commit targets them
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem = *tmem_slot;
-  // stage the weight chunk `i` into ring slot `slot`: own slice only when clustered
-  auto load_chunk = [&](int i, int slot) {
-    const uint32_t bf = bar_full + 8 * slot;
-    mbar_expect_tx(bf, B_STAGE_BYTES);                       // the whole chunk lands here (all slices)
-    if (CL > 1) {
-      constexpr uint32_t slice = B_STAGE_BYTES / CL;
-      bulk_g2s_mcast(sbase + SMEM_B0 + slot * B_STAGE_BYTES + crank * slice,
-                     reinterpret_cast<const char*>(chunk_src_ptr(p, i)) + crank * slice, slice, bf, kMask);
-    } else {
-      bulk_g2s(sbase + SMEM_B0 + slot * B_STAGE_BYTES, chunk_src_ptr(p, i), B_STAGE_BYTES, bf);
-    }
-  };
+  if (CL > 1) cluster_sync_all();      // every CTA's barriers exist before any peer copy / arrive targets them
 
   const int n_gemm = p.n_planes + (p.has_q ? 1 : 0);      // + the second Linear of the q MLP
   const int total_chunks = n_gemm * NKC;
-  if (tid == 0) {
-    for (int i = 0; i < NSTAGE && i < total_chunks; ++i) load_chunk(i, i);
-  }
 
-  // destination node ids for the epilogue: this thread's accumulator row
-  const int q4 = warp & 3, chalf = warp >> 2;
-  const int my_row = 32 * q4 + lane;
-  const int grow = row0 + my_row;
-  const int dst = (grow < p.n_rows) ? (p.row_idx ? p.row_idx[grow] : grow) : -1;
-  const uint32_t t_lane = tmem + ((uint32_t)(32 * q4) << 16);
-
-  for (int g = 0; g < n_gemm; ++g) {
-    if (tid == 0) {
-      for (int c = 0; c < NKC; ++c) {
-        const int i = g * NKC + c, s = i % NSTAGE;
-        mbar_wait(bar_full + 8 * s, (uint32_t)((i / NSTAGE) & 1));
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t b_hi = sbase + SMEM_B0 + s * B_STAGE_BYTES, b_lo = b_hi + B_CHUNK_BYTES;
-#pragma unroll
-        for (int ks = 0; ks < KC / 8; ++ks) {
-          const uint32_t koff_a = (uint32_t)(c * (KC / 4) + ks * 2) * 128u;   // 2 core matrices per K=8 step
-          const uint32_t koff_b = (uint32_t)(ks * 2) * 128u;
-          const uint64_t a_hi = make_desc(sbase + SMEM_A_HI + koff_a, A_SBO);
-          const uint64_t a_lo = make_desc(sbase + SMEM_A_LO + koff_a, A_SBO);
-          const uint64_t d_bhi = make_desc(b_hi + koff_b, B_SBO);
-          const uint64_t d_blo = make_desc(b_lo + koff_b, B_SBO);
-          const uint32_t first = (c == 0 && ks == 0) ? 0u : 1u;
-          umma_tf32(tmem, a_lo, d_bhi, first);      // small terms first
-          umma_tf32(tmem, a_hi, d_blo, 1u);
-          umma_tf32(tmem, a_hi, d_bhi, 1u);
-        }
-        if (CL > 1) umma_commit_mcast(bar_empty + 8 * s, kMask);   // every peer learns this CTA is done with the slot
-        else umma_commit(bar_empty + 8 * s);        // stage reusable when these MMAs retire
-        if (c == NKC - 1) umma_commit(bar_acc);     // accumulator of this plane complete
-        // refill the stage of the PREVIOUS chunk (its MMAs retire before the ones just issued start),
-        // so the issuing thread never waits on the chunk it just queued
-        const int prev = i - 1, nxt = prev + NSTAGE;
-        if (prev >= 0 && nxt < total_chunks) {
-          const int ps = prev % NSTAGE;
-          mbar_wait(bar_empty + 8 * ps, (uint32_t)((prev / NSTAGE) & 1));   // all CL CTAs retired chunk prev
-          load_chunk(nxt, ps);
-        }
-      }
-    }
-    // ---- epilogue of GEMM g (all threads) -------------------------------------------------------
-    mbar_wait(bar_acc, (uint32_t)(g & 1));
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const bool is_qhid = p.has_q && (g == p.n_planes - 1);
-    const bool is_q2 = p.has_q && (g == p.n_planes);
-    if (!is_qhid) {
-      const float* bias = is_q2 ? p.q_b1 : (p.bias + g * CBG_H);
-      float* out = is_q2 ? p.out_q : p.out[g];
-#pragma unroll 1
-      for (int cb = 0; cb < 2; ++cb) {
-        const int col0 = chalf * 64 + cb * 32;
-        float v[32];
-        tmem_ld32(t_lane + (uint32_t)col0, v);
-        if (dst >= 0) {
-          float* o = out + (size_t)dst * CBG_H + col0;
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            const float4 b = ldg4(bias + col0 + 4 * j);
-            st4(o + 4 * j, make_float4(v[4 * j] + b.x, v[4 * j + 1] + b.y, v[4 * j + 2] + b.z, v[4 * j + 3] + b.w));
-          }
-        }
-      }
-    } else if (chalf == 0) {
-      // q hidden: + bias, LayerNorm(128) + ReLU per row (thread-local: one thread owns one row),
-      // then back into the A tiles as the operand of the second Linear
-      float v[128];
-#pragma unroll
-      for (int cb = 0; cb < 4; ++cb) {
-        float t[32];
-        tmem_ld32(t_lane + (uint32_t)(cb * 32), t);
-#pragma unroll
-        for (int j = 0; j < 32; ++j) v[cb * 32 + j] = t[j] + __ldg(p.bias + g * CBG_H + cb * 32 + j);
-      }
-      float s = 0.f;
-#pragma unroll
-      for (int j = 0; j < 128; ++j) s += v[j];
-      const float mean = s * (1.f / 128.f);
-      float q = 0.f;
-#pragma unroll
-      for (int j = 0; j < 128; ++j) { v[j] -= mean; q = fmaf(v[j], v[j], q); }
-      const float rstd = 1.f / sqrtf(q * (1.f / 128.f) + 1e-5f);
-#pragma unroll
-      for (int k4 = 0; k4 < 32; ++k4) {
-        const float4 ga = ldg4(p.q_ln + 4 * k4), be = ldg4(p.q_ln + 128 + 4 * k4);
-        float4 a;
-        a.x = fmaxf(fmaf(v[4 * k4 + 0] * rstd, ga.x, be.x), 0.f);
-        a.y = fmaxf(fmaf(v[4 * k4 + 1] * rstd, ga.y, be.y), 0.f);
-        a.z = fmaxf(fmaf(v[4 * k4 + 2] * rstd, ga.z, be.z), 0.f);
-        a.w = fmaxf(fmaf(v[4 * k4 + 3] * rstd, ga.w, be.w), 0.f);
-        store_split(smem, my_row, k4, a);
-      }
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();      // TMEM drained (and A rewritten for the q path) before the next plane's MMAs
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  }
-  if (CL > 1) cluster_sync_all();      // no CTA may exit while peers can still write its smem / signal its barriers
-  if (warp == 0) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(TMEM_COLS));
-  }
-}
-
-
-
-// ------------------------------------------------------------------------------------------------
-// Warp-specialised variant (default): 8 staging/epilogue warps + a weight-copy thread + an MMA-issuing
-// thread, two TMEM accumulators.  The copy thread runs ahead through the 3-stage weight ring, the MMA
-// thread streams the planes back to back (plane g+1 accumulates while the epilogue warps drain plane
-// g), the epilogue warps never wait on copies.  mbarriers: full/empty per ring stage, acc_full/acc_free
-// per accumulator, a_ready for the LayerNorm'ed operand of the q MLP's second Linear.
-constexpr int WS_STAGES = 3;
-constexpr uint32_t WS_SMEM_BAR = SMEM_B0 + WS_STAGES * B_STAGE_BYTES;
-constexpr uint32_t WS_SMEM_TOTAL = WS_SMEM_BAR + 128;
-constexpr uint32_t WS_TMEM_COLS = 256;
-
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-
-__global__ void __launch_bounds__(320, 1) node_gemm_ws_kernel(NodeGemmArgs p) {
-  extern __shared__ __align__(1024) uint8_t smem[];
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  if (p.n_rows_dev) {
-    const int nd = *p.n_rows_dev;
-    p.n_rows = nd < p.n_rows ? nd : p.n_rows;
-  }
-  const int row0 = blockIdx.x * TM;
-  if (row0 >= p.n_rows) return;
-  const uint32_t sbase = smem_u32(smem);
-  const uint32_t bar_full = sbase + WS_SMEM_BAR;              // [WS_STAGES]
-  const uint32_t bar_empty = bar_full + 8 * WS_STAGES;        // [WS_STAGES]
-  const uint32_t bar_acc_full = bar_empty + 8 * WS_STAGES;    // [2]
-  const uint32_t bar_acc_free = bar_acc_full + 16;            // [2]
-  const uint32_t bar_a_ready = bar_acc_free + 16;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + WS_SMEM_BAR + 8 * (2 * WS_STAGES + 5));
-
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)),
-                 "r"(WS_TMEM_COLS));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
-  if (tid == 32) {
-    for (int s = 0; s < WS_STAGES; ++s) { mbar_init(bar_full + 8 * s, 1); mbar_init(bar_empty + 8 * s, 1); }
-    for (int b = 0; b < 2; ++b) { mbar_init(bar_acc_full + 8 * b, 1); mbar_init(bar_acc_free + 8 * b, 8); }
-    mbar_init(bar_a_ready, 8);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  const int n_gemm = p.n_planes + (p.has_q ? 1 : 0);
-  const int total_chunks = n_gemm * NKC;
-
-  if (warp < 8) {
-    // A tile: rows of h -> (hi, lo) tf32 tiles; lanes <-> rows keeps the 16 B shared stores conflict free
-    const int r = tid & (TM - 1);
-    const int row = row0 + r;
-    const bool live = row < p.n_rows;
-    const float* arow = p.a + (size_t)(live ? (p.row_idx ? p.row_idx[row] : row) : 0) * CBG_H;
-#pragma unroll
-    for (int it = 0; it < 16; it += 8) {
-      float4 v[8];
-#pragma unroll
-      for (int j = 0; j < 8; ++j)
-        v[j] = live ? ldg4(arow + 4 * ((tid >> 7) + 2 * (it + j))) : make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-      for (int j = 0; j < 8; ++j) store_split(smem, r, (tid >> 7) + 2 * (it + j), v[j]);
-    }
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem = *tmem_slot;
-
-  if (warp == 9) {
-    // ===== weight-chunk producer =====
+  if (warp == 8) {
+    // ===== weight-chunk producer: own slice only when clustered =====
     if (lane == 0) {
       for (int i = 0; i < total_chunks; ++i) {
-        const int s = i % WS_STAGES;
-        if (i >= WS_STAGES) mbar_wait(bar_empty + 8 * s, (uint32_t)(((i / WS_STAGES) - 1) & 1));
-        mbar_expect_tx(bar_full + 8 * s, B_STAGE_BYTES);
-        bulk_g2s(sbase + SMEM_B0 + s * B_STAGE_BYTES, chunk_src_ptr(p, i), B_STAGE_BYTES, bar_full + 8 * s);
-      }
-    }
-  } else if (warp == 8) {
-    // ===== MMA issuer =====
-    if (lane == 0) {
-      for (int g = 0; g < n_gemm; ++g) {
-        const int buf = g & 1;
-        if (g >= 2) mbar_wait(bar_acc_free + 8 * buf, (uint32_t)(((g >> 1) - 1) & 1));   // epilogue drained this accumulator
-        if (p.has_q && g == p.n_planes) mbar_wait(bar_a_ready, 0u);                      // A tiles now hold relu(LN(q_hidden))
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t d_tmem = tmem + (uint32_t)(buf * 128);
-        for (int c = 0; c < NKC; ++c) {
-          const int i = g * NKC + c, s = i % WS_STAGES;
-          mbar_wait(bar_full + 8 * s, (uint32_t)((i / WS_STAGES) & 1));
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-          const uint32_t b_hi = sbase + SMEM_B0 + s * B_STAGE_BYTES, b_lo = b_hi + B_CHUNK_BYTES;
-#pragma unroll
-          for (int ks = 0; ks < KC / 8; ++ks) {
-            const uint32_t koff_a = (uint32_t)(c * (KC / 4) + ks * 2) * 128u;
-            const uint32_t koff_b = (uint32_t)(ks * 2) * 128u;
-            const uint64_t a_hi = make_desc(sbase + SMEM_A_HI + koff_a, A_SBO);
-            const uint64_t a_lo = make_desc(sbase + SMEM_A_LO + koff_a, A_SBO);
-            const uint64_t d_bhi = make_desc(b_hi + koff_b, B_SBO);
-            const uint64_t d_blo = make_desc(b_lo + koff_b, B_SBO);
-            const uint32_t first = (c == 0 && ks == 0) ? 0u : 1u;
-            umma_tf32(d_tmem, a_lo, d_bhi, first);
-            umma_tf32(d_tmem, a_hi, d_blo, 1u);
-            umma_tf32(d_tmem, a_hi, d_bhi, 1u);
-          }
-          umma_commit(bar_empty + 8 * s);
+        const int s = i % NSTAGE;
+        if (i >= NSTAGE) mbar_wait(bar_empty + 8 * s, (uint32_t)(((i / NSTAGE) - 1) & 1));   // all CL CTAs released the stage
+        const uint32_t bf = bar_full + 8 * s;
+        mbar_expect_tx(bf, B_STAGE_BYTES);                       // the whole chunk lands here (all slices)
+        if (CL > 1) {
+          constexpr uint32_t slice = B_STAGE_BYTES / CL;
+          bulk_g2s_mcast(sbase + SMEM_B0 + s * B_STAGE_BYTES + crank * slice,
+                         reinterpret_cast<const char*>(chunk_src_ptr(p, i)) + crank * slice, slice, bf, kMask);
+        } else {
+          bulk_g2s(sbase + SMEM_B0 + s * B_STAGE_BYTES, chunk_src_ptr(p, i), B_STAGE_BYTES, bf);
         }
-        umma_commit(bar_acc_full + 8 * buf);
       }
     }
   } else {
-    // ===== epilogue warps =====
-    const int q4 = warp & 3, chalf = warp >> 2;
-    const int my_row = 32 * q4 + lane;
-    const int grow = row0 + my_row;
-    const int dst = (grow < p.n_rows) ? (p.row_idx ? p.row_idx[grow] : grow) : -1;
+    // ===== consumer warpgroups: MMAs and epilogue of rows 64 wg .. 64 wg + 63 =====
+    const int wg = warp >> 2, qg = lane >> 2, qt = lane & 3;
+    const int r_lo = 64 * wg + 16 * (warp & 3) + qg;          // this thread's accumulator rows: r_lo and r_lo + 8
+    int dst[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int grow = row0 + r_lo + 8 * h;
+      dst[h] = (grow < p.n_rows) ? (p.row_idx ? p.row_idx[grow] : grow) : -1;
+    }
+    const uint32_t a_base = sbase + (uint32_t)(8 * wg) * A_SBO;
+    const uint64_t da_hi = smem_desc(a_base + SMEM_A_HI, LBO, A_SBO), da_lo = smem_desc(a_base + SMEM_A_LO, LBO, A_SBO);
     for (int g = 0; g < n_gemm; ++g) {
-      const int buf = g & 1;
-      mbar_wait(bar_acc_full + 8 * buf, (uint32_t)((g >> 1) & 1));
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const uint32_t t_lane = tmem + ((uint32_t)(32 * q4) << 16) + (uint32_t)(buf * 128);
+      float d[64];
+#pragma unroll
+      for (int c = 0; c < NKC; ++c) {
+        const int i = g * NKC + c, s = i % NSTAGE;
+        mbar_wait(bar_full + 8 * s, (uint32_t)((i / NSTAGE) & 1));
+        const uint64_t db_hi = smem_desc(sbase + SMEM_B0 + s * B_STAGE_BYTES, LBO, B_SBO);
+        const uint64_t db_lo = smem_desc(sbase + SMEM_B0 + s * B_STAGE_BYTES + B_CHUNK_BYTES, LBO, B_SBO);
+        wgmma_fence();
+#pragma unroll
+        for (int ks = 0; ks < KC / 8; ++ks) {
+          const uint64_t ka = (uint64_t)(16 * (c * (KC / 8) + ks)), kb = (uint64_t)(16 * ks);   // 2 core matrices = 256 bytes per K = 8 step
+          wgmma_tf32_ss(d, da_lo + ka, db_hi + kb, (c == 0 && ks == 0) ? 0u : 1u);              // small terms first
+          wgmma_tf32_ss(d, da_hi + ka, db_lo + kb, 1u);
+          wgmma_tf32_ss(d, da_hi + ka, db_hi + kb, 1u);
+        }
+        wgmma_commit();
+        wgmma_wait0();
+        if ((tid & 127) == 0) {        // this warpgroup is done with the ring stage: tell the producer of every CTA
+          if (CL > 1) { for (uint32_t r = 0; r < (uint32_t)CL; ++r) mbar_arrive_cluster(bar_empty + 8 * s, r); }
+          else mbar_arrive(bar_empty + 8 * s);
+        }
+      }
+      wgmma_settle(d);
       const bool is_qhid = p.has_q && (g == p.n_planes - 1);
       const bool is_q2 = p.has_q && (g == p.n_planes);
       if (!is_qhid) {
         const float* bias = is_q2 ? p.q_b1 : (p.bias + g * CBG_H);
         float* out = is_q2 ? p.out_q : p.out[g];
-#pragma unroll 1
-        for (int cb = 0; cb < 2; ++cb) {
-          const int col0 = chalf * 64 + cb * 32;
-          float v[32];
-          tmem_ld32(t_lane + (uint32_t)col0, v);
-          if (dst >= 0) {
-            float* o = out + (size_t)dst * CBG_H + col0;
 #pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              const float4 b = ldg4(bias + col0 + 4 * j);
-              st4(o + 4 * j, make_float4(v[4 * j] + b.x, v[4 * j + 1] + b.y, v[4 * j + 2] + b.z, v[4 * j + 3] + b.w));
-            }
+        for (int h = 0; h < 2; ++h) {
+          if (dst[h] < 0) continue;
+          float* o = out + (size_t)dst[h] * CBG_H + 2 * qt;
+#pragma unroll
+          for (int j = 0; j < 16; ++j) {
+            const float2 b = __ldg(reinterpret_cast<const float2*>(bias + 8 * j + 2 * qt));
+            *reinterpret_cast<float2*>(o + 8 * j) = make_float2(d[4 * j + 2 * h] + b.x, d[4 * j + 2 * h + 1] + b.y);
           }
         }
       } else {
-        if (chalf == 0) {
-          // q hidden: + bias, two-pass LayerNorm over the row (TMEM is re-read instead of keeping 128 values
-          // live), ReLU, back into the A tiles as the operand of the second Linear
-          const float* bias = p.bias + g * CBG_H;
-          float s = 0.f;
-#pragma unroll 1
-          for (int cb = 0; cb < 4; ++cb) {
-            float t[32];
-            tmem_ld32(t_lane + (uint32_t)(cb * 32), t);
+        // q hidden: + bias, LayerNorm(128) + ReLU per row (a row's columns live in the 4 lanes of a quad), then back
+        // into this warpgroup's rows of the A tiles as the operand of the second Linear
+        const float* bias = p.bias + g * CBG_H;
+        float s0 = 0.f, s1 = 0.f;
 #pragma unroll
-            for (int j = 0; j < 32; ++j) s += t[j] + __ldg(bias + cb * 32 + j);
-          }
-          const float mean = s * (1.f / 128.f);
-          float q = 0.f;
-#pragma unroll 1
-          for (int cb = 0; cb < 4; ++cb) {
-            float t[32];
-            tmem_ld32(t_lane + (uint32_t)(cb * 32), t);
-#pragma unroll
-            for (int j = 0; j < 32; ++j) { const float d = t[j] + __ldg(bias + cb * 32 + j) - mean; q = fmaf(d, d, q); }
-          }
-          const float rstd = 1.f / sqrtf(q * (1.f / 128.f) + 1e-5f);
-#pragma unroll 1
-          for (int cb = 0; cb < 4; ++cb) {
-            float t[32];
-            tmem_ld32(t_lane + (uint32_t)(cb * 32), t);
-#pragma unroll
-            for (int k4 = 0; k4 < 8; ++k4) {
-              const int col = cb * 32 + 4 * k4;
-              const float4 bi = ldg4(bias + col), ga = ldg4(p.q_ln + col), be = ldg4(p.q_ln + 128 + col);
-              float4 a;
-              a.x = fmaxf(fmaf((t[4 * k4 + 0] + bi.x - mean) * rstd, ga.x, be.x), 0.f);
-              a.y = fmaxf(fmaf((t[4 * k4 + 1] + bi.y - mean) * rstd, ga.y, be.y), 0.f);
-              a.z = fmaxf(fmaf((t[4 * k4 + 2] + bi.z - mean) * rstd, ga.z, be.z), 0.f);
-              a.w = fmaxf(fmaf((t[4 * k4 + 3] + bi.w - mean) * rstd, ga.w, be.w), 0.f);
-              store_split(smem, my_row, col >> 2, a);
-            }
-          }
-          asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+        for (int j = 0; j < 16; ++j) {
+          const float2 b = __ldg(reinterpret_cast<const float2*>(bias + 8 * j + 2 * qt));
+          d[4 * j] += b.x; d[4 * j + 1] += b.y; d[4 * j + 2] += b.x; d[4 * j + 3] += b.y;
+          s0 += d[4 * j] + d[4 * j + 1];
+          s1 += d[4 * j + 2] + d[4 * j + 3];
         }
-        __syncwarp();
-        if (lane == 0) mbar_arrive(bar_a_ready);
+        const float mean0 = quad_sum(s0) * (1.f / 128.f), mean1 = quad_sum(s1) * (1.f / 128.f);
+        float q0 = 0.f, q1 = 0.f;
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+          d[4 * j] -= mean0; d[4 * j + 1] -= mean0; d[4 * j + 2] -= mean1; d[4 * j + 3] -= mean1;
+          q0 = fmaf(d[4 * j], d[4 * j], q0); q0 = fmaf(d[4 * j + 1], d[4 * j + 1], q0);
+          q1 = fmaf(d[4 * j + 2], d[4 * j + 2], q1); q1 = fmaf(d[4 * j + 3], d[4 * j + 3], q1);
+        }
+        const float rstd0 = 1.f / sqrtf(quad_sum(q0) * (1.f / 128.f) + 1e-5f);
+        const float rstd1 = 1.f / sqrtf(quad_sum(q1) * (1.f / 128.f) + 1e-5f);
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+          const float2 ga = __ldg(reinterpret_cast<const float2*>(p.q_ln + 8 * j + 2 * qt));
+          const float2 be = __ldg(reinterpret_cast<const float2*>(p.q_ln + 128 + 8 * j + 2 * qt));
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const float rs = h ? rstd1 : rstd0;
+            const float a0 = fmaxf(fmaf(d[4 * j + 2 * h] * rs, ga.x, be.x), 0.f);
+            const float a1 = fmaxf(fmaf(d[4 * j + 2 * h + 1] * rs, ga.y, be.y), 0.f);
+            const float h0 = to_tf32(a0), h1 = to_tf32(a1);
+            const uint32_t off = a_off(r_lo + 8 * h, 8 * j + 2 * qt);
+            *reinterpret_cast<float2*>(smem + SMEM_A_HI + off) = make_float2(h0, h1);
+            *reinterpret_cast<float2*>(smem + SMEM_A_LO + off) = make_float2(to_tf32(a0 - h0), to_tf32(a1 - h1));
+          }
+        }
+        fence_proxy_async();
+        warpgroup_sync(wg);      // the second Linear of this warpgroup reads exactly the rows it has just rewritten
       }
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_acc_free + 8 * buf);
     }
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 0) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(WS_TMEM_COLS));
-  }
+  if (CL > 1) cluster_sync_all();      // no CTA may exit while peers can still write its smem / signal its barriers
 }
 
-int launch_ws(const NodeGemmArgs& a, cudaStream_t st) {
-  static bool attr_dev[CBG_MAX_DEVICES] = {};
-  bool& attr_set = cbg_dev_flag(attr_dev);
-  if (!attr_set) {
-    CBG_CUDA_OK(cudaFuncSetAttribute(node_gemm_ws_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WS_SMEM_TOTAL));
-    attr_set = true;
-  }
-  CBG_PROF_BEGIN(CBG_K_NODE_GEMM, st);
-  node_gemm_ws_kernel<<<(a.n_rows + TM - 1) / TM, 320, WS_SMEM_TOTAL, st>>>(a);
-  CBG_LAUNCHED(CBG_K_NODE_GEMM, st);
-  return 0;
-}
-
-template <int CL, int NSTAGE>
+template <int CL>
 int launch_tc(const NodeGemmArgs& a, cudaStream_t st) {
-  constexpr uint32_t SMEM_TOTAL = smem_total(NSTAGE);
   static bool attr_dev[CBG_MAX_DEVICES] = {};
   bool& attr_set = cbg_dev_flag(attr_dev);
   if (!attr_set) {
-    CBG_CUDA_OK(cudaFuncSetAttribute(node_gemm_tc_kernel<CL, NSTAGE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_TOTAL));
+    CBG_CUDA_OK(cudaFuncSetAttribute(node_gemm_tc_kernel<CL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_TOTAL));
     attr_set = true;
   }
   const int tiles = (a.n_rows + TM - 1) / TM;
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = dim3((unsigned)((tiles + CL - 1) / CL * CL));   // padded tiles run the protocol with zero rows
-  cfg.blockDim = dim3(256);
+  cfg.blockDim = dim3(288);
   cfg.dynamicSmemBytes = SMEM_TOTAL;
   cfg.stream = st;
   cudaLaunchAttribute attr[1];
@@ -549,7 +244,7 @@ int launch_tc(const NodeGemmArgs& a, cudaStream_t st) {
   attr[0].val.clusterDim.x = CL; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
   cfg.attrs = attr; cfg.numAttrs = (CL > 1) ? 1 : 0;
   CBG_PROF_BEGIN(CBG_K_NODE_GEMM, st);
-  CBG_CUDA_OK(cudaLaunchKernelEx(&cfg, node_gemm_tc_kernel<CL, NSTAGE>, a));
+  CBG_CUDA_OK(cudaLaunchKernelEx(&cfg, node_gemm_tc_kernel<CL>, a));
   CBG_LAUNCHED(CBG_K_NODE_GEMM, st);
   return 0;
 }
@@ -559,28 +254,15 @@ int launch_tc(const NodeGemmArgs& a, cudaStream_t st) {
 int cbg_launch_node_gemm_tc(const NodeGemmArgs& a, cudaStream_t st, int cluster) {
   if (a.n_rows <= 0) return 0;
   if (!a.tc_planes) { cbg_set_error("tensor-core node GEMM needs the pre-split weight planes"); return 1; }
-  static int cl_env = -1, stages = -1, use_ws = 1;
+  static int cl_env = -1;
   if (cl_env < 0) {
-    const char* v = getenv("CBG_GEMM_WS");
-    use_ws = !(v && atoi(v) == 0);
     const char* e = getenv("CBG_GEMM_CLUSTER");
     cl_env = e ? atoi(e) : 1;
     if (cl_env != 1 && cl_env != 2 && cl_env != 4) cl_env = 1;
-    const char* s = getenv("CBG_GEMM_STAGES");
-    stages = (s && atoi(s) == 2) ? 2 : 3;
   }
-  if (cluster == 0 && use_ws && cl_env == 1) return launch_ws(a, st);     // default: warp-specialised kernel
-  const int cl = (cluster == 1 || cluster == 2 || cluster == 4) ? cluster : cl_env;
-  if (stages == 2) {
-    switch (cl) {
-      case 2: return launch_tc<2, 2>(a, st);
-      case 4: return launch_tc<4, 2>(a, st);
-      default: return launch_tc<1, 2>(a, st);
-    }
-  }
-  switch (cl) {
-    case 2: return launch_tc<2, 3>(a, st);
-    case 4: return launch_tc<4, 3>(a, st);
-    default: return launch_tc<1, 3>(a, st);
+  switch ((cluster == 1 || cluster == 2 || cluster == 4) ? cluster : cl_env) {
+    case 2: return launch_tc<2>(a, st);
+    case 4: return launch_tc<4>(a, st);
+    default: return launch_tc<1>(a, st);
   }
 }

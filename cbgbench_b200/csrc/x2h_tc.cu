@@ -1,43 +1,32 @@
-// X2H attention on the 5th-generation tensor cores: one CTA tile = 4 destination nodes x 32 in-edges = 128 edge rows.
+// X2H attention on the Hopper tensor cores (wgmma): one CTA tile = 4 destination nodes x 32 in-edges = 128 edge rows,
+// two warpgroups of 64 rows (2 nodes) each.
 //
 // Reference semantics: repo/modules/attention/x2h_attention.py:43-97 (per edge e = (j -> i):
 //   kv = [onehot(type) | onehot(type) (x) g(d) | h_i | h_j], k = MLP_k(kv), v = MLP_v(kv) * e_w,
 //   alpha = softmax_j(<q_i, k_ij>/sqrt(8)) per head, h_i += sum_j alpha_ij v_ij).
 //
-// Both edge MLPs are 340 -> 128 -> LayerNorm -> ReLU -> 128.  Per 128-row tile the kernel runs two GEMMs on tcgen05:
-//   MMA1  pre[128 x 128] = G[128 x 96] * Wg[96 x 128]      G = [onehot(t) (x) g(d) | onehot(t) | onehot(node slot)]
-//                                                           Wg = [Wrf[t] ; c[t] ; Pi rows of the tile's 4 nodes]
-//         (the type-dependent RBF mat-vec, the type bias and the destination-node plane Pi in one K = 96 product;
-//          the source plane Pj[j] is added by the SIMT stage from rows staged in shared memory)
-//   MMA2  out[128 x 128] = relu(LN(pre + Pj)) * W1^T
+// Both edge MLPs are 340 -> 128 -> LayerNorm -> ReLU -> 128.  Per 64-row half tile a warpgroup runs two GEMMs:
+//   MMA1  pre[64 x 128] = G[64 x 96] * Wg[96 x 128]        G = [onehot(t) (x) g(d) | onehot(t)], Wg = [Wrf[t] ; c[t]]
+//         (the type-dependent RBF mat-vec and the type bias in one K = 96 product, A and B from shared memory; the
+//          node planes Pi[i] and Pj[j] are added to the accumulator fragment straight from global memory / L2)
+//   MMA2  out[64 x 128] = relu(LN(pre + Pi + Pj)) * W1^T   (A from REGISTERS: the fp32 accumulator fragment of MMA1,
+//         packed to f16 pairs, is exactly the A fragment wgmma expects - the activations never touch shared memory)
 // fp32 accuracy comes from the split x = hi + lo into two f16 values (scaled by powers of two so lo stays normal)
-// and the three products hi*hi + hi*lo + lo*hi accumulated in fp32 in TMEM (cbg_tc.cuh): same error class as 3xTF32
+// and the three products hi*hi + hi*lo + lo*hi accumulated in fp32 (cbg_tc.cuh): same error class as 3xTF32
 // at twice the tensor-core rate and half the operand bytes.
 //
-// A operands (G and the activations) live in TENSOR MEMORY (tcgen05.mma with A from TMEM: lane = edge row), written
-// by tcgen05.st from the warps that produce them; B operands (weight images, pre-split and pre-laid-out by the host
-// packer) stay resident in shared memory for the whole persistent CTA.  Nothing of size [E, 128] touches HBM and no
-// R-cache is needed: the only per-edge gather is the 512-byte Pj row (cp.async, L2 resident).
-//
-// Warp roles (17 warps x 120 registers):
-//   warps 0-3   EPI       thread = edge row, inputs prefetched one tile ahead.  k: <q_i, k> per head, softmax over the
-//                         node's 32 edges through a shared-memory transpose, w = alpha * e_w;
-//                         v: (v + b1v) * w, sum over the node's 32 edges, h_i += .
-//   warps 4-11  S1        thread = (edge row, column half).  S1(tile t): TMEM(pre) + Pj -> LayerNorm (mean-free: the
-//                         packer centres the first Linear over the feature axis) -> ReLU -> (hi, lo) f16 -> TMEM (in
-//                         place).  Nothing else: this chain is the longest of the pipeline.
-//   warps 12-15 GP        one per TMEM lane quarter / node slot q, one tile ahead of S1: builds the G rows of the slot's 32
-//                         edges (geometry, type, Gaussian smearing -> TMEM, after MMA1 of the previous tile), writes the
-//                         node's Pi row into its K column of the Wg images, and copies the 32 Pj rows into chunk q (cp.async)
-//   warp 16     MMA       one lane issues every tcgen05.mma / commit (fully unrolled, tile-invariant descriptors)
-// Pipelining: TMEM holds two pre/activation buffers, so MMA1 of tile t+1 and MMA2 of tile t-1 run while S1 works on
-// tile t and EPI on tile t-1.
+// B operands (weight images, pre-split and pre-laid-out by the host packer) stay resident in shared memory for the whole
+// persistent CTA (bulk copies, mbarrier).  Nothing of size [E, 128] touches HBM and no R-cache is needed: the only
+// per-edge gather is the 512-byte Pj row, read in the accumulator layout (a quad of lanes = one 32-byte sector of a row).
+// In that layout a row's 128 columns live in the 4 lanes of a quad, so LayerNorm is two shuffles, and a head's 8 columns
+// are one quad's registers, so <q_i, k> per head is two shuffles as well; the softmax over a node's 32 edges (2 warps)
+// and the sum over them go through a small shared-memory buffer.  The two warpgroups only share the weights: each walks
+// its own 2 nodes of every tile, and while one waits on its MMAs or gathers the other one computes.
 //
 // H2X (repo/modules/attention/h2x_attention.py:34-73) runs on the same kernel over the list of generated nodes:
 //   launch 1  MODE_K with the xk / xq weights -> w = alpha * e_w (compact buffer, indexed by list position)
 //   launch 2  MODE_XV with the xv weights: the second Linear has one output per head (N = 16 MMA), and the epilogue forms
 //             dx_i = (1/16) sum_e (sum_hd w_e,hd (v_e,hd + b1_hd)) (x_i - x_j)     (mean over heads of alpha * v * e_w * rel_x)
-// replacing the fp32 SIMT h2x_kernel (edge.cu), whose 4 GFLOP per launch ran at ~65 % of the fp32 pipe.
 #include <math.h>
 #include <stdlib.h>
 #include <string.h>
@@ -77,58 +66,31 @@ struct TcWeights {
 };
 
 // ---- scales (exact powers of two; must match modules.py: tc_f16_image) ----------------------------------------
-constexpr float kScaleG = 1024.f;        // g(d) and the type one-hot in G
 // Wrf, c in Wg are scaled by 16 (packer)                       -> pre accumulates at 2^14
 constexpr float kInvPre = 1.f / 16384.f;
 constexpr uint32_t kHalfTypeOne = 0x6400u;   // f16 1024
-constexpr uint32_t kHalfNodeOne = 0x7400u;   // f16 16384: node one-hot x unscaled Pi = Pi * 2^14
 constexpr float kScaleA = 64.f;          // activations
 constexpr float kInvOut = 1.f / 4096.f;  // W1 image is scaled by 64 -> out accumulates at 2^12
 
 // ---- shapes -----------------------------------------------------------------------------------------------------
-constexpr int KG = 96;                   // K of MMA1 (84 used + 8 node one-hot columns (2 tile parities x 4) + 4 zero)
+constexpr int KG = 96;                   // K of MMA1 (84 used: the packer leaves k >= 84 of the Wg images zero)
 constexpr int KG_LO = 80;                // the lo part of G is non-zero only in the RBF columns
-// Pj ring: 32-row chunks (one node's in-edges), item n = 4 * tile + slot lives in chunk n % R.  With R = 4 the copy of a
-// slot's next rows could only start once the slot's S1 warps had read the current ones, and the 64 KB burst per tile
-// through L2 (~2.7 K cycles) sat on the S1 critical path.  With R = 6 half of a tile's chunks are fetched a whole tile
-// earlier (all quarters consume at the same time, so extra lead comes in whole tiles).  R is what fits beside the weights:
-// 6 for the attention-weight / H2X kernels, 5 for the aggregation kernel (its epilogue scratch is 18 KB).
-constexpr int NCH_MAX = 6;
-__host__ __device__ constexpr int pj_ring_max(int mode) { return mode == 1 ? 5 : 6; }
-// Pj rows: 512 bytes, 128-byte aligned like their source in global memory, the 16-byte pieces of every 128-byte group
-// XOR-swizzled by (row & 7): the row-per-lane reads of S1 are conflict free AND the cp.async row copies take the ideal 4
-// wavefronts (a 528-byte padded stride cost 10.5 on average: the copies alone were 40 % of the kernel's shared-memory
-// wavefronts, and shared memory - LSU traffic + the B operands of 41 MMAs per tile - is the busiest unit of the kernel)
-constexpr uint32_t PJ_ROW = 512;
-constexpr uint32_t PJ_CHUNK = 32 * PJ_ROW;
 constexpr uint32_t W1_IMG = 128 * 128 * 2;            // one (hi | lo) image, bytes
 constexpr uint32_t W1X_IMG = 16 * 128 * 2;            // MODE_XV: 16 output rows
 constexpr uint32_t WG_IMG = 128 * KG * 2;
+constexpr uint32_t G_IMG = 64 * KG * 2;               // one warpgroup's G rows (hi or lo), same layout as the weight images
 constexpr uint32_t W1_SBO = (128 / 8) * 128, WG_SBO = (KG / 8) * 128, LBO = 128;
 constexpr uint32_t SM_W1 = 0;                         // hi | lo
 constexpr uint32_t SM_WG = SM_W1 + 2 * W1_IMG;
-constexpr uint32_t SM_LN = SM_WG + 2 * WG_IMG;        // gamma * 64 [128] | beta * 64 [128]
+constexpr uint32_t SM_G = SM_WG + 2 * WG_IMG;         // [warpgroup][hi | lo]
+constexpr uint32_t SM_LN = SM_G + 4 * G_IMG;          // gamma * 64 [128] | beta * 64 [128]
 constexpr uint32_t SM_B1 = SM_LN + 1024;              // b1v [128]
 constexpr uint32_t SM_RBF = SM_B1 + 512;              // Gaussian offsets [20] + coeff
-constexpr uint32_t SM_XCH = SM_RBF + 128;              // sum-of-squares exchange between the two half-row S1 warps
-constexpr uint32_t SM_QBUF = SM_XCH + 2048;             // EPI: [warp][tile parity][128] q row of the warp's node
-constexpr uint32_t SM_SOFT = SM_QBUF + 4096;            // EPI: [warp][32 edges][17] logits <-> weights transpose
-constexpr uint32_t SM_VRED = SM_QBUF;                   // EPI of the v kernel (aliases QBUF / SOFT): [warp][32 edges][36] transpose
-constexpr int NBAR = 13 + 2 * NCH_MAX;
-// mode-dependent tail of the layout: EPI scratch (k: q rows + softmax transpose, v: the 32 x 36 transposes), barriers, Pj ring
-__host__ __device__ constexpr uint32_t sm_bar(int mode) { return SM_QBUF + (mode == 1 ? 4u * 32 * 36 * 4 : 4096u + 4u * 32 * 17 * 4); }
-__host__ __device__ constexpr uint32_t sm_pj(int mode) { return (sm_bar(mode) + 8u * NBAR + 16u + 127u) & ~127u; }
-__host__ __device__ constexpr uint32_t sm_total(int mode, int nch) { return sm_pj(mode) + (uint32_t)nch * PJ_CHUNK; }
-static_assert(sm_total(0, 6) <= 232448 && sm_total(1, 5) <= 232448 && sm_total(2, 6) <= 232448, "shared memory budget");
-enum { B_WFULL = 0 /* Wg images */, B_GREADY, B_W1FULL /* W1 images */, B_ACC1 /*2*/ = 3, B_AREADY /*2*/ = 5, B_ACC2 /*2*/ = 7, B_ACC2FREE /*2*/ = 9,
-       B_PJFULL = 11, B_PJFREE = 11 + NCH_MAX, B_PIREADY /*2*/ = 11 + 2 * NCH_MAX };
-// TMEM columns
-constexpr uint32_t TM_BUF = 0;           // 2 x 128: pre (fp32) -> a_hi (64 cols) | a_lo (64 cols)
-constexpr uint32_t TM_OUT = 256;         // 128: output accumulator of MMA2
-constexpr uint32_t TM_GHI = 384;         // 48 columns = 96 f16
-constexpr uint32_t TM_GLO = 432;         // 40 columns = 80 f16
-constexpr uint32_t TM_COLS = 512;
-constexpr uint32_t IDESC128 = idesc_f16(128), IDESC16 = idesc_f16(16);
+constexpr uint32_t SM_EPI = SM_RBF + 128;             // k: [node slot][32 edges][17] logits; v: [slot][warp][128] partial sums; xv: [slot][warp][4]
+constexpr uint32_t SM_BAR = SM_EPI + 4 * 32 * 17 * 4;
+constexpr uint32_t SM_TOTAL = SM_BAR + 64;
+static_assert(SM_TOTAL <= 232448, "shared memory budget");
+enum { B_WFULL = 0 /* Wg images */, B_W1FULL /* W1 images */ };
 
 __device__ __forceinline__ int list_len(const EdgeArgs& p) {
   int n = p.n_nodes;
@@ -139,31 +101,34 @@ __device__ __forceinline__ int node_of(const EdgeArgs& p, int n, int n_list) {
   const int nc = n < n_list ? n : n_list - 1;
   return p.node_idx ? p.node_idx[nc] : nc;
 }
-__device__ __forceinline__ float warp_sum_x(float v) {      // fixed butterfly order: deterministic
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(CBG_FULL, v, o);
-  return v;
+__device__ __forceinline__ float quad_sum(float v) {        // fixed butterfly order: deterministic
+  v += __shfl_xor_sync(CBG_FULL, v, 1);
+  return v + __shfl_xor_sync(CBG_FULL, v, 2);
 }
+__device__ __forceinline__ float rows_sum(float v) {        // over the 8 row groups of a warp (lanes with equal lane % 4)
+  v += __shfl_xor_sync(CBG_FULL, v, 4);
+  v += __shfl_xor_sync(CBG_FULL, v, 8);
+  return v + __shfl_xor_sync(CBG_FULL, v, 16);
+}
+__device__ __forceinline__ float2 ldg2(const float* p) { return __ldg(reinterpret_cast<const float2*>(p)); }
 
-// pipeline event stamps of CTA 0 (debugging; p.trace == nullptr in production: one predicated-off branch per event)
+// pipeline event stamps of warpgroup 0 of CTA 0 (debugging; p.trace == nullptr in production: one predicated-off branch per
+// event).  Events of a tile: 0 G rows staged, 1 MMA1 complete, 2 activations ready, 3 MMA2 complete, 4 epilogue done
 #define TC_STAMP(k, ev)                                                                                  \
   do {                                                                                                   \
-    if (p.trace != nullptr && blockIdx.x == 0 && lane == 0 && (k) < p.trace_tiles) p.trace[(k) * 16 + (ev)] = clock64(); \
+    if (p.trace != nullptr && blockIdx.x == 0 && tid == 0 && (k) < p.trace_tiles) p.trace[(k) * 16 + (ev)] = clock64(); \
   } while (0)
 
 // =================================================================================================================
-template <int MODE, int NCH>
-__global__ void __launch_bounds__(544, 1) x2h_tc_kernel(EdgeArgs p, TcWeights W) {
-  static_assert(NCH >= 4 && NCH <= pj_ring_max(MODE), "Pj ring depth");
+template <int MODE>
+__global__ void __launch_bounds__(256, 1) x2h_tc_kernel(EdgeArgs p, TcWeights W) {
   constexpr bool IS_V = MODE == MODE_V, IS_XV = MODE == MODE_XV;
   extern __shared__ __align__(1024) uint8_t smem[];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const uint32_t sbase = smem_u32(smem);
-  constexpr uint32_t SM_BAR = sm_bar(MODE), SM_PJ = sm_pj(MODE);
   constexpr uint32_t W1B = IS_XV ? W1X_IMG : W1_IMG;      // bytes of one second-Linear image
   const uint32_t bars = sbase + SM_BAR;
   auto bar = [&](int i) { return bars + 8u * (uint32_t)i; };
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + SM_BAR + 8 * NBAR);
 
   // ---- prologue: nothing here reads what the previous kernel of the stream produces (weights are constants), so with a
   // programmatic dependent launch it overlaps that kernel's tail; pdl_wait() below is the dependency
@@ -171,24 +136,13 @@ __global__ void __launch_bounds__(544, 1) x2h_tc_kernel(EdgeArgs p, TcWeights W)
   // debugging: CTA 0 stamps kernel entry / end of prologue / exit into the row behind the per-tile rows of the trace buffer
 #define TC_STAMP_CTA(ev) do { if (p.trace != nullptr && blockIdx.x == 0 && tid == 0) p.trace[p.trace_tiles * 16 + (ev)] = clock64(); } while (0)
   TC_STAMP_CTA(0);
-  if (warp == 0) tmem_alloc(smem_u32(tmem_slot), TM_COLS);
   if (tid == 32) {
     mbar_init(bar(B_WFULL), 1);
     mbar_init(bar(B_W1FULL), 1);
-    mbar_init(bar(B_GREADY), 4);
-    mbar_init(bar(B_PIREADY), 4);
-    mbar_init(bar(B_PIREADY + 1), 4);
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(bar(B_ACC1 + b), 1);
-      mbar_init(bar(B_AREADY + b), 8);
-      mbar_init(bar(B_ACC2 + b), 1);
-      mbar_init(bar(B_ACC2FREE + b), 4);
-    }
-    for (int c = 0; c < NCH; ++c) { mbar_init(bar(B_PJFULL + c), 32); mbar_init(bar(B_PJFREE + c), 2); }
     fence_mbar_init();
     // Resident weight images by bulk (TMA) copies.  Wg first on its own barrier: MMA1 of the first tile needs only Wg,
-    // W1 is not read before MMA2 (a tile's S1 later).  Every CTA of the grid reads the same 112 KB at the same moment, so
-    // each image goes in four pieces whose order is rotated by the CTA index: at any time the CTAs pull different L2 lines.
+    // W1 is not read before MMA2.  Every CTA of the grid reads the same 112 KB at the same moment, so each image goes
+    // in four pieces whose order is rotated by the CTA index: at any time the CTAs pull different L2 lines.
     mbar_expect_tx(bar(B_WFULL), 2 * WG_IMG);
     mbar_expect_tx(bar(B_W1FULL), 2 * W1B);
     const uint32_t rot = blockIdx.x & 3u;
@@ -203,12 +157,12 @@ __global__ void __launch_bounds__(544, 1) x2h_tc_kernel(EdgeArgs p, TcWeights W)
       bulk_g2s(sbase + SM_W1 + pc * nb, reinterpret_cast<const uint8_t*>(W.w1) + pc * nb, nb, bar(B_W1FULL));
     }
   }
-  {   // LayerNorm affine (pre-multiplied by the activation scale) and the value bias
+  {   // LayerNorm affine (pre-multiplied by the activation scale), the value bias and the Gaussian table
     float* s_ln = reinterpret_cast<float*>(smem + SM_LN);
     float* s_b1 = reinterpret_cast<float*>(smem + SM_B1);
-    if (tid < 256) s_ln[tid] = W.ln[tid] * kScaleA;
-    else if (tid < 384) s_b1[tid - 256] = (IS_V || (IS_XV && tid - 256 < CBG_HEADS)) ? W.b1[tid - 256] : 0.f;
-    else if (tid < 384 + 24) reinterpret_cast<float*>(smem + SM_RBF)[tid - 384] = W.rbf[tid - 384];
+    s_ln[tid] = W.ln[tid] * kScaleA;
+    if (tid < 128) s_b1[tid] = (IS_V || (IS_XV && tid < CBG_HEADS)) ? W.b1[tid] : 0.f;
+    else if (tid < 128 + 24) reinterpret_cast<float*>(smem + SM_RBF)[tid - 128] = W.rbf[tid - 128];
   }
   pdl_wait();
   const int n_list = list_len(p);
@@ -217,498 +171,307 @@ __global__ void __launch_bounds__(544, 1) x2h_tc_kernel(EdgeArgs p, TcWeights W)
   const int n_my = has_work ? (n_tiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;     // tiles of this CTA: blockIdx.x + k * gridDim.x
   // node of slot `slot` of this CTA's kk-th tile (clamped to the list: surplus slots of the last tile redo the last node)
   auto tile_node = [&](int kk, int slot) { return node_of(p, 4 * ((int)blockIdx.x + kk * (int)gridDim.x) + slot, n_list); };
-  // row of the w buffer: the node id (X2H: [N, 32, 16]) or the list position (H2X: compact [n_list, 32, 16])
-  auto w_row = [&](int kk, int slot, int i) {
-    const int n = 4 * ((int)blockIdx.x + kk * (int)gridDim.x) + slot;
-    return p.w_compact ? (n < n_list ? n : n_list - 1) : i;
-  };
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
   TC_STAMP_CTA(1);
+  // the bulk copies must land before the CTA reads the images - or exits (device-side list shorter than the grid)
+  mbar_wait(bar(B_WFULL), 0u);
+  mbar_wait(bar(B_W1FULL), 0u);
 
-  if (!has_work) {
-    if (tid == 32) { mbar_wait(bar(B_WFULL), 0u); mbar_wait(bar(B_W1FULL), 0u); }      // (device-side list shorter than the grid) the bulk copies must land before the CTA exits
-  } else if (warp >= 4 && warp < 12) {
-    // ===================================== S1 (tile k) =================================================================
-    // thread = (edge row, column half hf).  S1: pre = TMEM + Pj -> LayerNorm -> ReLU -> (hi, lo) f16 -> TMEM.  The
-    // first Linear is centred over the feature axis by the packer, so pre has zero mean and LayerNorm needs only the
-    // sum of squares.  (The G rows, the Pj copies and the Pi columns are produced by the GP warps below: with the G build
-    // inside this loop the S1 chain was ~5.1 K of the 5.6 K cycles per tile - the limiter of the kernel.)
-    const int wq = warp & 3, hf = (warp >> 2) - 1;      // warps 4-7: column half 0, 8-11: half 1 (lane quarter = warp % 4)
-    const uint32_t t_lane = tmem + ((uint32_t)(32 * wq) << 16);
-    const float* s_ln = reinterpret_cast<const float*>(smem + SM_LN) + 64 * hf;
-    float* s_x = reinterpret_cast<float*>(smem + SM_XCH);
-    const int row = 32 * wq + lane;
-    for (int k = 0; k < n_my; ++k) {
-      const int b = k & 1;
-      const int item = 4 * k + wq;                        // Pj ring: item n lives in chunk n % NCH, use number n / NCH
-      const int c = item % NCH;
-      mbar_wait(bar(B_ACC1 + b), (uint32_t)((k >> 1) & 1));      // MMA1(k) complete: pre is ready
-      tc_fence_after();
-      if (warp == 4) TC_STAMP(k, 0);
-      if (warp == 8) TC_STAMP(k, 5);
-      mbar_wait(bar(B_PJFULL + c), (uint32_t)((item / NCH) & 1));
-      // ---- S1
-      const uint32_t t_buf = t_lane + TM_BUF + 128u * (uint32_t)b;
-      float v[64];
-      {
-        uint32_t r[2][32];
-        tmem_ld32_nowait(t_buf + 64u * hf, r[0]);
-        tmem_ld32_nowait(t_buf + 64u * hf + 32u, r[1]);
-        tmem_wait_ld();
-        const uint8_t* prow = smem + SM_PJ + (uint32_t)c * PJ_CHUNK + (uint32_t)lane * PJ_ROW + 256u * hf;
-        uint32_t x7 = (uint32_t)(lane & 7);                // swizzle key of this thread's row
-        asm volatile("" : "+r"(x7));                       // recompute the 16 piece offsets per tile (2 ALU ops each): hoisted out of
-                                                           // the tile loop they are spilled and reloaded through L1 instead
+  // ---- thread roles ------------------------------------------------------------------------------------------------
+  const int wg = warp >> 2, w4 = warp & 3, qg = lane >> 2, qt = lane & 3;
+  // G build: thread = (row of the warpgroup's half tile, hi | lo image)
+  const int g_row = tid & 63, g_part = (tid >> 6) & 1;
+  const int g_slot = 2 * wg + (g_row >> 5);
+  // MMA fragments / epilogue: node slot of this warp, its two edge rows e0 and e0 + 8 of the node's 32
+  const int slot = 2 * wg + (w4 >> 1), wp = w4 & 1, e0 = 16 * wp + qg;
+  const float* rbf = reinterpret_cast<const float*>(smem + SM_RBF);
+  const float c2 = rbf[20] * 1.4426950408889634f;      // exp(c u^2) = 2^(c log2(e) u^2)
+  const float* s_ln = reinterpret_cast<const float*>(smem + SM_LN);
+  const float* s_b1 = reinterpret_cast<const float*>(smem + SM_B1);
+  float* s_epi = reinterpret_cast<float*>(smem + SM_EPI);
+  const float* pj_plane = MODE != MODE_K ? p.pj_v : p.pj_k;
+  const float* pi_plane = MODE != MODE_K ? p.pi_v : p.pi_k;
+  const uint32_t g_base = sbase + SM_G + (uint32_t)wg * 2u * G_IMG;
+  const uint64_t dg_hi = smem_desc(g_base, LBO, WG_SBO), dg_lo = smem_desc(g_base + G_IMG, LBO, WG_SBO);
+  const uint64_t dw_hi = smem_desc(sbase + SM_WG, LBO, WG_SBO), dw_lo = smem_desc(sbase + SM_WG + WG_IMG, LBO, WG_SBO);
+  const uint64_t d1_hi = smem_desc(sbase + SM_W1, LBO, W1_SBO), d1_lo = smem_desc(sbase + SM_W1 + W1B, LBO, W1_SBO);
+
+  for (int k = 0; k < n_my; ++k) {
+    // ---- G row of this thread's edge (x2h_attention.py:46-52, unitransformer.py:88-99; explicit operation order:
+    // position-independent results; the factor 1024 of the G scale rides in the exponent).  Type block tb occupies
+    // k = 20 tb .. 20 tb + 19, the type one-hot k = 80 .. 83 of G_hi.
+    {
+      const int i = tile_node(k, g_slot);
+      const int jn = p.nbr[(size_t)i * CBG_KMAX + (g_row & 31)];
+      const float4 xi = p.x4[i], xj = p.x4[jn >= 0 ? jn : i];
+      const float rx = xi.x - xj.x, ry = xi.y - xj.y, rz = xi.z - xj.z;
+      const float d = sqrtf(__fmaf_rn(rz, rz, __fmaf_rn(ry, ry, __fmul_rn(rx, rx))));
+      const int fi = node_flags(xi), fj = node_flags(xj);
+      const int t_e = ((fj & 1) ? 0 : 2) + ((fi & 1) ? 0 : 1);
+      uint32_t gv[10];
 #pragma unroll
-        for (int j = 0; j < 16; ++j) {
-          const float4 pj = *reinterpret_cast<const float4*>(prow + 128u * (j >> 3) + 16u * ((uint32_t)(j & 7) ^ x7));
-          const uint32_t* rv = &r[j >> 3][4 * (j & 7)];
-          const float2 a0 = __ffma2_rn(make_float2(__uint_as_float(rv[0]), __uint_as_float(rv[1])),
-                                       make_float2(kInvPre, kInvPre), make_float2(pj.x, pj.y));
-          const float2 a1 = __ffma2_rn(make_float2(__uint_as_float(rv[2]), __uint_as_float(rv[3])),
-                                       make_float2(kInvPre, kInvPre), make_float2(pj.z, pj.w));
-          v[4 * j] = a0.x; v[4 * j + 1] = a0.y; v[4 * j + 2] = a1.x; v[4 * j + 3] = a1.y;
-        }
+      for (int mp = 0; mp < 10; ++mp) {
+        const float u0 = d - rbf[2 * mp], u1 = d - rbf[2 * mp + 1];
+        float g0, g1;
+        asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(g0) : "f"(fmaf(c2 * u0, u0, 10.f)));
+        asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(g1) : "f"(fmaf(c2 * u1, u1, 10.f)));
+        uint32_t hi, lo;
+        split_pair(g0, g1, hi, lo);
+        gv[mp] = g_part ? lo : hi;
       }
-      if (warp == 4) TC_STAMP(k, 2);
-      float2 q2 = make_float2(0.f, 0.f);
+      uint8_t* grow = smem + SM_G + (uint32_t)(2 * wg + g_part) * G_IMG + (uint32_t)(g_row >> 3) * WG_SBO + (uint32_t)(g_row & 7) * 16u;
 #pragma unroll
-      for (int j = 0; j < 32; ++j) q2 = __ffma2_rn(make_float2(v[2 * j], v[2 * j + 1]), make_float2(v[2 * j], v[2 * j + 1]), q2);
-      const float qs = q2.x + q2.y;
-      s_x[256 * b + 128 * hf + row] = qs;
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar(B_PJFREE + c));          // this warp is done with the ring chunk
-      asm volatile("bar.sync %0, 64;" ::"r"(1 + wq) : "memory");   // the two half-row warps of this row quarter
-      if (warp == 4) TC_STAMP(k, 3);
-      const float qo = s_x[256 * b + 128 * (hf ^ 1) + row];
-      float rstd = rsqrtf((qs + qo) * (1.f / 128.f) + 1e-5f);      // MUFU.RSQ + one Newton step: < 1 ulp
-      rstd = rstd * (1.5f - 0.5f * ((qs + qo) * (1.f / 128.f) + 1e-5f) * rstd * rstd);
-      const float2 rr = make_float2(rstd, rstd);
-      // relu((pre * rstd) * gamma + beta) * 64 -> (hi, lo) f16 into the buffer's columns: hi 0-63, lo 64-127
-      // (the partner thread has read its accumulator columns before the barrier above)
-#pragma unroll
-      for (int ch = 0; ch < 2; ++ch) {
-        uint32_t hi[16], lo[16];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const float4 ga = *reinterpret_cast<const float4*>(s_ln + 32 * ch + 4 * j);
-          const float4 be = *reinterpret_cast<const float4*>(s_ln + 128 + 32 * ch + 4 * j);
-          const int e = 32 * ch + 4 * j;
-          float2 y0 = __fmul2_rn(make_float2(v[e], v[e + 1]), rr);
-          float2 y1 = __fmul2_rn(make_float2(v[e + 2], v[e + 3]), rr);
-          y0 = __ffma2_rn(y0, make_float2(ga.x, ga.y), make_float2(be.x, be.y));
-          y1 = __ffma2_rn(y1, make_float2(ga.z, ga.w), make_float2(be.z, be.w));
-          split_pair_relu(y0.x, y0.y, hi[2 * j], lo[2 * j]);
-          split_pair_relu(y1.x, y1.y, hi[2 * j + 1], lo[2 * j + 1]);
-        }
-        tmem_st16(t_buf + 32u * hf + 16u * ch, hi);
-        tmem_st16(t_buf + 64u + 32u * hf + 16u * ch, lo);
+      for (int c = 0; c < KG_LO / 8; ++c) {        // 16-byte core-matrix rows: f16 pairs 4 c .. 4 c + 3
+        uint4 w;
+        w.x = (t_e == (4 * c) / 10) ? gv[(4 * c) % 10] : 0u;
+        w.y = (t_e == (4 * c + 1) / 10) ? gv[(4 * c + 1) % 10] : 0u;
+        w.z = (t_e == (4 * c + 2) / 10) ? gv[(4 * c + 2) % 10] : 0u;
+        w.w = (t_e == (4 * c + 3) / 10) ? gv[(4 * c + 3) % 10] : 0u;
+        *reinterpret_cast<uint4*>(grow + 128u * c) = w;
       }
-      tmem_wait_st();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar(B_AREADY + b));
-      if (warp == 4) TC_STAMP(k, 4);
-      if (warp == 8) TC_STAMP(k, 6);
+      if (g_part == 0) {        // k = 80 .. 95 exist in G_hi only: the type one-hot, then zeros
+        uint4 w = make_uint4(0u, 0u, 0u, 0u);
+        w.x = (t_e == 0) ? kHalfTypeOne : ((t_e == 1) ? (kHalfTypeOne << 16) : 0u);
+        w.y = (t_e == 2) ? kHalfTypeOne : ((t_e == 3) ? (kHalfTypeOne << 16) : 0u);
+        *reinterpret_cast<uint4*>(grow + 128u * 10) = w;
+        *reinterpret_cast<uint4*>(grow + 128u * 11) = make_uint4(0u, 0u, 0u, 0u);
+      }
     }
-  } else if (warp < 4) {
-    // ===================================== EPI (tile k), inputs prefetched one tile ahead ========================
-    const int wq = warp;
-    const uint32_t t_lane = tmem + ((uint32_t)(32 * wq) << 16);
-    const float* s_b1 = reinterpret_cast<const float*>(smem + SM_B1);
-    float* s_q = reinterpret_cast<float*>(smem + SM_QBUF) + wq * 256;          // [tile parity][128]: q row of the node
-    float* s_sm = reinterpret_cast<float*>(smem + SM_SOFT) + wq * (32 * 17);   // [edge][17]: logits / weights transpose
-    float* s_vr = reinterpret_cast<float*>(smem + SM_VRED) + wq * (32 * 36);   // v kernel: [edge][36] transpose (aliases the two above)
-    // prefetched inputs of the next tile
-    int i_n = tile_node(0, wq), i_nn = n_my > 1 ? tile_node(1, wq) : 0;
-    int jn_n = -1;          // raw neighbour id of the next tile's edge (compared where it is used: no stall on the load)
-    float ew_n = 0.f, h_n[4] = {0.f, 0.f, 0.f, 0.f};
-    float4 w_n[4];
-    auto prefetch = [&](int kk, int i) {
-      const size_t eoff = (size_t)i * CBG_KMAX + lane;
-      const size_t woff = ((size_t)w_row(kk, wq, i) * CBG_KMAX + lane) * CBG_HEADS;
-      if constexpr (MODE == MODE_K) {
-        jn_n = p.nbr[eoff];
-        ew_n = p.ew[eoff];
-        cp_async16(smem_u32(s_q + 128 * (kk & 1)) + 16u * (uint32_t)lane, p.q + (size_t)i * CBG_H + 4 * lane);
-        asm volatile("cp.async.commit_group;" ::: "memory");
-      } else {
-        const float* wi = p.w + woff;
+    fence_proxy_async();
+    warpgroup_sync(wg);
+    TC_STAMP(k, 0);
+
+    // ---- inputs of this thread's two accumulator rows
+    const int n = 4 * ((int)blockIdx.x + k * (int)gridDim.x) + slot;
+    const bool live = n < n_list;
+    const int i = tile_node(k, slot);
+    const int w_row = p.w_compact ? (n < n_list ? n : n_list - 1) : i;       // row of the w buffer: list position (H2X) or node id
+    const size_t eoff = (size_t)i * CBG_KMAX + e0;
+    const int jn0 = p.nbr[eoff], jn1 = p.nbr[eoff + 8];
+    float v[64];
+    {   // Pi[i] + Pj[j] in the accumulator layout
+      const float* pi = pi_plane + (size_t)i * CBG_H + 2 * qt;
+      const float* pj0 = pj_plane + (size_t)(jn0 >= 0 ? jn0 : i) * CBG_H + 2 * qt;
+      const float* pj1 = pj_plane + (size_t)(jn1 >= 0 ? jn1 : i) * CBG_H + 2 * qt;
 #pragma unroll
-        for (int j = 0; j < 4; ++j) w_n[j] = ld4(wi + 4 * j);
-        if constexpr (IS_V) {
-#pragma unroll
-          for (int j = 0; j < 4; ++j) h_n[j] = p.h[(size_t)i * CBG_H + 32 * j + lane];
-        } else {      // MODE_XV: x_i - x_j of this lane's edge (padded slots: j = i, and their w is zero)
-          const int jn = p.nbr[eoff];
-          const float4 xi = p.x4[i], xj = p.x4[jn >= 0 ? jn : i];
-          h_n[0] = xi.x - xj.x; h_n[1] = xi.y - xj.y; h_n[2] = xi.z - xj.z;
-        }
+      for (int j = 0; j < 16; ++j) {
+        const float2 a = ldg2(pi + 8 * j), b0 = ldg2(pj0 + 8 * j), b1 = ldg2(pj1 + 8 * j);
+        v[4 * j] = a.x + b0.x; v[4 * j + 1] = a.y + b0.y; v[4 * j + 2] = a.x + b1.x; v[4 * j + 3] = a.y + b1.y;
       }
-    };
-    prefetch(0, i_n);
-    for (int k = 0; k < n_my; ++k) {
-      const int n = 4 * ((int)blockIdx.x + k * (int)gridDim.x) + wq;
-      const bool live = n < n_list;
-      const int i = i_n;
-      const size_t eoff = (size_t)i * CBG_KMAX + lane;
-      // take over this tile's inputs, start the next tile's
-      const bool valid = jn_n >= 0;
-      const float ew = ew_n;
-      float wv[CBG_HEADS], hv[4];
-      const size_t woff = ((size_t)w_row(k, wq, i) * CBG_KMAX + lane) * CBG_HEADS;
-      if constexpr (MODE != MODE_K) {
+    }
+    // ---- MMA1: small terms first
+    float d[64];
+    wgmma_fence();
 #pragma unroll
-        for (int j = 0; j < 4; ++j) { wv[4 * j] = w_n[j].x; wv[4 * j + 1] = w_n[j].y; wv[4 * j + 2] = w_n[j].z; wv[4 * j + 3] = w_n[j].w; hv[j] = h_n[j]; }
-      } else {
-        asm volatile("cp.async.wait_group 0;" ::: "memory");      // q row of this tile has landed (own copies only)
-        __syncwarp();
+    for (int ks = 0; ks < KG_LO / 16; ++ks) wgmma_f16_ss(d, dg_lo + 16u * ks, dw_hi + 16u * ks, ks > 0 ? 1u : 0u);
+#pragma unroll
+    for (int ks = 0; ks < KG / 16; ++ks) wgmma_f16_ss(d, dg_hi + 16u * ks, dw_lo + 16u * ks, 1u);
+#pragma unroll
+    for (int ks = 0; ks < KG / 16; ++ks) wgmma_f16_ss(d, dg_hi + 16u * ks, dw_hi + 16u * ks, 1u);
+    wgmma_commit();
+    wgmma_wait0();
+    wgmma_settle(d);
+    TC_STAMP(k, 1);
+    // ---- S1: pre = acc + Pi + Pj -> LayerNorm -> ReLU -> (hi, lo) f16 A fragments.  The first Linear is centred over
+    // the feature axis by the packer, so pre has zero mean and LayerNorm needs only the sum of squares.
+    uint32_t a_hi[8][4], a_lo[8][4];
+    {
+      float q0 = 0.f, q1 = 0.f;
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        v[4 * j] = fmaf(d[4 * j], kInvPre, v[4 * j]);
+        v[4 * j + 1] = fmaf(d[4 * j + 1], kInvPre, v[4 * j + 1]);
+        v[4 * j + 2] = fmaf(d[4 * j + 2], kInvPre, v[4 * j + 2]);
+        v[4 * j + 3] = fmaf(d[4 * j + 3], kInvPre, v[4 * j + 3]);
+        q0 = fmaf(v[4 * j], v[4 * j], q0); q0 = fmaf(v[4 * j + 1], v[4 * j + 1], q0);
+        q1 = fmaf(v[4 * j + 2], v[4 * j + 2], q1); q1 = fmaf(v[4 * j + 3], v[4 * j + 3], q1);
       }
-      i_n = i_nn;
-      if (k + 1 < n_my) prefetch(k + 1, i_n);
-      if (k + 2 < n_my) i_nn = tile_node(k + 2, wq);
-      if constexpr (MODE == MODE_K) {
-        const float* qs = s_q + 128 * (k & 1);
-        float* my = s_sm + lane * 17;
+      float rs[2];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const float var = quad_sum(h ? q1 : q0) * (1.f / 128.f) + 1e-5f;
+        const float r = rsqrtf(var);                      // MUFU.RSQ + one Newton step: < 1 ulp
+        rs[h] = r * (1.5f - 0.5f * var * r * r);
+      }
+      // relu((pre * rstd) * gamma + beta) * 64; accumulator columns 16 s .. 16 s + 15 are the A fragment of K step s
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        const float2 ga = *reinterpret_cast<const float2*>(s_ln + 8 * j + 2 * qt);
+        const float2 be = *reinterpret_cast<const float2*>(s_ln + 128 + 8 * j + 2 * qt);
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
-          if (h == 0) { mbar_wait(bar(B_ACC2), (uint32_t)(k & 1)); tc_fence_after(); }
-          if (warp == 0) TC_STAMP(k, 7 + h);
-          uint32_t r[2][32];
-          tmem_ld32_nowait(t_lane + TM_OUT + 64u * h, r[0]);
-          tmem_ld32_nowait(t_lane + TM_OUT + 64u * h + 32u, r[1]);
-          tmem_wait_ld();
-          if (h == 1) {      // the whole accumulator row is in registers: MMA2 of the next tile may overwrite it
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(bar(B_ACC2FREE));
-          }
-#pragma unroll
-          for (int hh = 0; hh < 8; ++hh) {
-            const float4 q0 = *reinterpret_cast<const float4*>(qs + 64 * h + 8 * hh);
-            const float4 q1 = *reinterpret_cast<const float4*>(qs + 64 * h + 8 * hh + 4);
-            const uint32_t* rv = &r[hh >> 2][8 * (hh & 3)];
-            float2 tt = __fmul2_rn(make_float2(__uint_as_float(rv[0]), __uint_as_float(rv[1])), make_float2(q0.x, q0.y));
-            tt = __ffma2_rn(make_float2(__uint_as_float(rv[2]), __uint_as_float(rv[3])), make_float2(q0.z, q0.w), tt);
-            tt = __ffma2_rn(make_float2(__uint_as_float(rv[4]), __uint_as_float(rv[5])), make_float2(q1.x, q1.y), tt);
-            tt = __ffma2_rn(make_float2(__uint_as_float(rv[6]), __uint_as_float(rv[7])), make_float2(q1.z, q1.w), tt);
-            my[8 * h + hh] = valid ? (tt.x + tt.y) * kInvOut : -INFINITY;      // row = edge, stride 17: conflict free
-          }
-        }
-        __syncwarp();
-        // softmax over the 32 edges per head through the shared-memory transpose: lane = (head, half of the edges)
-        {
-          const int hd = lane & 15, e0 = 16 * (lane >> 4);
-          float l[16];
-          float mx = -INFINITY;
-#pragma unroll
-          for (int j = 0; j < 16; ++j) { l[j] = s_sm[(e0 + j) * 17 + hd]; mx = fmaxf(mx, l[j]); }
-          mx = fmaxf(mx, __shfl_xor_sync(CBG_FULL, mx, 16));
-          float sum = 0.f;
-#pragma unroll
-          for (int j = 0; j < 16; ++j) { l[j] = (mx == -INFINITY) ? 0.f : __expf(l[j] - mx); sum += l[j]; }
-          sum += __shfl_xor_sync(CBG_FULL, sum, 16);
-          const float inv = 1.f / ((sum > 0.f) ? sum : 1.f);
-          __syncwarp();
-#pragma unroll
-          for (int j = 0; j < 16; ++j) s_sm[(e0 + j) * 17 + hd] = l[j] * inv;
-        }
-        __syncwarp();
-        if (live) {      // w = alpha * e_w, this lane's edge row
-          const float sc = valid ? ew : 0.f;
-          float* wo = p.w + woff;
-#pragma unroll
-          for (int j = 0; j < 4; ++j)
-            st4(wo + 4 * j, make_float4(my[4 * j] * sc, my[4 * j + 1] * sc, my[4 * j + 2] * sc, my[4 * j + 3] * sc));
-        }
-        __syncwarp();
-      } else if constexpr (IS_XV) {
-        // H2X coordinate update: s_e = sum_hd w_e,hd (v_e,hd + b1_hd), dx_i = (1/16) sum_e s_e (x_i - x_j)
-        mbar_wait(bar(B_ACC2), (uint32_t)(k & 1));
-        tc_fence_after();
-        if (warp == 0) TC_STAMP(k, 7);
-        uint32_t r[16];
-        tmem_ld16_nowait(t_lane + TM_OUT, r);
-        tmem_wait_ld();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(bar(B_ACC2FREE));
-        float sacc = 0.f;
-#pragma unroll
-        for (int hd = 0; hd < CBG_HEADS; ++hd) sacc = fmaf(fmaf(__uint_as_float(r[hd]), kInvOut, s_b1[hd]), wv[hd], sacc);
-        const float ax = warp_sum_x(sacc * hv[0]), ay = warp_sum_x(sacc * hv[1]), az = warp_sum_x(sacc * hv[2]);
-        if (live && lane == 0) st4(p.dx + 4 * (size_t)n, make_float4(ax * (1.f / 16.f), ay * (1.f / 16.f), az * (1.f / 16.f), 0.f));
-      } else {
-        // Four rounds of 32 columns (features 32 p .. 32 p + 31).  This warp is the critical one of the aggregation kernel
-        // (TMEM load -> scale -> transpose -> reduce -> store, four dependent rounds per tile), so the TMEM load of round
-        // p + 1 is issued as soon as round p's registers have gone to shared memory and flies during the reduction.
-        mbar_wait(bar(B_ACC2), (uint32_t)(k & 1));
-        tc_fence_after();
-        if (warp == 0) TC_STAMP(k, 7);
-        uint32_t r[32];
-        tmem_ld32_nowait(t_lane + TM_OUT, r);
-#pragma unroll
-        for (int pp = 0; pp < 4; ++pp) {
-          const int h = pp >> 1, qq = pp & 1;
-          tmem_wait_ld();
-          if (pp == 3) {      // last piece of the accumulator row is in registers
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(bar(B_ACC2FREE));
-          }
-          if (warp == 0 && pp == 2) TC_STAMP(k, 8);
-          // (v + b1v) * w -> this lane's row of the transpose buffer (stride 36 words: 16-byte stores conflict free),
-          // then lane l sums column l over the node's 32 edges (fixed order: deterministic)
-          float* vrow = s_vr + lane * 36;
-#pragma unroll
-          for (int c4 = 0; c4 < 8; ++c4) {
-            const float4 b1 = *reinterpret_cast<const float4*>(s_b1 + 64 * h + 32 * qq + 4 * c4);
-            const float wh = wv[8 * h + 4 * qq + (c4 >> 1)];
-            float4 o;
-            o.x = fmaf(__uint_as_float(r[4 * c4 + 0]), kInvOut, b1.x) * wh;
-            o.y = fmaf(__uint_as_float(r[4 * c4 + 1]), kInvOut, b1.y) * wh;
-            o.z = fmaf(__uint_as_float(r[4 * c4 + 2]), kInvOut, b1.z) * wh;
-            o.w = fmaf(__uint_as_float(r[4 * c4 + 3]), kInvOut, b1.w) * wh;
-            *reinterpret_cast<float4*>(vrow + 4 * c4) = o;
-          }
-          if (pp < 3) tmem_ld32_nowait(t_lane + TM_OUT + 32u * (uint32_t)(pp + 1), r);
-          __syncwarp();
-          float val;
-          {
-            float s0 = 0.f, s1 = 0.f, s2 = 0.f, s3 = 0.f;
-#pragma unroll
-            for (int e = 0; e < 32; e += 4) {
-              s0 += s_vr[(e + 0) * 36 + lane];
-              s1 += s_vr[(e + 1) * 36 + lane];
-              s2 += s_vr[(e + 2) * 36 + lane];
-              s3 += s_vr[(e + 3) * 36 + lane];
-            }
-            val = (s0 + s1) + (s2 + s3);
-          }
-          __syncwarp();
-          if (live) p.h[(size_t)i * CBG_H + 32 * pp + lane] = hv[pp] + val;
+          const float y0 = fmaf(v[4 * j + 2 * h] * rs[h], ga.x, be.x), y1 = fmaf(v[4 * j + 2 * h + 1] * rs[h], ga.y, be.y);
+          split_pair_relu(y0, y1, a_hi[j >> 1][2 * (j & 1) + h], a_lo[j >> 1][2 * (j & 1) + h]);
         }
       }
-      if (warp == 0) TC_STAMP(k, 9);
     }
-  } else if (warp >= 12 && warp < 16) {
-    // ===================================== GP: everything tile t needs from outside the tensor pipe, for lane quarter q ==
-    // Warp 12 + q serves node slot q (= TMEM lane quarter q, Pj chunk q) of every tile of this CTA, one tile ahead of S1:
-    //   G     thread = edge row: geometry, edge type, 20 Gaussians (x2h_attention.py:46-52, unitransformer.py:88-99; the
-    //         factor 1024 of the G scale rides in the exponent), (hi, lo) f16, tcgen05.st once MMA1 of the previous tile
-    //         has completed (the G region of TMEM is single-buffered).  G_hi: 48 columns (96 f16), G_lo: 40 columns; type
-    //         block tb occupies columns 10 tb .. 10 tb + 9, the type / node one-hots columns 40 .. 45 of G_hi.
-    //   Pi    the node's Pi row into its K column (84 + q + 4 * tile parity) of the Wg images (hi, lo); the columns of a
-    //         tile parity were last read by MMA1 of tile t - 2, complete once MMA1(t - 1) is (in-order completion)
-    //   Pj    cp.async of the node's 32 Pj rows into chunk q as soon as the quarter's S1 warps have consumed tile t - 1
-    // Every chunk / lane quarter has ONE producer warp that walks the tiles in order (a parity wait is only sound while the
-    // waiter can never be two phases ahead of the barrier).  Indices and coordinates are prefetched 1 - 3 tiles ahead and
-    // consumed one iteration after their load was issued.
-    const int q = warp - 12;
-    const uint32_t t_lane = tmem + ((uint32_t)(32 * q) << 16);
-    const float* rbf = reinterpret_cast<const float*>(smem + SM_RBF);
-    const float c2 = rbf[20] * 1.4426950408889634f;      // exp(c u^2) = 2^(c log2(e) u^2)
-    const float* pj_plane = MODE != MODE_K ? p.pj_v : p.pj_k;
-    const float* pi_plane = MODE != MODE_K ? p.pi_v : p.pi_k;
-    // current tile (t): node, raw neighbour id, coordinates, Pi row piece; stage C = tile t + 1 (loads in flight),
-    // stage B = tile t + 2 (node + neighbour id), stage A = tile t + 3 (node id)
-    int i_t = tile_node(0, q);
-    int jn_t = p.nbr[(size_t)i_t * CBG_KMAX + lane];
-    float4 xi_t = p.x4[i_t], xj_t = p.x4[jn_t >= 0 ? jn_t : i_t];
-    auto load_pi = [&](int i) {      // Pi[i][lane + 32 e], e < 4 (coalesced 128-byte rows)
-      const float* r = pi_plane + (size_t)i * CBG_H + lane;
-      return make_float4(__ldg(r), __ldg(r + 32), __ldg(r + 64), __ldg(r + 96));
-    };
-    float4 pi_t = load_pi(i_t);
-    int iC = 0, jnC = -1, iB = 0, jnB = -1, iA = 0;
-    float4 xiC = xi_t, xjC = xj_t, piC = pi_t;
-    if (n_my > 1) {
-      iC = tile_node(1, q);
-      jnC = p.nbr[(size_t)iC * CBG_KMAX + lane];
-      xiC = p.x4[iC]; xjC = p.x4[jnC >= 0 ? jnC : iC];
-      piC = load_pi(iC);
-    }
-    if (n_my > 2) { iB = tile_node(2, q); jnB = p.nbr[(size_t)iB * CBG_KMAX + lane]; }
-    if (n_my > 3) iA = tile_node(3, q);
-    mbar_wait(bar(B_WFULL), 0u);          // the Pi columns live in the Wg images: the bulk copy must have landed
-    for (int t = 0; t < n_my; ++t) {
-      if (warp == 12) TC_STAMP(t, 14);
-      // ---- G values of this lane's edge row (explicit operation order: position-independent results)
-      uint32_t ghi[10], glo[10];
-      int t_e;
+    TC_STAMP(k, 2);
+    // ---- MMA2 (A from registers) and the epilogue
+    if constexpr (MODE == MODE_K) {
+      // attention weights: <q_i, k> per head (a head's 8 columns = one quad's registers), softmax over the node's 32
+      // edges through shared memory, w = alpha * e_w
+      float qv[32];
       {
-        const float rx = xi_t.x - xj_t.x, ry = xi_t.y - xj_t.y, rz = xi_t.z - xj_t.z;
-        const float d = sqrtf(__fmaf_rn(rz, rz, __fmaf_rn(ry, ry, __fmul_rn(rx, rx))));
-        const int fi = node_flags(xi_t), fj = node_flags(xj_t);
-        t_e = ((fj & 1) ? 0 : 2) + ((fi & 1) ? 0 : 1);
+        const float* qr = p.q + (size_t)i * CBG_H + 2 * qt;
 #pragma unroll
-        for (int mp = 0; mp < 10; ++mp) {
-          const float u0 = d - rbf[2 * mp], u1 = d - rbf[2 * mp + 1];
-          float g0, g1;
-          asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(g0) : "f"(fmaf(c2 * u0, u0, 10.f)));
-          asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(g1) : "f"(fmaf(c2 * u1, u1, 10.f)));
-          split_pair(g0, g1, ghi[mp], glo[mp]);
+        for (int j = 0; j < 16; ++j) { const float2 t = ldg2(qr + 8 * j); qv[2 * j] = t.x; qv[2 * j + 1] = t.y; }
+      }
+      // softmax role: lane = (head, half of the edges); this warp stores edges 16 half + 8 wp .. + 7
+      const int hd = lane & 15, eh = 16 * (lane >> 4);
+      float sc[8];
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const size_t eo = (size_t)i * CBG_KMAX + eh + 8 * wp + j;
+        sc[j] = p.nbr[eo] >= 0 ? p.ew[eo] : 0.f;
+      }
+      float o[64];
+      wgmma_fence();
+#pragma unroll
+      for (int ks = 0; ks < 8; ++ks) wgmma_f16_rs(o, a_lo[ks], d1_hi + 16u * ks, ks > 0 ? 1u : 0u);
+#pragma unroll
+      for (int ks = 0; ks < 8; ++ks) wgmma_f16_rs(o, a_hi[ks], d1_lo + 16u * ks, 1u);
+#pragma unroll
+      for (int ks = 0; ks < 8; ++ks) wgmma_f16_rs(o, a_hi[ks], d1_hi + 16u * ks, 1u);
+      wgmma_commit();
+      wgmma_wait0();
+      wgmma_settle(o);
+      TC_STAMP(k, 3);
+      float* s_sm = s_epi + slot * (32 * 17);              // [edge][17]: conflict-free rows
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        const float l0 = quad_sum(fmaf(o[4 * j + 1], qv[2 * j + 1], o[4 * j] * qv[2 * j]));
+        const float l1 = quad_sum(fmaf(o[4 * j + 3], qv[2 * j + 1], o[4 * j + 2] * qv[2 * j]));
+        if ((j & 3) == qt) {
+          s_sm[e0 * 17 + j] = jn0 >= 0 ? l0 * kInvOut : -INFINITY;
+          s_sm[(e0 + 8) * 17 + j] = jn1 >= 0 ? l1 * kInvOut : -INFINITY;
         }
       }
-      // ---- G rows into TMEM once MMA1(t - 1) has completed
-      if (t >= 1) { mbar_wait(bar(B_ACC1 + ((t - 1) & 1)), (uint32_t)(((t - 1) >> 1) & 1)); tc_fence_after(); }
+      warpgroup_sync(wg);
       {
-        uint32_t w[32];
+        float l[16];
+        float mx = -INFINITY;
 #pragma unroll
-        for (int cc = 0; cc < 32; ++cc) w[cc] = (t_e == cc / 10) ? ghi[cc % 10] : 0u;          // G_hi columns 0 .. 31
-        tmem_st32(t_lane + TM_GHI, w);
-        uint32_t w16[16];
+        for (int j = 0; j < 16; ++j) { l[j] = s_sm[(eh + j) * 17 + hd]; mx = fmaxf(mx, l[j]); }
+        mx = fmaxf(mx, __shfl_xor_sync(CBG_FULL, mx, 16));
+        float sum = 0.f;
 #pragma unroll
-        for (int cc = 0; cc < 8; ++cc) w16[cc] = (t_e == 3) ? ghi[2 + cc] : 0u;                // columns 32 .. 39 (type block 3)
+        for (int j = 0; j < 16; ++j) { l[j] = (mx == -INFINITY) ? 0.f : __expf(l[j] - mx); sum += l[j]; }
+        sum += __shfl_xor_sync(CBG_FULL, sum, 16);
+        const float inv = 1.f / ((sum > 0.f) ? sum : 1.f);
+        if (live) {      // 16 lanes = the 16 heads of one edge: 64-byte rows
+          float* wo = p.w + ((size_t)w_row * CBG_KMAX + eh + 8 * wp) * CBG_HEADS + hd;
 #pragma unroll
-        for (int cc = 0; cc < 8; ++cc) {
-          const int col = 40 + cc;                   // f16 pair (2*col, 2*col + 1): k = 80 .. 95
-          uint32_t val = 0u;
-          if (col == 40) {
-            val = (t_e == 0) ? kHalfTypeOne : ((t_e == 1) ? (kHalfTypeOne << 16) : 0u);
-          } else if (col == 41) {
-            val = (t_e == 2) ? kHalfTypeOne : ((t_e == 3) ? (kHalfTypeOne << 16) : 0u);
-          } else if (col < 46) {
-            const int kc = 84 + q + 4 * (t & 1);
-            val = ((kc >> 1) == col) ? ((kc & 1) ? (kHalfNodeOne << 16) : kHalfNodeOne) : 0u;
-          }
-          w16[8 + cc] = val;
+          for (int j = 0; j < 8; ++j) wo[j * CBG_HEADS] = (wp ? l[8 + j] : l[j]) * inv * sc[j];
         }
-        tmem_st16(t_lane + TM_GHI + 32u, w16);
-#pragma unroll
-        for (int cc = 0; cc < 32; ++cc) w[cc] = (t_e == cc / 10) ? glo[cc % 10] : 0u;          // G_lo columns 0 .. 31
-        tmem_st32(t_lane + TM_GLO, w);
-        uint32_t w8[8];
-#pragma unroll
-        for (int cc = 0; cc < 8; ++cc) w8[cc] = (t_e == 3) ? glo[2 + cc] : 0u;                 // columns 32 .. 39
-        tmem_st8(t_lane + TM_GLO + 32u, w8);
       }
-      tmem_wait_st();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar(B_GREADY));
-      if (warp == 12) TC_STAMP(t, 1);
-      // ---- Pi row of node slot q -> K column 84 + q + 4 * (t & 1) of the Wg images.  Lane = output feature n (+ 32 e):
-      // the elements of a K column are 16 bytes apart inside an 8-row group and the groups alias in the banks, so 32
-      // consecutive n cost 4 wavefronts per store - a lane owning 4 consecutive n cost 16
-      {
-        const int kcol = 84 + q + 4 * (t & 1);
-        const uint32_t cbase = (uint32_t)(kcol >> 3) * 128u + (uint32_t)(kcol & 7) * 2u;
-        const float pv[4] = {pi_t.x, pi_t.y, pi_t.z, pi_t.w};
+    } else if constexpr (IS_V) {
+      // aggregation: (v + b1v) * w summed over the node's 32 edges, h_i +=
+      float wv[2][CBG_HEADS];
 #pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const int nn = lane + 32 * e;
-          const uint32_t off = (uint32_t)(nn >> 3) * WG_SBO + (uint32_t)(nn & 7) * 16u + cbase;
-          const __half hh = __float2half_rn(pv[e]);
-          const __half hl = __float2half_rn(pv[e] - __half2float(hh));
-          *reinterpret_cast<__half*>(smem + SM_WG + off) = hh;
-          *reinterpret_cast<__half*>(smem + SM_WG + WG_IMG + off) = hl;
+      for (int h = 0; h < 2; ++h) {
+        const float* wi = p.w + ((size_t)w_row * CBG_KMAX + e0 + 8 * h) * CBG_HEADS;
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const float4 t = ld4(wi + 4 * j);
+          wv[h][4 * j] = t.x; wv[h][4 * j + 1] = t.y; wv[h][4 * j + 2] = t.z; wv[h][4 * j + 3] = t.w;
         }
-        fence_proxy_async();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(bar(B_PIREADY + (t & 1)));
       }
-      // ---- Pj rows of the node's 32 in-edges into chunk q (one row-coalesced 512-byte copy per instruction)
+      float o[64];
+      wgmma_fence();
+#pragma unroll
+      for (int ks = 0; ks < 8; ++ks) wgmma_f16_rs(o, a_lo[ks], d1_hi + 16u * ks, ks > 0 ? 1u : 0u);
+#pragma unroll
+      for (int ks = 0; ks < 8; ++ks) wgmma_f16_rs(o, a_hi[ks], d1_lo + 16u * ks, 1u);
+#pragma unroll
+      for (int ks = 0; ks < 8; ++ks) wgmma_f16_rs(o, a_hi[ks], d1_hi + 16u * ks, 1u);
+      wgmma_commit();
+      wgmma_wait0();
+      wgmma_settle(o);
+      TC_STAMP(k, 3);
+      float* s_vr = s_epi + (slot * 2 + wp) * CBG_H;       // this warp's 16-edge partial sums
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        const float2 b1 = *reinterpret_cast<const float2*>(s_b1 + 8 * j + 2 * qt);
+        const float sx = rows_sum(fmaf(fmaf(o[4 * j + 2], kInvOut, b1.x), wv[1][j], fmaf(o[4 * j], kInvOut, b1.x) * wv[0][j]));
+        const float sy = rows_sum(fmaf(fmaf(o[4 * j + 3], kInvOut, b1.y), wv[1][j], fmaf(o[4 * j + 1], kInvOut, b1.y) * wv[0][j]));
+        if ((j >> 1) == qg) *reinterpret_cast<float2*>(s_vr + 8 * j + 2 * qt) = make_float2(sx, sy);
+      }
+      warpgroup_sync(wg);
+      if (live) {
+        const int c = 2 * (32 * wp + lane);
+        const float* s0 = s_epi + (slot * 2) * CBG_H + c;
+        float2* hp = reinterpret_cast<float2*>(p.h + (size_t)i * CBG_H + c);
+        const float2 hv = *hp;
+        *hp = make_float2(hv.x + (s0[0] + s0[CBG_H]), hv.y + (s0[1] + s0[CBG_H + 1]));
+      }
+    } else {
+      // H2X coordinate update: s_e = sum_hd w_e,hd (v_e,hd + b1_hd), dx_i = (1/16) sum_e s_e (x_i - x_j)
+      float2 wx[2][2];
+      float rel[2][3];
       {
-        const int jj = jn_t >= 0 ? jn_t : i_t;
-        const int item = 4 * t + q, c = item % NCH;       // the chunk's previous tenant (item - NCH) must have been consumed
-        if (item >= NCH) mbar_wait(bar(B_PJFREE + c), (uint32_t)((item / NCH - 1) & 1));
-        const uint32_t dst = sbase + SM_PJ + (uint32_t)c * PJ_CHUNK + 16u * (uint32_t)(lane & ~7);
-        const uint32_t l7 = (uint32_t)(lane & 7);
-        int jr[32];
+        const float4 xi = p.x4[i];
 #pragma unroll
-        for (int r = 0; r < 32; ++r) jr[r] = __shfl_sync(CBG_FULL, jj, r);       // all shuffles first: no per-row latency chain
+        for (int h = 0; h < 2; ++h) {
+          const float* wi = p.w + ((size_t)w_row * CBG_KMAX + e0 + 8 * h) * CBG_HEADS + 2 * qt;
+          wx[h][0] = *reinterpret_cast<const float2*>(wi);
+          wx[h][1] = *reinterpret_cast<const float2*>(wi + 8);
+          const int jn = h ? jn1 : jn0;       // padded slots: j = i, and their w is zero
+          const float4 xj = p.x4[jn >= 0 ? jn : i];
+          rel[h][0] = xi.x - xj.x; rel[h][1] = xi.y - xj.y; rel[h][2] = xi.z - xj.z;
+        }
+      }
+      float o[8];
+      wgmma_fence();
 #pragma unroll
-        for (int r = 0; r < 32; ++r)
-          cp_async16(dst + (uint32_t)r * PJ_ROW + 16u * (l7 ^ (uint32_t)(r & 7)), pj_plane + (size_t)jr[r] * CBG_H + 4 * lane);
-        cp_async_arrive(bar(B_PJFULL + c));
+      for (int ks = 0; ks < 8; ++ks) wgmma_f16_rs_n16(o, a_lo[ks], d1_hi + 16u * ks, ks > 0 ? 1u : 0u);
+#pragma unroll
+      for (int ks = 0; ks < 8; ++ks) wgmma_f16_rs_n16(o, a_hi[ks], d1_lo + 16u * ks, 1u);
+#pragma unroll
+      for (int ks = 0; ks < 8; ++ks) wgmma_f16_rs_n16(o, a_hi[ks], d1_hi + 16u * ks, 1u);
+      wgmma_commit();
+      wgmma_wait0();
+      wgmma_settle(o);
+      TC_STAMP(k, 3);
+      float se[2];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        float acc = 0.f;
+#pragma unroll
+        for (int j = 0; j < 2; ++j) {
+          const float2 b1 = *reinterpret_cast<const float2*>(s_b1 + 8 * j + 2 * qt);
+          acc = fmaf(fmaf(o[4 * j + 2 * h], kInvOut, b1.x), wx[h][j].x, acc);
+          acc = fmaf(fmaf(o[4 * j + 2 * h + 1], kInvOut, b1.y), wx[h][j].y, acc);
+        }
+        se[h] = quad_sum(acc);
       }
-      if (warp == 12) TC_STAMP(t, 15);
-      // ---- rotate the prefetch stages (every value is consumed one iteration after its load was issued)
-      i_t = iC; jn_t = jnC; xi_t = xiC; xj_t = xjC; pi_t = piC;
-      if (t + 2 < n_my) {
-        iC = iB; jnC = jnB;
-        xiC = p.x4[iB]; xjC = p.x4[jnB >= 0 ? jnB : iB];
-        piC = load_pi(iB);
+      float* s_dx = s_epi + (slot * 2 + wp) * 4;
+#pragma unroll
+      for (int c = 0; c < 3; ++c) {
+        const float a = rows_sum(fmaf(se[1], rel[1][c], se[0] * rel[0][c]));
+        if (lane == 0) s_dx[c] = a;
       }
-      if (t + 3 < n_my) { iB = iA; jnB = p.nbr[(size_t)iA * CBG_KMAX + lane]; }
-      if (t + 4 < n_my) iA = tile_node(t + 4, q);
+      warpgroup_sync(wg);
+      if (live && wp == 0 && lane == 0) {
+        const float* s0 = s_epi + slot * 8;
+        st4(p.dx + 4 * (size_t)n, make_float4((s0[0] + s0[4]) * (1.f / 16.f), (s0[1] + s0[5]) * (1.f / 16.f), (s0[2] + s0[6]) * (1.f / 16.f), 0.f));
+      }
     }
-  } else if (warp == 16) {
-    // ===================================== MMA issuer ============================================================
-    if (lane == 0) {
-      constexpr uint32_t IDESC2 = IS_XV ? IDESC16 : IDESC128;
-      mbar_wait(bar(B_WFULL), 0u);
-      // Descriptors are tile-invariant: build the four bases once; a K step of 16 f16 (two core matrices, 256 bytes)
-      // adds 16 to the 14-bit start-address field, so every MMA below costs one integer add and the issue itself
-      // (the loops are fully unrolled - a rolled loop spends ~100 cycles per MMA on the uniform datapath, which made the
-      // single issuing thread, not the tensor pipe, the limiter of the whole kernel).
-      const uint64_t dg_hi = smem_desc(sbase + SM_WG, LBO, WG_SBO), dg_lo = smem_desc(sbase + SM_WG + WG_IMG, LBO, WG_SBO);
-      const uint64_t d1_hi = smem_desc(sbase + SM_W1, LBO, W1_SBO), d1_lo = smem_desc(sbase + SM_W1 + W1B, LBO, W1_SBO);
-      auto issue_mma2 = [&](int kk) {
-        const int bb = kk & 1;
-        mbar_wait(bar(B_AREADY + bb), (uint32_t)((kk >> 1) & 1));
-        tc_fence_after();
-        TC_STAMP(kk, 12);
-        const uint32_t a_hi = tmem + TM_BUF + 128u * (uint32_t)bb, a_lo = a_hi + 64u;
-        // one N = 128 accumulator: an MMA costs ~64 cycles whether N is 64 or 128 (measured: two N = 64 halves took 3.0K
-        // cycles per tile, twice the N = 128 figure), so the output is not split
-        if (kk > 0) { mbar_wait(bar(B_ACC2FREE), (uint32_t)((kk - 1) & 1)); tc_fence_after(); }
-        else mbar_wait(bar(B_W1FULL), 0u);                      // first use of the W1 images
-        const uint32_t d = tmem + TM_OUT;
-#pragma unroll
-        for (int ks = 0; ks < 8; ++ks)     // small terms first
-          umma_f16_ts(d, a_lo + 8u * ks, d1_hi + 16u * ks, IDESC2, ks > 0 ? 1u : 0u);
-#pragma unroll
-        for (int ks = 0; ks < 8; ++ks) umma_f16_ts(d, a_hi + 8u * ks, d1_lo + 16u * ks, IDESC2, 1u);
-#pragma unroll
-        for (int ks = 0; ks < 8; ++ks) umma_f16_ts(d, a_hi + 8u * ks, d1_hi + 16u * ks, IDESC2, 1u);
-        umma_commit(bar(B_ACC2));
-        TC_STAMP(kk, 13);
-      };
-      for (int k = 0; k < n_my; ++k) {
-        const int b = k & 1;
-        mbar_wait(bar(B_GREADY), (uint32_t)(k & 1));
-        mbar_wait(bar(B_PIREADY + b), (uint32_t)((k >> 1) & 1));
-        tc_fence_after();
-        TC_STAMP(k, 10);
-        const uint32_t d = tmem + TM_BUF + 128u * (uint32_t)b;
-#pragma unroll
-        for (int ks = 0; ks < KG_LO / 16; ++ks)
-          umma_f16_ts(d, tmem + TM_GLO + 8u * ks, dg_hi + 16u * ks, IDESC128, ks > 0 ? 1u : 0u);
-#pragma unroll
-        for (int ks = 0; ks < KG / 16; ++ks) umma_f16_ts(d, tmem + TM_GHI + 8u * ks, dg_lo + 16u * ks, IDESC128, 1u);
-#pragma unroll
-        for (int ks = 0; ks < KG / 16; ++ks) umma_f16_ts(d, tmem + TM_GHI + 8u * ks, dg_hi + 16u * ks, IDESC128, 1u);
-        umma_commit(bar(B_ACC1 + b));
-        TC_STAMP(k, 11);
-        if (k > 0) issue_mma2(k - 1);
-      }
-      issue_mma2(n_my - 1);
-    }
+    TC_STAMP(k, 4);
   }
-  tc_fence_before();
-  __syncthreads();
   TC_STAMP_CTA(2);
-  if (warp == 0) tmem_dealloc(tmem, TM_COLS);
 }
 
 // =================================================================================================================
-// Hardware self-test of the operand conventions the kernel above relies on (A from TMEM with two K-consecutive f16
-// per column, B in the canonical K-major no-swizzle layout, fp32 accumulator read back with tcgen05.ld 32x32b).
-// D[128 x 128] = A[128 x 32] * B[128 x 32]^T, one CTA of 128 threads.  a, b: f16 row-major [128][32]; d: fp32 [128][128].
-__global__ void __launch_bounds__(128, 1) umma_selftest_kernel(const __half* a, const __half* b, float* d, int a_from_smem) {
+// Hardware self-test of the operand conventions the kernels rely on (B in the canonical K-major no-swizzle layout, A
+// through a shared-memory descriptor in the same layout or from registers in the accumulator-compatible fragment layout,
+// fp32 accumulator fragment).  D[128 x 128] = A[128 x 32] * B[128 x 32]^T, one warpgroup, two 64-row halves.
+// a, b: f16 row-major [128][32]; d: fp32 [128][128].
+__global__ void __launch_bounds__(128, 1) wgmma_selftest_kernel(const __half* a, const __half* b, float* d, int a_from_smem) {
   extern __shared__ __align__(1024) uint8_t smem[];
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, qg = lane >> 2, qt = lane & 3;
   constexpr uint32_t SBO = (32 / 8) * 128;        // K = 32: 4 core matrices per 8-row group
   const uint32_t sbase = smem_u32(smem);
-  const uint32_t sb_b = sbase, sb_a = sbase + 128 * 32 * 2, bar0 = sbase + 2 * 128 * 32 * 2;
-  uint32_t* slot = reinterpret_cast<uint32_t*>(smem + 2 * 128 * 32 * 2 + 8);
-  if (warp == 0) tmem_alloc(smem_u32(slot), 256);
-  if (tid == 32) { mbar_init(bar0, 1); fence_mbar_init(); }
+  const uint32_t sb_b = sbase, sb_a = sbase + 128 * 32 * 2;
   for (int e = tid; e < 128 * 32; e += 128) {
     const int r = e >> 5, kk = e & 31;
     const uint32_t off = (uint32_t)(r >> 3) * SBO + (uint32_t)(kk >> 3) * 128u + (uint32_t)(r & 7) * 16u + (uint32_t)(kk & 7) * 2u;
@@ -716,54 +479,43 @@ __global__ void __launch_bounds__(128, 1) umma_selftest_kernel(const __half* a, 
     *reinterpret_cast<__half*>(smem + 128 * 32 * 2 + off) = a[e];
   }
   fence_proxy_async();
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *slot;
-  const uint32_t t_lane = tmem + ((uint32_t)(32 * warp) << 16);
-  if (!a_from_smem) {     // row tid of A -> TMEM columns 128..143 (16 columns = 32 f16)
-    uint32_t w16[16];
-    const uint32_t* arow = reinterpret_cast<const uint32_t*>(a + (size_t)tid * 32);
-#pragma unroll
-    for (int c = 0; c < 16; ++c) w16[c] = arow[c];
-    tmem_st16(t_lane + 128u, w16);
-    tmem_wait_st();
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  if (tid == 0) {
-    for (int ks = 0; ks < 2; ++ks) {
-      if (a_from_smem) umma_f16_ss(tmem, smem_desc(sb_a + 256u * ks, 128, SBO), smem_desc(sb_b + 256u * ks, 128, SBO), idesc_f16(128), ks > 0);
-      else umma_f16_ts(tmem, tmem + 128u + 8u * ks, smem_desc(sb_b + 256u * ks, 128, SBO), idesc_f16(128), ks > 0);
-    }
-    umma_commit(bar0);
-  }
-  mbar_wait(bar0, 0u);
-  tc_fence_after();
 #pragma unroll 1
-  for (int q = 0; q < 4; ++q) {
-    uint32_t r[32];
-    tmem_ld32_nowait(t_lane + 32u * q, r);
-    tmem_wait_ld();
+  for (int half = 0; half < 2; ++half) {
+    const int r0 = 64 * half + 16 * warp + qg;
+    float acc[64];
+    uint32_t af[2][4];
 #pragma unroll
-    for (int j = 0; j < 32; ++j) d[(size_t)tid * 128 + 32 * q + j] = __uint_as_float(r[j]);
+    for (int ks = 0; ks < 2; ++ks) {
+      af[ks][0] = *reinterpret_cast<const uint32_t*>(a + (size_t)r0 * 32 + 16 * ks + 2 * qt);
+      af[ks][1] = *reinterpret_cast<const uint32_t*>(a + (size_t)(r0 + 8) * 32 + 16 * ks + 2 * qt);
+      af[ks][2] = *reinterpret_cast<const uint32_t*>(a + (size_t)r0 * 32 + 16 * ks + 8 + 2 * qt);
+      af[ks][3] = *reinterpret_cast<const uint32_t*>(a + (size_t)(r0 + 8) * 32 + 16 * ks + 8 + 2 * qt);
+    }
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < 2; ++ks) {
+      if (a_from_smem) wgmma_f16_ss(acc, smem_desc(sb_a + (uint32_t)(8 * half) * SBO + 256u * ks, 128, SBO), smem_desc(sb_b + 256u * ks, 128, SBO), ks > 0);
+      else wgmma_f16_rs(acc, af[ks], smem_desc(sb_b + 256u * ks, 128, SBO), ks > 0);
+    }
+    wgmma_commit();
+    wgmma_wait0();
+    wgmma_settle(acc);
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+      *reinterpret_cast<float2*>(d + (size_t)r0 * 128 + 8 * j + 2 * qt) = make_float2(acc[4 * j], acc[4 * j + 1]);
+      *reinterpret_cast<float2*>(d + (size_t)(r0 + 8) * 128 + 8 * j + 2 * qt) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+    }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) tmem_dealloc(tmem, 256);
 }
 
 int g_tc_sms = 0;
-int g_ring_k = 4, g_ring_v = 5;      // Pj ring depths (measured at c2: the attention-weight kernel is fastest with 4, the aggregation kernel with 5)
 long long* g_tc_trace = nullptr;
 int g_tc_trace_tiles = 0;
 
 template <int MODE>
-void launch_tc(int ring, int grid, cudaStream_t st, const EdgeArgs& a, const TcWeights& w) {
-  if (ring == 4) cbg_launch_pdl(x2h_tc_kernel<MODE, 4>, dim3(grid), dim3(544), sm_total(MODE, 4), st, a, w);
-  else if (ring == 5 || MODE == MODE_V) cbg_launch_pdl(x2h_tc_kernel<MODE, 5>, dim3(grid), dim3(544), sm_total(MODE, 5), st, a, w);
-  else cbg_launch_pdl(x2h_tc_kernel<MODE, (MODE == MODE_V ? 5 : 6)>, dim3(grid), dim3(544), sm_total(MODE, MODE == MODE_V ? 5 : 6), st, a, w);
+void launch_tc(int grid, cudaStream_t st, const EdgeArgs& a, const TcWeights& w) {
+  cbg_launch_pdl(x2h_tc_kernel<MODE>, dim3(grid), dim3(256), SM_TOTAL, st, a, w);
 }
 
 int tc_init() {
@@ -773,15 +525,8 @@ int tc_init() {
   int dev = 0;
   CBG_CUDA_OK(cudaGetDevice(&dev));
   CBG_CUDA_OK(cudaDeviceGetAttribute(&g_tc_sms, cudaDevAttrMultiProcessorCount, dev));
-  {
-    const char* e = getenv("CBG_PJ_RING");          // "<k><v>", e.g. 45: ring depth of the attention-weight (4..6) and aggregation (4..5) kernels
-    if (e && e[0] >= '4' && e[0] <= '6') g_ring_k = e[0] - '0';
-    if (e && e[0] && e[1] >= '4' && e[1] <= '5') g_ring_v = e[1] - '0';
-  }
-#define TC_ATTR(MODE, N) CBG_CUDA_OK(cudaFuncSetAttribute(x2h_tc_kernel<MODE, N>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm_total(MODE, N)))
-  TC_ATTR(MODE_K, 4); TC_ATTR(MODE_K, 5); TC_ATTR(MODE_K, 6);
-  TC_ATTR(MODE_V, 4); TC_ATTR(MODE_V, 5);
-  TC_ATTR(MODE_XV, 4); TC_ATTR(MODE_XV, 5); TC_ATTR(MODE_XV, 6);
+#define TC_ATTR(MODE) CBG_CUDA_OK(cudaFuncSetAttribute(x2h_tc_kernel<MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SM_TOTAL))
+  TC_ATTR(MODE_K); TC_ATTR(MODE_V); TC_ATTR(MODE_XV);
 #undef TC_ATTR
   done = true;
   return 0;
@@ -806,10 +551,10 @@ int cbg_launch_x2h_tc(const EdgeArgs& a, cudaStream_t st) {
   const TcWeights wk{L + kOffKW1, L + kOffKWg, L + kOffKLn, nullptr, L + kOffRbf};
   const TcWeights wv{L + kOffVW1, L + kOffVWg, L + kOffVLn, L + kOffVB1, L + kOffRbf};
   CBG_PROF_BEGIN(CBG_K_X2H_K, st);
-  launch_tc<MODE_K>(g_ring_k, grid, st, ak, wk);
+  launch_tc<MODE_K>(grid, st, ak, wk);
   CBG_LAUNCHED(CBG_K_X2H_K, st);
   CBG_PROF_BEGIN(CBG_K_X2H_V, st);
-  launch_tc<MODE_V>(g_ring_v, grid, st, av, wv);
+  launch_tc<MODE_V>(grid, st, av, wv);
   CBG_LAUNCHED(CBG_K_X2H_V, st);
   return 0;
 }
@@ -828,10 +573,10 @@ int cbg_launch_h2x_tc(const EdgeArgs& a, cudaStream_t st) {
   const TcWeights wk{L + kOffXKW1, L + kOffXKWg, L + kOffXKLn, nullptr, L + kOffXRbf};
   const TcWeights wv{L + kOffXVW1, L + kOffXVWg, L + kOffXVLn, L + kOffXVB1, L + kOffXRbf};
   CBG_PROF_BEGIN(CBG_K_H2X, st);
-  launch_tc<MODE_K>(g_ring_k, grid, st, ax, wk);
+  launch_tc<MODE_K>(grid, st, ax, wk);
   CBG_LAUNCHED(CBG_K_H2X, st);
   CBG_PROF_BEGIN(CBG_K_H2X, st);
-  launch_tc<MODE_XV>(g_ring_k, grid, st, ax, wv);
+  launch_tc<MODE_XV>(grid, st, ax, wv);
   CBG_LAUNCHED(CBG_K_H2X, st);
   return 0;
 }
@@ -839,8 +584,8 @@ int cbg_launch_h2x_tc(const EdgeArgs& a, cudaStream_t st) {
 void cbg_x2h_tc_set_trace(long long* buf, int max_tiles) { g_tc_trace = buf; g_tc_trace_tiles = buf ? max_tiles : 0; }
 
 int cbg_launch_umma_selftest(const void* a, const void* b, float* d, int a_from_smem, cudaStream_t st) {
-  const int smem_bytes = 2 * 128 * 32 * 2 + 64;
-  umma_selftest_kernel<<<1, 128, smem_bytes, st>>>((const __half*)a, (const __half*)b, d, a_from_smem);
+  const int smem_bytes = 2 * 128 * 32 * 2;
+  wgmma_selftest_kernel<<<1, 128, smem_bytes, st>>>((const __half*)a, (const __half*)b, d, a_from_smem);
   CBG_CUDA_OK(cudaGetLastError());
   return 0;
 }

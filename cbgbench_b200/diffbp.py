@@ -1,4 +1,4 @@
-"""B200 drop-in for the reference's ``DiffBP`` model, sampling path (SURVEY.md section 8 row f2).
+"""CUDA (H100) drop-in for the reference's ``DiffBP`` model, sampling path (SURVEY.md section 8 row f2).
 
 Mirrors /root/reference repo/models/diffusion/diffbp.py:30-57 (``CoMPredictor`` parameters), :103-130 (constructor,
 sub-module names => state-dict keys) and :240-299 (``sample(batch) -> traj``).  Per step ONE C-ABI call

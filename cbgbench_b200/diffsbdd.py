@@ -1,4 +1,4 @@
-"""B200 drop-in for the reference's ``DiffSBDD`` model, sampling path (SURVEY.md section 8 row f2).
+"""CUDA (H100) drop-in for the reference's ``DiffSBDD`` model, sampling path (SURVEY.md section 8 row f2).
 
 Mirrors /root/reference repo/models/diffusion/diffsbdd.py:25-46 (constructor, sub-module names => state-dict
 keys) and :240-360 (``sample(batch) -> traj``, ``sample_p_xh_given_z0``).  Same denoiser kernels as TargetDiff;

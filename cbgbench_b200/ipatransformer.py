@@ -127,7 +127,7 @@ def pack_ipa_blob(sd, hidden, num_layers, num_x2h, num_classes):
 
 
 class IPATransformerB200(nn.Module):
-    """B200 drop-in for the reference's ``IPATransformer`` (itatransformer.py:14-145)."""
+    """CUDA (H100) drop-in for the reference's ``IPATransformer`` (itatransformer.py:14-145)."""
 
     def __init__(self, cfg):
         super().__init__()

@@ -112,8 +112,8 @@ def _round_tf32(x):
 
 
 def tc_weight_plane(w):
-    """[128 n][128 k] weight (natural nn.Linear layout) -> the tcgen05 operand image:
-    4 K-chunks x (hi | lo) x [128 n][32 k] tf32, each in the UMMA canonical K-major / no-swizzle layout
+    """[128 n][128 k] weight (natural nn.Linear layout) -> the tensor-core operand image:
+    4 K-chunks x (hi | lo) x [128 n][32 k] tf32, each in the canonical K-major / no-swizzle layout
     (8-row x 16-byte core matrices, 128 B apart along K, 1024 B between 8-row groups)."""
     import numpy as np
     w = w.detach().cpu().to(torch.float32).numpy()
@@ -131,7 +131,7 @@ def tc_weight_plane(w):
 
 def tc_f16_image(w):
     """[n][K k] matrix (n = 128, or 16 for the H2X value head; float64, already scaled by its power of two) -> the (hi | lo) f16 operand images of the
-    tcgen05 X2H kernels (csrc/x2h_tc.cu): w ~= hi + lo, each image in the UMMA canonical K-major / no-swizzle layout
+    wgmma X2H kernels (csrc/x2h_tc.cu): w ~= hi + lo, each image in the canonical K-major / no-swizzle layout
     for 16-bit types (8-row x 8-element core matrices, 128 B apart along K, K/8 * 128 B between 8-row groups).
     Returns the raw bits as an int32 tensor (two f16 per word)."""
     import numpy as np
@@ -222,7 +222,7 @@ def pack_denoiser_blob(sd, prefix, num_layers, num_classes, com_head=False):
             # Centre the first Linear of the edge MLPs (X2H and H2X alike) over the OUTPUT-feature axis: LayerNorm follows
             # it directly (common.py:151-171), so pre - mean_f(pre) is all that is ever used, and with
             # W0 <- W0 - mean_f W0, b0 <- b0 - mean_f b0 every piece (Pi, Pj, Wrf g, c) has zero feature mean by
-            # itself.  Exact; the tcgen05 kernels then need only the sum of squares (the SIMT kernels subtract
+            # itself.  Exact; the wgmma kernels then need only the sum of squares (the SIMT kernels subtract
             # a mean that is zero up to rounding).
             w0k, w0v = w0k - w0k.mean(0, keepdim=True), w0v - w0v.mean(0, keepdim=True)
             b0k, b0v = b0k - b0k.mean(), b0v - b0v.mean()
@@ -256,7 +256,7 @@ def pack_denoiser_blob(sd, prefix, num_layers, num_classes, com_head=False):
                 put(base, lf, 'X2H_V_RBF', rbf)
             else:
                 put(base, lf, 'H2X_RBF', rbf)
-            # operand images of the tcgen05 edge kernels (H2X: xv's second Linear has one output per head -> 16 rows)
+            # operand images of the wgmma edge kernels (H2X: xv's second Linear has one output per head -> 16 rows)
             for kv, w0, w1 in (('K', w0k, _t(sd[sp + kname + '.net.3.weight'])),
                                ('V', w0v, _t(sd[sp + vname + '.net.3.weight']))):
                 wg = torch.zeros(HIDDEN, TC_KG, dtype=torch.float64)     # [f][k]: k = 20 t + m | 80 + t | Pi columns
@@ -298,7 +298,7 @@ def graph_ptr_from_batch(batch_idx):
 
 
 class UniTransformerB200(nn.Module):
-    """B200 drop-in for the reference's ``UniTransformer`` (unitransformer.py:12-123)."""
+    """CUDA (H100) drop-in for the reference's ``UniTransformer`` (unitransformer.py:12-123)."""
 
     def __init__(self, cfg):
         super().__init__()

@@ -1,6 +1,6 @@
-"""Sampling driver: the B200 counterpart of the reference's ``sample.py`` loop (SURVEY.md section 8 row f1).
+"""Sampling driver: the CUDA (H100) counterpart of the reference's ``sample.py`` loop (SURVEY.md section 8 row f1).
 
-Mirrors /root/reference sample.py:159-241 for the part that belongs to the hot path: build mini-batches
+Mirrors the reference's sample.py:159-241 for the part that belongs to the hot path: build mini-batches
 of pocket+ligand graphs, ``model.sample(batch)``, take ``traj[0]`` (the state the reference consumes,
 sample.py:194-201), split it per pocket (``split_batch_into_samples``, sample.py:16-32) and collect
 ``{pos, v}`` per ligand.  What stays outside: LMDB/PDB parsing and RDKit/OpenBabel reconstruction (CPU

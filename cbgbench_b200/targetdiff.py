@@ -1,6 +1,6 @@
-"""B200 drop-in for the reference's ``TargetDiff`` model (sampling path).
+"""CUDA (H100) drop-in for the reference's ``TargetDiff`` model (sampling path).
 
-Mirrors /root/reference repo/models/diffusion/targetdiff.py:14-38 (constructor, sub-module
+Mirrors the reference's repo/models/diffusion/targetdiff.py:14-38 (constructor, sub-module
 names => state-dict keys) and :127-184 (``sample(batch) -> traj``).  The Python loop over the
 T diffusion steps stays here (north-star: host code keeps the outer schedule); each iteration
 is ONE C-ABI call (``cbg_sample_step_f32``) that enqueues: ligand embedding -> device kNN ->
@@ -56,7 +56,7 @@ class PLContextEmbedderB200(nn.Module):
             # embedding [N, 1, 128]; "h_lig + t_emb_lig" (context_emb.py:224) then broadcasts h to [N, N, 128] and
             # compose_context raises (common.py:209).  Verified against the live reference (DESIGN.md section 9).
             raise NotImplementedError('time / vec embeddings are not used by any shipped CBGBench config (the reference\'s '
-                                      'own time-embedding path raises a shape error) and are not implemented on the B200 path')
+                                      'own time-embedding path raises a shape error) and are not implemented on the CUDA path')
         atom = cfg_get(cfg, 'atom', None)
         res = cfg_get(cfg, 'residue', None)
         if atom is None or res is None or cfg_get(atom, 'type') != 'linear' or cfg_get(res, 'type') != 'linear':
@@ -107,8 +107,8 @@ class BaseDiffB200(nn.Module):
         # Static lists: atoms without gen_flag never move, so their static-only neighbour lists / edge gates are built
         # once per batch (incremental kNN, cached gates; exact).  On by default wherever the pocket is static.
         self.use_static_lists = self.allow_rcache and os.environ.get('CBG_STATIC_LISTS', '1') != '0'
-        # R-cache (legacy, for the non-tcgen05 X2H kernels only): step-invariant first-Linear terms of static edges,
-        # computed once per batch and streamed from HBM (2*L*N*16 KB).  The default tcgen05 kernels recompute these
+        # R-cache (for the fp32 SIMT X2H kernels only): step-invariant first-Linear terms of static edges,
+        # computed once per batch and streamed from HBM (2*L*N*16 KB).  The default wgmma kernels recompute these
         # terms on the tensor cores and never read it, so it is off unless CBG_RCACHE=1 / use_rcache=True.
         self.use_rcache = self.allow_rcache and os.environ.get('CBG_RCACHE', '0') == '1'
         # receptive-field pruning of the per-step denoiser (exact for the sampled ligand rows)

@@ -1,6 +1,6 @@
-/* cbg_b200 - C-ABI of the B200-native CBGBench diffusion-sampling hot path.
+/* cbg_b200 - C-ABI of the H100-native (sm_90a) CBGBench diffusion-sampling hot path.
  *
- * The reference (EDAPINENUT/CBGBench @ 983fca2, /root/reference) is 100 % Python/PyTorch and
+ * The reference (EDAPINENUT/CBGBench @ 983fca2) is 100 % Python/PyTorch and
  * has NO FFI / plugin / operator boundary of its own (SURVEY.md section 8b): its seam is the Python
  * factory get_e3_gnn() (repo/modules/e3nn/__init__.py:5-18) returning an nn.Module whose
  * forward(x, h, batch_idx, lig_flag, gen_flag) -> (x, h, c) is repo/modules/e3nn/unitransformer.py:102-123,
@@ -52,17 +52,17 @@ int32_t cbg_profile_enable(int32_t on);
 int32_t cbg_profile_collect(double* ms_per_family, int64_t* launches_per_family);
 
 /* TESTING hook (process-wide, not thread-safe; production code never calls it): implementation of the fused X2H / H2X
- * edge kernels.  impl 6 (default): the tcgen05 tile kernel (csrc/x2h_tc.cu: A operands in tensor memory, f16 hi/lo split);
+ * edge kernels.  impl 6 (default): the wgmma tile kernel (csrc/x2h_tc.cu: activations as register A fragments, f16 hi/lo split);
  * impl 0: the fp32 SIMT kernels (csrc/edge.cu), kept as an independent implementation for the parity tests - the only
  * consumer of the optional R-cache.  warps = CTA size of the SIMT kernels (8, 12, 16; 0 keeps the current value).
  * Also env CBG_EDGE_IMPL / CBG_EDGE_WARPS.  Needs a current CUDA device. */
 int32_t cbg_set_edge_impl(int32_t impl, int32_t warps);
-/* Hardware self-test of the tcgen05 operand conventions the X2H kernels rely on (tests only):
+/* Hardware self-test of the wgmma operand conventions the X2H kernels rely on (tests only):
  * d[128][128] (fp32) = a[128][32] * b[128][32]^T with f16 row-major device inputs; a_from_smem = 0 feeds A from
- * tensor memory (tcgen05.st, two K-consecutive f16 per column), 1 from shared memory (canonical K-major layout). */
+ * registers (the accumulator-compatible fragment layout), 1 from shared memory (canonical K-major layout). */
 int32_t cbg_selftest_umma_f16(const void* a, const void* b, float* d, int32_t a_from_smem, void* stream);
-/* Debugging: the next launch of the tcgen05 attention-weight kernel (max_tiles > 0) or aggregation kernel (max_tiles < 0,
- * |max_tiles| rows) stamps the pipeline events of CTA 0 (SM clock) into buf_dev[|max_tiles| + 1][16] (int64, device memory;
+/* Debugging: the next launch of the attention-weight tile kernel (max_tiles > 0) or aggregation kernel (max_tiles < 0,
+ * |max_tiles| rows) stamps the per-tile events of CTA 0 (SM clock; slots 0 - 4: G staged, MMA1, activations, MMA2, epilogue) into buf_dev[|max_tiles| + 1][16] (int64, device memory;
  * the last row takes kernel entry / end of prologue / exit); NULL turns it off.  Process-wide, one-shot. */
 int32_t cbg_debug_x2h_trace(int64_t* buf_dev, int32_t max_tiles);
 /* debug: %globaltimer stamps (ns) of CTA 0 of every following f16 node-GEMM launch into buf_dev[32] (NULL = off):
@@ -139,8 +139,9 @@ int32_t cbg_denoiser_forward_host_f32(const float* blob_host, int64_t blob_float
 /* Node projections of one attention sub-layer alone (testing / integration hook): the five planes
  * [Pj_k, Pj_v, Pi_k, Pi_v, q] of sub-layer `sublayer` (0 = X2H, 1 = H2X) for the listed rows
  * (row_idx NULL = rows 0..n_rows-1), planes = [5][n_nodes][128].  impl 0 = fp32 SIMT kernel,
- * 1 = tcgen05 3xTF32 kernel (warp-specialised, default), 11 = single-issuer variant, 12 / 14 = that variant
- * with weight chunks multicast over clusters of 2 / 4 CTAs.  blob_layer points at the layer's block inside the packed blob.
+ * 1 = wgmma 3xTF32 kernel, 2 = wgmma f16 (hi, lo) kernel (default of the library), 11 / 12 / 14 = the 3xTF32 kernel
+ * with weight chunks multicast over clusters of 1 / 2 / 4 CTAs (1 takes the cluster size from env CBG_GEMM_CLUSTER,
+ * default 1: without that variable 1 and 11 run the same code).  blob_layer points at the layer's block inside the packed blob.
  * Replaces the h-dependent part of MLP.net[0] and hq_func/xq_func (x2h_attention.py:58-83). */
 int32_t cbg_node_proj_f32(const float* blob_layer, int32_t sublayer, int32_t impl, const float* h,
                           const int32_t* row_idx, int32_t n_rows, int64_t n_nodes, float* planes, void* stream);

@@ -20,7 +20,7 @@ restated from its published semantics in ``oracle/graph_ops.py``.
 
 Pinning status: the reference ships no tests, golden vectors or fixtures for this
 path (SURVEY.md section 8c), so the oracle is pinned against outputs of the reference
-itself, imported unchanged in the build container through the shims in
+itself, imported unchanged through the shims in
 ``tests/golden/ref_shims.py``; the generating script is
 ``tests/golden/make_golden.py`` and the fixtures live in ``tests/golden/*.npz``.
 The two [3P] primitives have no reference-side pin (they are definitions).

@@ -1,6 +1,6 @@
 """Generate the golden fixtures from the UNMODIFIED reference (/root/reference).
 
-Run in the build container only (the GPU box has no /root/reference):
+Run where a checkout of the reference exists (tests/golden/ref_shims.py: REF_ROOT):
 
     python tests/golden/make_golden.py
 

@@ -1,5 +1,5 @@
 """Golden for BASELINE.json config 1: the UNMODIFIED reference's TargetDiff.sample on one synthetic pocket
-(200 protein + 24 ligand atoms), T = 50 denoise steps, with injected noise (build container only).
+(200 protein + 24 ligand atoms), T = 50 denoise steps, with injected noise (needs a checkout of the reference).
 
     python tests/golden/make_golden_c1.py      ->  tests/golden/trajectory_c1_T50.npz
 

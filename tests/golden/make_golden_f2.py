@@ -1,6 +1,6 @@
 """Golden fixtures for SURVEY.md section 8 row f2 (DiffSBDD / DiffBP samplers) from the UNMODIFIED reference.
 
-Run in the build container only (the GPU box has no /root/reference):
+Run where a checkout of the reference exists (tests/golden/ref_shims.py: REF_ROOT):
 
     python tests/golden/make_golden_f2.py
 

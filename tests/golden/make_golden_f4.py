@@ -1,7 +1,7 @@
 """Golden fixtures of SURVEY.md section 8 row f4 from the UNMODIFIED reference `IPATransformer`
 (/root/reference repo/modules/e3nn/itatransformer.py), imported through tests/golden/ref_shims.py.
 
-    python tests/golden/make_golden_f4.py          (build container only: the GPU box has no /root/reference)
+    python tests/golden/make_golden_f4.py          (needs a checkout of the reference)
 
 Inputs and weights are regenerated bit-identically by the tests (numpy RandomState seeds below, weights through
 cbgbench_b200.synthetic.seeded_state_dict on the host module, whose state-dict keys equal the reference's: asserted

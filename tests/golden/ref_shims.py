@@ -1,8 +1,8 @@
-"""Import the UNMODIFIED reference (``/root/reference``) in the build container.
+"""Import the UNMODIFIED reference from its checkout (``REF_ROOT`` below).
 
-Used only by the fixture generators ``tests/golden/make_golden*.py`` (build container; the GPU box has
-no ``/root/reference``).  bench.py's reference arms use the staged copy through ``baseline/ref_runner.py``
-instead.  Recipe from SURVEY.md Appendix C:
+Used only by the fixture generators ``tests/golden/make_golden*.py`` (run where the checkout exists).
+bench.py's reference arms use the copy that ``oracle/stage_ref.py`` installs into ``oracle/_ref/``, through
+``baseline/ref_runner.py``, instead.  Recipe from SURVEY.md Appendix C:
 
 * fake ``easydict`` (attr-dict), ``rdkit*`` (MagicMock: only touched at import time by
   repo/utils/molecule/constants.py:3-19);

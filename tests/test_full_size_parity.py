@@ -2,7 +2,7 @@
 64 x (300 + 24) atoms; config 3: 128 pockets, radius graph r = 10, partial generation; config 5: ragged 100-800-atom
 pockets), config 1 against a T = 50 trajectory of the live reference, and a long free-running trajectory.
 
-The oracle is the as-written [E, 340] formulation on the host CPU, so these tests take a few minutes on the GPU box
+The oracle is the as-written [E, 340] formulation on the host CPU, so these tests take a few minutes
 (one oracle forward of config 2 is ~10-30 s); they are what the smaller-shape tests of test_gpu_parity.py cannot show:
 300-atom graphs, 128-graph batches and 800-atom graphs compared element by element.
 """

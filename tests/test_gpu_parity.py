@@ -2,7 +2,7 @@
 
 Bars (BASELINE.json north_star): coordinates / logits within 1e-4 relative fp32
 (max|a-b| / max|b|), integer outputs (neighbour lists, atom-type argmax) bit-exact.
-Run on the B200 box:  python -m pytest tests -m gpu
+Run on an H100:  python -m pytest tests -m gpu
 """
 import ctypes as C
 
@@ -320,7 +320,7 @@ def test_ragged_config5_shape_vs_oracle_subset():
 
 
 # ---------------------------------------------------------------------------------------------
-# node projections: fp32 SIMT kernel and tcgen05 (3xTF32) kernel against a float64 reference
+# node projections: fp32 SIMT kernel and the wgmma (3xTF32, f16 split) kernels against a float64 reference
 @pytest.mark.parametrize('impl', [0, 1, 2, 11, 12, 14],
                          ids=['simt', 'tcgen05-tf32-ws', 'tcgen05-f16', 'tcgen05-single', 'tcgen05-cluster2', 'tcgen05-cluster4'])
 @pytest.mark.parametrize('sublayer', [0, 1], ids=['x2h', 'h2x'])
@@ -490,8 +490,8 @@ def test_sample_driver_single_gpu(tmp_path):
 
 
 # ---------------------------------------------------------------------------------------------
-# the two implementations of the fused X2H edge kernels: tcgen05 (default) and fp32 SIMT (independent cross-check)
-EDGE_IMPLS = {0: 'simt', 6: 'tcgen05'}
+# the two implementations of the fused X2H edge kernels: wgmma (default) and fp32 SIMT (independent cross-check)
+EDGE_IMPLS = {0: 'simt', 6: 'wgmma'}
 
 
 @pytest.fixture
@@ -534,7 +534,7 @@ def test_edge_kernel_implementations_agree(case, edge_impl_reset):
 
 
 def test_edge_kernel_implementations_agree_on_the_sampling_path(edge_impl_reset):
-    """Sampling path (static lists, pruning on): tcgen05 and SIMT kernels give the same atom types and coordinates equal
+    """Sampling path (static lists, pruning on): wgmma and SIMT kernels give the same atom types and coordinates equal
     to rounding; the SIMT kernels also with their R-cache on (streamed first-Linear terms of static edges)."""
     T = 5
     for gen_mode, sizes in (('denovo', ([140, 60, 20], [20, 9, 5])), ('partial', ([90, 70], [18, 12]))):

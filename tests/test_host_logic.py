@@ -82,7 +82,7 @@ def test_packing_places_reference_weights():
     o, n = lay['layer']['X2H_NODE_B']
     nb = blob[base + o: base + o + n]
     assert torch.equal(nb[:256], torch.zeros(256)) and torch.equal(nb[256:384], b0)
-    # f16 (hi | lo) images of the tcgen05 X2H kernels: hi + lo reproduces the scaled fp64 weight to ~2^-22
+    # f16 (hi | lo) images of the wgmma X2H kernels: hi + lo reproduces the scaled fp64 weight to ~2^-22
     import numpy as np
     o, n = lay['layer']['X2H_K_TCWG']
     img = blob.view(torch.int32)[base + o: base + o + n].numpy().view(np.float16)
@@ -104,7 +104,7 @@ def test_packing_places_reference_weights():
                        xk0c[:, 1])
     o, n = lay['layer']['H2X_V_W1']
     assert torch.equal(blob[base + o: base + o + n].view(16, 128), den['blocks.4.h2x_layers.0.xv_func.net.3.weight'])
-    # f16 images of the tcgen05 H2X kernels: the value head's second Linear is a [16 n][128 k] image
+    # f16 images of the wgmma H2X kernels: the value head's second Linear is a [16 n][128 k] image
     o, n = lay['layer']['H2X_V_TCW1']
     assert n == 16 * 128
     img = blob.view(torch.int32)[base + o: base + o + n].numpy().view(np.float16)

@@ -1,5 +1,5 @@
-"""The drop-in seams on the REAL reference (INTEGRATION.md section 2), on the GPU box: the staged copy of the reference
-(baseline/_ref, see baseline/ref_runner.py) is imported unmodified, the ~15-line plugin is applied, and
+"""The drop-in seams on the REAL reference (INTEGRATION.md section 2), on the GPU: the staged copy of the reference
+(oracle/_ref, see oracle/stage_ref.py) is imported unmodified, the ~15-line plugin is applied, and
 
 * seam 1: the reference's own ``TargetDiff`` (its sample() loop, its embedder, its schedulers) runs with
   ``UniTransformerB200`` as the denoiser (``get_e3_gnn`` patched) - same checkpoint keys, same trajectory;
@@ -21,7 +21,7 @@ torch.set_grad_enabled(False)
 def _reference():
     from baseline import ref_runner
     if ref_runner.ref_root() is None:
-        pytest.skip('no staged reference (baseline/_ref) and no /root/reference')
+        pytest.skip('no staged reference (oracle/_ref): build() found no reference checkout to install')
     ref_runner.install()
     return ref_runner
 
@@ -81,7 +81,7 @@ def test_reference_sample_loop_with_b200_denoiser_and_get_model_seam():
     want = OD.sample(sd, batch, T, pn, tu)
     dbatch = {k: (v.to(dev) if torch.is_tensor(v) else v) for k, v in batch.items()}
 
-    # ---- seam 1: reference TargetDiff.sample, B200 denoiser inside
+    # ---- seam 1: reference TargetDiff.sample, the CUDA denoiser inside
     cfg = rr.targetdiff_cfg(T)
     cfg.type = 'targetdiff_ref_loop'
     ref = registry.get_model(cfg)

@@ -1,4 +1,4 @@
-"""tcgen05 X2H kernels (csrc/x2h_tc.cu, edge impl 6): operand-convention self-test on the hardware, parity against the
+"""wgmma X2H tile kernels (csrc/x2h_tc.cu, edge impl 6): operand-convention self-test on the hardware, parity against the
 reference goldens / the fp32 SIMT kernels / the oracle, on the forward and on the sampling path."""
 import numpy as np
 import pytest
@@ -22,10 +22,10 @@ def edge_impl_reset():
     _lib.check(_lib.lib().cbg_set_edge_impl(_lib.DEFAULT_EDGE_IMPL, 0))
 
 
-@pytest.mark.parametrize('a_from_smem', [1, 0], ids=['A_smem', 'A_tmem'])
-def test_umma_f16_operand_conventions(a_from_smem):
-    """D = A B^T with f16 operands on tcgen05: B in the canonical K-major shared-memory layout, A from shared memory or
-    from tensor memory (two K-consecutive f16 per 32-bit column, lane = row), fp32 accumulator read with tcgen05.ld."""
+@pytest.mark.parametrize('a_from_smem', [1, 0], ids=['A_smem', 'A_regs'])
+def test_wgmma_f16_operand_conventions(a_from_smem):
+    """D = A B^T with f16 operands on wgmma: B in the canonical K-major shared-memory layout, A from shared memory or
+    from registers (the accumulator-compatible fragment layout), fp32 accumulator fragment stored row by row."""
     rs = np.random.RandomState(5 + a_from_smem)
     a = rs.normal(size=(128, 32)).astype(np.float16)
     b = rs.normal(size=(128, 32)).astype(np.float16)
@@ -97,14 +97,14 @@ def test_sampling_path_tcgen05_matches_simt(edge_impl_reset):
 
 
 def test_tcgen05_many_tiles_per_cta_and_ragged_tail(edge_impl_reset):
-    """More tiles than SMs (every CTA loops, both TMEM buffers and the whole Pj ring wrap around) and a node count that
-    is not a multiple of the 4-node tile: forward against the SIMT kernels."""
+    """More tiles than SMs (every CTA loops over several tiles) and a node count that is not a multiple of the 4-node
+    tile: forward against the SIMT kernels."""
     L = _lib.lib()
     model, sd = make_model(10, device=dev(), num_layers=2)
     sizes = [300] * 9 + [37]
     batch = synthetic.make_batch(sizes, [24] * 9 + [6], seed=77)
     x, h, bidx, lig, gen = composed_inputs(sd, batch)
-    assert x.shape[0] % 4 != 0 and x.shape[0] // 4 > 3 * 148
+    assert x.shape[0] % 4 != 0 and x.shape[0] // 4 > 3 * 132
     args = [t.to(dev()) for t in (x, h, bidx, lig, gen)]
     outs = {}
     for impl in (0, 6):
@@ -117,7 +117,7 @@ def test_tcgen05_many_tiles_per_cta_and_ragged_tail(edge_impl_reset):
 @pytest.mark.parametrize('gen_mode', ['denovo', 'partial'])
 def test_h2x_tcgen05_matches_simt(gen_mode, edge_impl_reset):
     """H2X on the tile kernel (attention weights into the compact buffer, then the 16-output value head + coordinate
-    update): coordinates after 1, 2 and all layers against the fp32 SIMT h2x_kernel.  > 4 * 148 generated atoms (every
+    update): coordinates after 1, 2 and all layers against the fp32 SIMT h2x_kernel.  > 4 * 132 generated atoms (every
     CTA loops) and a count that is not a multiple of the 4-node tile."""
     L = _lib.lib()
     model, sd = make_model(10, device=dev(), num_layers=3)
@@ -127,7 +127,7 @@ def test_h2x_tcgen05_matches_simt(gen_mode, edge_impl_reset):
     x, h, bidx, lig, gen = composed_inputs(sd, batch)
     n_gen = int(gen.sum())
     if gen_mode == 'denovo':
-        assert n_gen > 4 * 148 and n_gen % 4 != 0
+        assert n_gen > 4 * 132 and n_gen % 4 != 0
     args = [t.to(dev()) for t in (x, h, bidx, lig, gen)]
     outs = {}
     for impl in (0, 6):
@@ -142,9 +142,9 @@ def test_h2x_tcgen05_matches_simt(gen_mode, edge_impl_reset):
 
 
 def test_tcgen05_repeated_runs_are_bit_identical(edge_impl_reset):
-    """The Pj ring, the Pi columns and the TMEM buffers are handed between warps through mbarriers only (cp.async +
-    mbarrier arrive; no bar.sync a race detector could see): a lost hand-over would show up as run-to-run differences.
-    Config-2-sized forward (every CTA loops ~35 times), 8 repeats, outputs must be bit-identical."""
+    """The G rows and the per-node partial results are handed between the warps of a warpgroup through shared memory and
+    named barriers, and every sum has a fixed order: a lost hand-over would show up as run-to-run differences.
+    Config-2-sized forward (every CTA loops ~40 times), 8 repeats, outputs must be bit-identical."""
     model, sd = make_model(10, device=dev(), num_layers=3)
     batch = synthetic.make_batch([300] * 64, [24] * 64, seed=2024)
     x, h, bidx, lig, gen = composed_inputs(sd, batch)
