@@ -53,7 +53,11 @@ def cuda_neighbors(x, batch_idx, k=32, mode=0, r_max=10.0):
 
 # ---------------------------------------------------------------------------------------------
 # stage: neighbour lists (bit-exact)
-@pytest.mark.parametrize('sizes', [[224], [299, 25, 1, 2, 33, 32], [850, 100, 450]])
+# A graph above 3 072 atoms (48 KB of float4 coordinates) needs the kNN kernel's opt-in dynamic shared memory.
+LARGE_GRAPH_BATCH = [3500, 40, 7]
+
+
+@pytest.mark.parametrize('sizes', [[224], [299, 25, 1, 2, 33, 32], [850, 100, 450], LARGE_GRAPH_BATCH])
 @pytest.mark.parametrize('k', [32, 8])
 def test_knn_bit_exact(sizes, k):
     from oracle import graph_ops as G
@@ -69,14 +73,31 @@ def test_knn_bit_exact(sizes, k):
 
 def test_radius_graph_bit_exact():
     from oracle import graph_ops as G
-    rs = np.random.RandomState(9)
-    sizes = [300, 120]
-    x = torch.from_numpy((6.0 * rs.normal(size=(sum(sizes), 3))).astype(np.float32))
-    bidx = torch.repeat_interleave(torch.arange(2), torch.tensor(sizes))
-    want = G.neighbor_table(x, [0, 300, 420], k=32, r_max=6.0)
-    got = cuda_neighbors(x, bidx, k=32, mode=1, r_max=6.0)
-    assert torch.equal(got, want)
-    assert (want == -1).any() and (want[:, 0] >= 0).any()
+    for sizes in ([300, 120], LARGE_GRAPH_BATCH):
+        rs = np.random.RandomState(9)
+        x = torch.from_numpy((6.0 * rs.normal(size=(sum(sizes), 3))).astype(np.float32))
+        bidx = torch.repeat_interleave(torch.arange(len(sizes)), torch.tensor(sizes))
+        want = G.neighbor_table(x, [0] + list(np.cumsum(sizes)), k=32, r_max=6.0)
+        got = cuda_neighbors(x, bidx, k=32, mode=1, r_max=6.0)
+        assert torch.equal(got, want), sizes
+        assert (want == -1).any() and (want[:, 0] >= 0).any(), sizes
+
+
+def test_knn_rejects_graph_over_shared_memory_limit():
+    """The neighbour search holds one graph's coordinates in shared memory (200 KB, 12 800 atoms): a larger graph is
+    refused on the host with an error, before any launch."""
+    L = _lib.lib()
+    sizes = [12801, 5]
+    N = sum(sizes)
+    x = torch.zeros((N, 3), dtype=torch.float32, device=dev())
+    gptr = torch.tensor([0, sizes[0], N], dtype=torch.int32, device=dev())
+    nbr = torch.full((N, 32), -7, dtype=torch.int32, device=dev())
+    buf, wsp, wsb = _ws(N)
+    rc = L.cbg_build_neighbors_f32(x.data_ptr(), gptr.data_ptr(), 2, N, max(sizes), 0, 32, 10.0, nbr.data_ptr(), wsp, wsb, None)
+    torch.cuda.synchronize()
+    assert rc != 0
+    assert b'12801 atoms exceeds the 12800-atom shared-memory limit' in L.cbg_last_error()
+    assert bool((nbr == -7).all())                     # nothing was written
 
 
 # ---------------------------------------------------------------------------------------------
@@ -149,6 +170,23 @@ def test_forward_radius_mode_vs_oracle():
     xo, ho, co = ODn.unitransformer_forward(sd, x, h, bidx, lig, gen, cutoff_mode='radius', r_max=9.0)
     xg, hg, cg = model.denoiser(x.to(dev()), h.to(dev()), bidx.to(dev()), lig.to(dev()), gen.to(dev()))
     assert rel_err(xg.cpu(), xo) < TOL and rel_err(hg.cpu(), ho) < TOL and rel_err(cg.cpu(), co) < TOL
+
+
+@pytest.mark.parametrize('enc', [{}, {'cutoff_mode': 'radius', 'r_max': 9.0}], ids=['knn', 'radius9'])
+def test_forward_with_large_graph_vs_oracle(enc):
+    """A 2-layer forward on a batch with one 3 500-atom pocket (the neighbour search's opt-in shared-memory path)."""
+    from oracle import denoiser as ODn
+    model, sd = make_model(10, device=dev(), num_layers=2, **enc)
+    batch = synthetic.make_batch([3476, 60], [24, 12], seed=33)
+    x, h, bidx, lig, gen = composed_inputs(sd, batch)
+    assert int(torch.bincount(bidx).max()) == 3500
+    xo, ho, co = ODn.unitransformer_forward(sd, x, h, bidx, lig, gen, cutoff_mode=enc.get('cutoff_mode', 'knn'),
+                                            r_max=enc.get('r_max', 10.0))
+    xg, hg, cg = model.denoiser(x.to(dev()), h.to(dev()), bidx.to(dev()), lig.to(dev()), gen.to(dev()))
+    for name, a, b in (('x', xg, xo), ('h', hg, ho), ('c', cg, co)):
+        err = rel_err(a.cpu(), b)
+        assert err < TOL, f'{name}: rel err {err:.2e}'
+    assert torch.equal(xg.cpu()[~gen], x[~gen])
 
 
 def test_forward_host_buffers_equals_device_path():
@@ -321,19 +359,35 @@ def test_ragged_config5_shape_vs_oracle_subset():
 
 # ---------------------------------------------------------------------------------------------
 # node projections: fp32 SIMT kernel and the wgmma (3xTF32, f16 split) kernels against a float64 reference
+# (n_nodes, which rows): 'all' = rows 0..n-1 (row_idx NULL), 'sorted' / 'unsorted' = 150 listed rows, 'none' = n_rows 0.
+# The wgmma kernels work in 64-row warpgroups of 128-row CTAs, so 64 / 65 / 128 / 129 rows sit on either side of a
+# warpgroup and a CTA edge; 257 rows fill three CTAs, which leaves the last cluster of 2 or 4 CTAs partly padded.
+NODE_PROJ_ROWS = {'n1': (1, 'all'), 'n64': (64, 'all'), 'n65': (65, 'all'), 'n128': (128, 'all'), 'n129': (129, 'all'),
+                  'n257': (257, 'all'), 'n333': (333, 'all'), 'n333-sorted': (333, 'sorted'),
+                  'n333-unsorted': (333, 'unsorted'), 'none': (64, 'none')}
+
+
 @pytest.mark.parametrize('impl', [0, 1, 2, 11, 12, 14],
-                         ids=['simt', 'tcgen05-tf32-ws', 'tcgen05-f16', 'tcgen05-single', 'tcgen05-cluster2', 'tcgen05-cluster4'])
+                         ids=['simt', 'wgmma-tf32', 'wgmma-f16', 'wgmma-tf32-cluster1', 'wgmma-tf32-cluster2',
+                              'wgmma-tf32-cluster4'])
 @pytest.mark.parametrize('sublayer', [0, 1], ids=['x2h', 'h2x'])
-def test_node_projections_match_float64(impl, sublayer):
+@pytest.mark.parametrize('rows', list(NODE_PROJ_ROWS))
+def test_node_projections_match_float64(impl, sublayer, rows):
     model, sd = make_model(10, device=dev())
     L = _lib.lib()
     lay = _lib.blob_layout()
     blob = model.denoiser.packed_blob(dev())
     layer = 3
     rs = np.random.RandomState(17)
-    N = 333                                              # not a multiple of the 64/128-row tiles
+    N, kind = NODE_PROJ_ROWS[rows]
     h = torch.from_numpy((1.5 * rs.normal(size=(N, 128))).astype(np.float32))
-    rows = torch.from_numpy(np.sort(rs.choice(N, size=150, replace=False)).astype(np.int32))
+    subset = rs.choice(N, size=150, replace=False) if kind in ('sorted', 'unsorted') else None
+    row_idx = None
+    if kind == 'sorted':
+        row_idx = torch.from_numpy(np.sort(subset).astype(np.int32))
+    elif kind == 'unsorted':
+        row_idx = torch.from_numpy(subset.astype(np.int32))
+        assert not bool((row_idx[1:] > row_idx[:-1]).all())
     hd = h.to(dev())
     base_ptr = blob.data_ptr() + 4 * (lay['global_floats'] + layer * lay['layer_floats'])
     pre = f'denoiser.blocks.{layer}.' + ('x2h_layers.0.' if sublayer == 0 else 'h2x_layers.0.')
@@ -349,21 +403,23 @@ def test_node_projections_match_float64(impl, sublayer):
     qh = F.layer_norm(h64 @ d(qn + '.net.0.weight').T + d(qn + '.net.0.bias'), (128,), d(qn + '.net.1.weight'),
                       d(qn + '.net.1.bias'), 1e-5).relu()
     want.append((qh @ d(qn + '.net.3.weight').T + d(qn + '.net.3.bias')) / np.sqrt(8.0))
-    for row_idx in (None, rows):
-        planes = torch.full((5, N, 128), float('nan'), device=dev())
-        ridx = row_idx.to(dev()) if row_idx is not None else None
-        n_rows = N if row_idx is None else int(row_idx.numel())
-        _lib.check(L.cbg_node_proj_f32(base_ptr, sublayer, impl, hd.data_ptr(), ridx.data_ptr() if ridx is not None else None,
-                                       n_rows, N, planes.data_ptr(), None))
-        torch.cuda.synchronize()
-        sel = slice(None) if row_idx is None else row_idx.long()
-        for p in range(5):
-            err = rel_err(planes[p].cpu()[sel], want[p][sel])
-            assert err < 2e-6, f'impl {impl} sublayer {sublayer} plane {p}: rel err {err:.2e}'
-        if row_idx is not None:                                   # rows not listed stay untouched
-            mask = torch.ones(N, dtype=torch.bool)
-            mask[row_idx.long()] = False
-            assert torch.isnan(planes.cpu()[:, mask]).all()
+    planes = torch.full((5, N, 128), float('nan'), device=dev())
+    ridx = row_idx.to(dev()) if row_idx is not None else None
+    n_rows = 0 if kind == 'none' else (N if row_idx is None else int(row_idx.numel()))
+    assert L.cbg_node_proj_f32(base_ptr, sublayer, impl, hd.data_ptr(), ridx.data_ptr() if ridx is not None else None,
+                               n_rows, N, planes.data_ptr(), None) == 0, L.cbg_last_error()
+    torch.cuda.synchronize()
+    if kind == 'none':                                            # nothing to do: every plane stays untouched
+        assert torch.isnan(planes.cpu()).all()
+        return
+    sel = slice(None) if row_idx is None else row_idx.long()
+    for p in range(5):
+        err = rel_err(planes[p].cpu()[sel], want[p][sel])
+        assert err < 2e-6, f'impl {impl} sublayer {sublayer} plane {p}: rel err {err:.2e}'
+    if row_idx is not None:                                       # rows not listed stay untouched
+        mask = torch.ones(N, dtype=torch.bool)
+        mask[row_idx.long()] = False
+        assert torch.isnan(planes.cpu()[:, mask]).all()
 
 
 def test_rcache_matches_uncached_path(edge_impl_reset):
@@ -503,8 +559,9 @@ def edge_impl_reset():
 
 @pytest.mark.parametrize('case', FORWARD_CASES, ids=[c[0] for c in FORWARD_CASES])
 def test_edge_kernel_implementations_agree(case, edge_impl_reset):
-    """Both implementations of the X2H kernels (and the SIMT kernels at every CTA size) must match the reference golden
-    and each other."""
+    """Both implementations of the X2H kernels (the SIMT ones at every CTA size) must match the reference golden and
+    each other.  cbg_set_edge_impl sets the CTA size of the SIMT X2H kernels only, so with impl 0 the SIMT H2X kernel
+    runs at its default 12 warps; its other CTA sizes are covered by tests/test_kernel_variants.py (CBG_H2X_WARPS)."""
     name, n_prot, n_lig, seed, gen_mode, enc = case
     gold = golden('forward_cases.npz')
     model, sd = make_model(10, device=dev(), **enc)
