@@ -34,6 +34,17 @@ class StepCoef(C.Structure):
     ]
 
 
+class EvalCoef(C.Structure):
+    _fields_ = [
+        ('alphas_cumprod', C.c_float), ('log_alphas_cumprod', C.c_float), ('log_one_minus_alphas_cumprod', C.c_float),
+        ('log_alphas_cumprod_prev', C.c_float), ('log_one_minus_alphas_cumprod_prev', C.c_float),
+        ('log_alpha', C.c_float), ('log_one_minus_alpha', C.c_float), ('t_is_zero', C.c_int32),
+    ]
+
+
+EVAL_MAX_REPLICAS = 64     # replicas per cbg_eval_loss_f32 call (csrc/cbg_kernels.cuh: CBG_EVAL_MAX_REPLICAS)
+
+
 class SbddCoef(C.Structure):
     _fields_ = [('a', C.c_float), ('b', C.c_float), ('s', C.c_float), ('mode', C.c_int32)]
 
@@ -78,6 +89,7 @@ SIGNATURES = {
     'cbg_sample_step_f32': (_I32, [C.POINTER(SamplePlan), C.POINTER(StepCoef), _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     'cbg_sample_step_graph_f32': (_I32, [C.POINTER(SamplePlan), C.POINTER(StepCoef), _P, _P, _P, _P, _P, _P, _P, _P]),
     'cbg_sample_step_graph_nodes': (_I64, [C.POINTER(SamplePlan), _P]),
+    'cbg_eval_loss_f32': (_I32, [C.POINTER(SamplePlan), C.POINTER(EvalCoef), _I32, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     'cbg_sbdd_step_f32': (_I32, [C.POINTER(SamplePlan), C.POINTER(SbddCoef), _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     'cbg_bp_step_f32': (_I32, [C.POINTER(SamplePlan), _P, _I32, C.POINTER(BpCoef), _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     'cbg_pocket_stats_f32': (_I32, [_P, _P, _I32, _P, _P, _I32, _P, _P, _P]),

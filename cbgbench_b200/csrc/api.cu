@@ -891,6 +891,45 @@ int32_t cbg_reverse_step_f32(const cbg_step_coef* coef, const float* x0_pred, co
   return cbg_launch_reverse(r, coef->pos_logvar, coef->pos_nonzero, (cudaStream_t)stream);
 }
 
+int32_t cbg_eval_loss_f32(const cbg_sample_plan* plan, const cbg_eval_coef* coefs, int32_t n_rep, const float* x0,
+                          const int64_t* v0, const float* pos_noise, const float* type_uniform, float* xt, int64_t* vt,
+                          float* x_pred, float* c_pred, float* graph_loss, float* rep_loss, void* stream) {
+  if (!plan || !coefs || !x0 || !v0 || !pos_noise || !type_uniform || !xt || !vt || !x_pred || !c_pred || !graph_loss || !rep_loss) {
+    cbg_set_error("cbg_eval_loss_f32: null argument"); return 1;
+  }
+  if (n_rep < 1 || n_rep > CBG_EVAL_MAX_REPLICAS) { cbg_set_error("n_rep=%d outside [1,%d]", n_rep, CBG_EVAL_MAX_REPLICAS); return 1; }
+  if (plan->n_lig < n_rep || plan->n_lig % n_rep || plan->n_graphs % n_rep) {
+    cbg_set_error("plan (n_lig=%d, n_graphs=%d) is not %d replicas of one batch", plan->n_lig, plan->n_graphs, n_rep); return 1;
+  }
+  NvtxRange nvtx_eval("cbg:eval_loss");
+  Workspace ws;
+  if (int rc = check_ws(plan->workspace, plan->workspace_bytes, plan->n_nodes, plan->n_gen, &ws)) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  const int K = plan->num_classes;
+  if (K < 1 || K > CBG_MAXCLS) { cbg_set_error("num_classes=%d outside [1,%d]", K, CBG_MAXCLS); return 1; }
+  EvalArgs e{};
+  for (int r = 0; r < n_rep; ++r) {
+    const cbg_eval_coef& c = coefs[r];
+    e.coef.c[r] = EvalCoefDev{c.alphas_cumprod, c.log_alphas_cumprod, c.log_one_minus_alphas_cumprod, c.log_alphas_cumprod_prev,
+                              c.log_one_minus_alphas_cumprod_prev, c.log_alpha, c.log_one_minus_alpha, c.t_is_zero ? 1 : 0};
+  }
+  e.n_rep = n_rep; e.n_lig = plan->n_lig; e.n_graphs = plan->n_graphs; e.num_classes = K;
+  e.lig_node = plan->lig_node; e.graph_ptr = plan->graph_ptr; e.gen = plan->gen_lig;
+  e.x0 = x0; e.v0 = (const long long*)v0; e.pos_noise = pos_noise; e.type_u = type_uniform;
+  e.emb_wt = plan->emb_wt; e.h_lig_bias = plan->h_lig_bias;
+  e.x4 = ws.x4; e.h = ws.h; e.xt = xt; e.vt = (long long*)vt; e.x_pred = x_pred; e.c_pred = c_pred;
+  e.logits = ws.w;                  // classifier scratch: the attention-weight buffer is free after the layers
+  e.graph_cnt = (int*)ws.ew;        // so is the edge-gate buffer (n_nodes * 32 >= n_graphs entries)
+  e.graph_loss = graph_loss; e.rep_loss = rep_loss;
+  CBG_CUDA_OK(cudaMemcpyAsync(ws.h, plan->h_static, (size_t)plan->n_nodes * CBG_H * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  if (int rc = cbg_launch_eval_noise(e, st)) return rc;
+  if (int rc = run_core(plan->blob, plan->num_layers, ws, plan->graph_ptr, plan->n_graphs, plan->max_graph_nodes,
+                        plan->n_nodes, plan->gen_node, plan->n_gen, plan->mode, plan->k, plan->r_max, plan->rcache,
+                        plan->lig_node, plan->n_lig, plan->prune != 0 && prune_enabled(), st, plan->static_lists != 0)) return rc;
+  if (int rc = cbg_launch_classifier(plan->blob, ws.h, plan->lig_node, plan->n_lig, K, ws.w, st)) return rc;
+  return cbg_launch_eval_loss(e, st);
+}
+
 // ---- row f3: device-side batch construction ---------------------------------------------------------------------
 int32_t cbg_pocket_stats_f32(const float* prot_pos, const int32_t* prot_ptr, int32_t n_pockets, const float* ctx_pos,
                              const int32_t* ctx_ptr, int32_t centre_mode, float* space_size, float* centre, void* stream) {

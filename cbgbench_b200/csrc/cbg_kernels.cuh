@@ -147,6 +147,41 @@ int cbg_launch_step_init_io(const StepIO* io, const int* lig_node, int n_lig, in
 // the step-invariant members of `a` are used, the per-step ones (x_t, c_t, noise, outputs, coefficients) come from *io
 int cbg_launch_reverse_io(const ReverseArgs& a, const StepIO* io, cudaStream_t st);
 
+// eval.cu: TargetDiff validation loss over R replicas of a batch (cbg_eval_loss_f32).  The plan's ligand atoms and graphs
+// are replica-major: atom i belongs to replica i / (n_lig / n_rep) and is atom i % (n_lig / n_rep) of the batch.
+constexpr int CBG_EVAL_MAX_REPLICAS = 64;
+struct EvalCoefDev {       // same members as cbg_eval_coef (include/cbg_b200.h)
+  float alphas_cumprod, lac, l1mac, lac_prev, l1mac_prev, la, l1ma;
+  int t_is_zero;
+};
+struct EvalCoefs { EvalCoefDev c[CBG_EVAL_MAX_REPLICAS]; };   // passed by value: no H2D copy per call
+struct EvalArgs {
+  EvalCoefs coef;
+  int n_rep, n_lig, n_graphs, num_classes;   // n_lig / n_graphs: replicated totals
+  const int* lig_node;       // [n_lig] ascending composed node index
+  const int* graph_ptr;      // [n_graphs+1]
+  const unsigned char* gen;  // [n_lig] replicated ligand_gen_flag
+  const float* x0;           // [n_lig/n_rep,3]
+  const long long* v0;       // [n_lig/n_rep]
+  const float* pos_noise;    // [n_lig,3]
+  const float* type_u;       // [n_lig,K]
+  const float* emb_wt;       // [K,128]
+  const float* h_lig_bias;   // [n_lig,128]
+  const float* logits;       // [n_lig,K] classifier output (loss kernel)
+  float4* x4;                // node coordinates + flags
+  float* h;                  // [N,128] node features
+  float* xt;                 // [n_lig,3]
+  long long* vt;             // [n_lig]
+  float* x_pred;             // [n_lig,3]
+  float* c_pred;             // [n_lig,K]
+  float* graph_loss;         // [n_graphs,2] per-graph (pos, atom) means over generated atoms (0 without any)
+  int* graph_cnt;            // [n_graphs] generated atoms per graph (scratch)
+  float* rep_loss;           // [n_rep,2]
+};
+int cbg_launch_eval_noise(const EvalArgs& a, cudaStream_t st);
+// eval_loss_kernel (one CTA per graph) followed by eval_reduce_kernel (one thread per replica)
+int cbg_launch_eval_loss(const EvalArgs& a, cudaStream_t st);
+
 // DiffSBDD reverse step (SURVEY.md section 8 row f2): one CTA per graph.
 //   mode 0  zs = z_t / a - b * eps_pred + s * noise              (sample_p_zs_given_zt, diffusion_scheduler.py:1005-1039)
 //   mode 1  zs = a * (z_t - b * eps_pred) + s * noise            (sample_p_xh_given_z0, diffsbdd.py:323-360; a = 1/alpha_0)

@@ -11,10 +11,14 @@ the compose_context permutation, graph offsets, flag arrays.
 Random numbers are drawn with torch on the model device in the reference's order
 (positions ``randn_like`` then types ``rand_like``, diffusion_scheduler.py:158-163 /
 categorical.py:27), or injected for parity tests.
+
+The eval-mode ``forward(batch)`` (targetdiff.py:41-124, the validation loss) is built too: ``eval_losses`` runs the
+noised copies of the batch for all its timesteps through ONE C-ABI call (``cbg_eval_loss_f32``, DESIGN.md section 13).
 """
 import ctypes as C
 import os
 
+import numpy as np
 import torch
 from torch import nn
 import torch.nn.functional as F
@@ -39,6 +43,25 @@ def register_model(name):
 def get_model(config):
     """Mirror of repo/models/_base.py:10-12."""
     return _MODEL_DICT[config.type](config)
+
+
+def eval_t_values(num_timesteps, eval_interval=10):
+    """Timesteps of the reference's eval-mode forward (targetdiff.py:67-71): ``np.linspace(0, T-1, eval_interval)``,
+    each truncated toward zero by ``torch.tensor([t] * B).long()``.  T = 50 gives [0, 5, 10, 16, 21, 27, 32, 38, 43, 49]."""
+    return [int(t) for t in np.linspace(0, num_timesteps - 1, eval_interval).astype(np.int64)]
+
+
+def replicate_batch(batch, n_rep, n_graphs):
+    """``n_rep`` copies of a batch (dict of tensors) as one batch of n_rep * n_graphs graphs: every tensor is tiled along
+    dim 0 and copy r's graph ids are offset by r * n_graphs, so the copies stay replica-major and sorted."""
+    out = {}
+    for k, t in batch.items():
+        if k in ('ligand_element_batch', 'protein_element_batch'):
+            off = torch.arange(n_rep, device=t.device, dtype=t.dtype).unsqueeze(1) * n_graphs
+            out[k] = (t.unsqueeze(0) + off).reshape(-1)
+        else:
+            out[k] = t.repeat(n_rep, *([1] * (t.dim() - 1)))
+    return out
 
 
 class PLContextEmbedderB200(nn.Module):
@@ -131,8 +154,8 @@ class BaseDiffB200(nn.Module):
                                'belongs to the newer batch); finish one batch before preparing the next, or use a second model')
 
     def forward(self, batch):
-        raise NotImplementedError(f'{type(self).__name__} is a forward-only sampling build: the training / '
-                                  'validation losses of the reference models are out of scope (DESIGN.md)')
+        raise NotImplementedError(f'{type(self).__name__} is a sampling build: the training / validation losses of this '
+                                  'model are not implemented on the CUDA path (DESIGN.md section 9)')
 
     # ---- setup of the step-invariant state ------------------------------------------------
     @torch.no_grad()
@@ -249,6 +272,107 @@ class TargetDiffB200(BaseDiffB200):
             log_one_minus_alphas_cumprod_prev=float(ts.host_table('log_one_minus_alphas_cumprod_v')[tm1]),
             log_alpha=float(ts.host_table('log_alphas_v')[t_idx]),
             log_one_minus_alpha=float(ts.host_table('log_one_minus_alphas_v')[t_idx]))
+
+    # ---- validation loss (TargetDiff.forward with self.training == False) -------------------------------------------
+    eval_max_nodes = 1 << 20    # composed nodes per cbg_eval_loss_f32 launch (about 9 GB of workspace at ~8.5 KB/node)
+
+    def forward(self, batch, pos_noise=None, type_uniform=None):
+        """TargetDiff.forward (targetdiff.py:41-80).  Eval mode only: returns ``(loss_dict, results)`` for the
+        ``eval_interval`` (default 10) timesteps ``np.linspace(0, T-1, eval_interval)`` truncated to integers, exactly
+        like the reference; see ``eval_losses``.  Training mode needs autograd through the denoiser and raises."""
+        if self.training:
+            raise NotImplementedError(f'{type(self).__name__}.forward in training mode needs autograd through the '
+                                      'denoiser, which the CUDA path does not provide: training is out of scope '
+                                      '(call model.eval() for the validation losses)')
+        t_values = eval_t_values(self.num_diffusion_timesteps, cfg_get(self.cfg, 'eval_interval', 10))
+        return self.eval_losses(batch, t_values, pos_noise=pos_noise, type_uniform=type_uniform)
+
+    def eval_coef(self, t_idx):
+        ps, ts = self.pos_scheduler, self.type_scheduler
+        tm1 = max(t_idx - 1, 0)
+        tab = ts.host_table
+        return _lib.EvalCoef(
+            alphas_cumprod=float(ps.host_table('alphas_cumprod')[t_idx]),
+            log_alphas_cumprod=float(tab('log_alphas_cumprod_v')[t_idx]),
+            log_one_minus_alphas_cumprod=float(tab('log_one_minus_alphas_cumprod_v')[t_idx]),
+            log_alphas_cumprod_prev=float(tab('log_alphas_cumprod_v')[tm1]),
+            log_one_minus_alphas_cumprod_prev=float(tab('log_one_minus_alphas_cumprod_v')[tm1]),
+            log_alpha=float(tab('log_alphas_v')[t_idx]),
+            log_one_minus_alpha=float(tab('log_one_minus_alphas_v')[t_idx]),
+            t_is_zero=1 if t_idx == 0 else 0)
+
+    @torch.no_grad()
+    def eval_losses(self, batch, t_values, pos_noise=None, type_uniform=None, max_nodes=None):
+        """Validation losses of ``batch`` at the timesteps ``t_values`` (TargetDiff.get_loss, targetdiff.py:82-124, once
+        per t).  Returns ``(loss_dict, results)`` like the reference's eval-mode forward: ``loss_dict`` = {'pos', 'atom'}
+        as CPU 0-d float32 tensors (mean over t of the per-t losses), ``results`` one dict per t with the device tensors
+        x0, xt, x_pred, mask_gen, v0, vt, c_pred.  A t whose batch has no generated atom gets NaN losses, like the
+        reference's mean of an empty tensor.
+
+        The denoiser is not conditioned on t, so the R = len(t_values) noised copies of the batch go through ONE
+        denoiser pass as R*B graphs.  When R copies would exceed ``max_nodes`` composed nodes (default
+        ``eval_max_nodes``), or more than 64 replicas are asked for, the replicas are split over several launches; graphs
+        are processed independently, so the split does not change any result bit.
+
+        ``pos_noise`` [R,n_lig,3] / ``type_uniform`` [R,n_lig,K] inject the draws; by default they are drawn with torch on
+        the model device in the reference's order (for each t: randn [n_lig,3], then rand [n_lig,K])."""
+        t_values = [int(t) for t in t_values]
+        R, T, K = len(t_values), self.num_diffusion_timesteps, self.num_classes
+        if R == 0:
+            raise ValueError('t_values is empty')
+        if any(t < 0 or t >= T for t in t_values):
+            raise ValueError(f't_values must lie in [0, {T - 1}]')
+        dev = next(self.parameters()).device
+        if dev.type != 'cuda':
+            raise RuntimeError(f'{type(self).__name__}.forward needs the model on a CUDA device (no CPU fallback)')
+        g = lambda k, d=None: batch.get(k, d) if hasattr(batch, 'get') else (batch[k] if k in batch else d)
+        keys = ['ligand_pos', 'ligand_atom_type', 'protein_pos', 'protein_atom_feature', 'protein_aa_type',
+                'ligand_lig_flag', 'protein_lig_flag', 'ligand_element_batch', 'protein_element_batch',
+                'ligand_gen_flag', 'protein_gen_flag']
+        b = {k: g(k).to(dev) for k in keys if g(k) is not None}
+        x0 = b['ligand_pos'].float().contiguous()
+        v0 = b['ligand_atom_type'].long().contiguous()
+        mask_gen = b['ligand_gen_flag'].bool() if 'ligand_gen_flag' in b else b['ligand_lig_flag'].bool()
+        n_lig = x0.shape[0]
+        if n_lig == 0:
+            raise ValueError('the batch has no ligand atoms')
+        n_nodes = n_lig + b['protein_pos'].shape[0]
+        n_graphs = int(torch.cat([b['ligand_element_batch'], b['protein_element_batch']]).max()) + 1
+        if pos_noise is None or type_uniform is None:
+            draws = [(torch.randn(n_lig, 3, device=dev), torch.rand(n_lig, K, device=dev)) for _ in range(R)]
+            pos_noise = torch.stack([d[0] for d in draws]) if pos_noise is None else pos_noise
+            type_uniform = torch.stack([d[1] for d in draws]) if type_uniform is None else type_uniform
+        pos_noise = pos_noise.to(dev, torch.float32).reshape(R, n_lig, 3).contiguous()
+        type_uniform = type_uniform.to(dev, torch.float32).reshape(R, n_lig, K).contiguous()
+
+        xt = torch.empty(R, n_lig, 3, device=dev)
+        vt = torch.empty(R, n_lig, dtype=torch.int64, device=dev)
+        x_pred = torch.empty(R, n_lig, 3, device=dev)
+        c_pred = torch.empty(R, n_lig, K, device=dev)
+        rep_loss = torch.empty(R, 2, device=dev)
+        budget = self.eval_max_nodes if max_nodes is None else int(max_nodes)
+        per_launch = max(1, min(_lib.EVAL_MAX_REPLICAS, budget // n_nodes))
+        L = _lib.lib()
+        launches0 = L.cbg_launch_count()
+        for r0 in range(0, R, per_launch):
+            r1 = min(R, r0 + per_launch)
+            n = r1 - r0
+            state = self.prepare(replicate_batch(b, n, n_graphs))
+            coefs = (_lib.EvalCoef * n)(*[self.eval_coef(t) for t in t_values[r0:r1]])
+            graph_loss = torch.empty(n * n_graphs, 2, device=dev)
+            with torch.cuda.device(dev):
+                _lib.check(L.cbg_eval_loss_f32(
+                    C.byref(state['plan']), coefs, n, x0.data_ptr(), v0.data_ptr(), pos_noise[r0:r1].data_ptr(),
+                    type_uniform[r0:r1].data_ptr(), xt[r0:r1].data_ptr(), vt[r0:r1].data_ptr(), x_pred[r0:r1].data_ptr(),
+                    c_pred[r0:r1].data_ptr(), graph_loss.data_ptr(), rep_loss[r0:r1].data_ptr(), _lib.stream_ptr(dev)))
+        self.last_launches = L.cbg_launch_count() - launches0
+        per_t = rep_loss.cpu()
+        # get_dict_mean (common.py:33-42): mean over t of the per-t scalars, as a CPU float32 tensor
+        loss_dict = {'pos': torch.mean(torch.tensor(per_t[:, 0].tolist())),
+                     'atom': torch.mean(torch.tensor(per_t[:, 1].tolist()))}
+        results = [{'x0': x0, 'xt': xt[r], 'x_pred': x_pred[r], 'mask_gen': mask_gen,
+                    'v0': v0, 'vt': vt[r], 'c_pred': c_pred[r]} for r in range(R)]
+        return loss_dict, results
 
     @torch.no_grad()
     def run_steps(self, state, t_seq, X, Cc, V=None, pos_noise=None, type_uniform=None,

@@ -224,6 +224,36 @@ int32_t cbg_sample_step_graph_f32(const cbg_sample_plan* plan, const cbg_step_co
                                   float* x_next, float* c_next, int64_t* v_next, void* stream);
 int64_t cbg_sample_step_graph_nodes(const cbg_sample_plan* plan, void* stream);
 
+/* ---- validation loss: TargetDiff.forward in eval mode (targetdiff.py:41-124) -----------------------------------------
+ *
+ * The plan is one cbg_sample_begin_f32 filled over n_rep replicas of one batch of B graphs and n_lig / n_rep ligand atoms:
+ * graph r*B + g and ligand atom r*(n_lig/n_rep) + a of the plan are graph g and atom a of the batch, noised at replica r's
+ * timestep.  One call enqueues: forward noising of positions (CTNVPScheduler.forward_add_noise, diffusion_scheduler.py:
+ * 117-134) and types (q(v_t | v_0) Gumbel sample, :339-346 / :380-396) -> the denoiser with receptive-field pruning ->
+ * classifier on the ligand rows -> per-graph position MSE and type KL (decoder NLL at t == 0) (:185-201, :348-418) ->
+ * per-replica scatter_mean(...).mean().  The denoiser does not see t, so the replicas share one pass.  Every reduction
+ * runs in a fixed order (no atomics): repeated calls are bit-identical. */
+typedef struct cbg_eval_coef {  /* scheduler table entries of one replica's timestep t (host scalars) */
+  float alphas_cumprod;                    /* pos_scheduler.alphas_cumprod[t] */
+  float log_alphas_cumprod;                /* type_scheduler.log_alphas_cumprod_v[t] */
+  float log_one_minus_alphas_cumprod;      /* type_scheduler.log_one_minus_alphas_cumprod_v[t] */
+  float log_alphas_cumprod_prev;           /* type_scheduler.log_alphas_cumprod_v[max(t-1,0)] */
+  float log_one_minus_alphas_cumprod_prev; /* type_scheduler.log_one_minus_alphas_cumprod_v[max(t-1,0)] */
+  float log_alpha;                         /* type_scheduler.log_alphas_v[t] */
+  float log_one_minus_alpha;               /* type_scheduler.log_one_minus_alphas_v[t] */
+  int32_t t_is_zero;                       /* 1: the type loss is the decoder NLL instead of the KL */
+} cbg_eval_coef;
+
+/* coefs: host array [n_rep], n_rep <= 64.  x0 / v0: the batch's ligand_pos [n_lig/n_rep,3] / ligand_atom_type.
+ * Noise [n_rep, n_lig/n_rep, 3] (normal) and [n_rep, n_lig/n_rep, K] (uniform) comes from the caller.
+ * Outputs: xt, x_pred [n_rep, n_lig/n_rep, 3]; vt [n_rep, n_lig/n_rep]; c_pred = softmax(logits) [n_rep, n_lig/n_rep, K];
+ * graph_loss [n_rep*B, 2] per-graph (pos, atom) means over generated atoms (0 for a graph without any);
+ * rep_loss [n_rep, 2] per-replica (pos, atom) losses (NaN when no atom is generated). */
+int32_t cbg_eval_loss_f32(const cbg_sample_plan* plan, const cbg_eval_coef* coefs, int32_t n_rep,
+                          const float* x0, const int64_t* v0, const float* pos_noise, const float* type_uniform,
+                          float* xt, int64_t* vt, float* x_pred, float* c_pred, float* graph_loss, float* rep_loss,
+                          void* stream);
+
 /* the reverse step alone (testing / integration hook) */
 int32_t cbg_reverse_step_f32(const cbg_step_coef* coef, const float* x0_pred /*[n,3]*/, const float* logits /*[n,K]*/,
                              const float* x_t, const float* c_t, const uint8_t* gen /*[n]*/,
