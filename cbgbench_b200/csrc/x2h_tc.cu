@@ -30,6 +30,7 @@
 #include <math.h>
 #include <stdlib.h>
 #include <string.h>
+#include <type_traits>
 #include "cbg_kernels.cuh"
 #include "cbg_tc.cuh"
 
@@ -113,7 +114,8 @@ __device__ __forceinline__ float rows_sum(float v) {        // over the 8 row gr
 __device__ __forceinline__ float2 ldg2(const float* p) { return __ldg(reinterpret_cast<const float2*>(p)); }
 
 // pipeline event stamps of warpgroup 0 of CTA 0 (debugging; p.trace == nullptr in production: one predicated-off branch per
-// event).  Events of a tile: 0 G rows staged, 1 MMA1 complete, 2 activations ready, 3 MMA2 complete, 4 epilogue done
+// event).  Events of tile k, in loop order: 0 MMA1(k) complete, 1 MMA2(k) issued (S1 done), 2 MMA2(k) complete (G(k+1)
+// built meanwhile), 3 MMA1(k+1) issued (G(k+1) handed over; not stamped on the last tile), 4 epilogue(k) done
 #define TC_STAMP(k, ev)                                                                                  \
   do {                                                                                                   \
     if (p.trace != nullptr && blockIdx.x == 0 && tid == 0 && (k) < p.trace_tiles) p.trace[(k) * 16 + (ev)] = clock64(); \
@@ -196,82 +198,108 @@ __global__ void __launch_bounds__(256, 1) x2h_tc_kernel(EdgeArgs p, TcWeights W)
   const uint64_t dw_hi = smem_desc(sbase + SM_WG, LBO, WG_SBO), dw_lo = smem_desc(sbase + SM_WG + WG_IMG, LBO, WG_SBO);
   const uint64_t d1_hi = smem_desc(sbase + SM_W1, LBO, W1_SBO), d1_lo = smem_desc(sbase + SM_W1 + W1B, LBO, W1_SBO);
 
-  for (int k = 0; k < n_my; ++k) {
-    // ---- G row of this thread's edge (x2h_attention.py:46-52, unitransformer.py:88-99; explicit operation order:
-    // position-independent results; the factor 1024 of the G scale rides in the exponent).  Type block tb occupies
-    // k = 20 tb .. 20 tb + 19, the type one-hot k = 80 .. 83 of G_hi.
-    {
-      const int i = tile_node(k, g_slot);
-      const int jn = p.nbr[(size_t)i * CBG_KMAX + (g_row & 31)];
-      const float4 xi = p.x4[i], xj = p.x4[jn >= 0 ? jn : i];
-      const float rx = xi.x - xj.x, ry = xi.y - xj.y, rz = xi.z - xj.z;
-      const float d = sqrtf(__fmaf_rn(rz, rz, __fmaf_rn(ry, ry, __fmul_rn(rx, rx))));
-      const int fi = node_flags(xi), fj = node_flags(xj);
-      const int t_e = ((fj & 1) ? 0 : 2) + ((fi & 1) ? 0 : 1);
-      uint32_t gv[10];
+  // ---- stages of a tile ----------------------------------------------------------------------------------------------
+  // Index loads of tile kk: the node and neighbour of this thread's G row, the node and the two neighbours of its two
+  // accumulator rows
+  auto load_idx = [&](int kk, int& gi, int& gjn, int& ti, int& tj0, int& tj1) {
+    gi = tile_node(kk, g_slot);
+    gjn = p.nbr[(size_t)gi * CBG_KMAX + (g_row & 31)];
+    ti = tile_node(kk, slot);
+    const size_t eoff = (size_t)ti * CBG_KMAX + e0;
+    tj0 = p.nbr[eoff];
+    tj1 = p.nbr[eoff + 8];
+  };
+  // G row of this thread's edge into the warpgroup's G buffer (x2h_attention.py:46-52, unitransformer.py:88-99; explicit
+  // operation order: position-independent results; the factor 1024 of the G scale rides in the exponent).  Type block tb
+  // occupies k = 20 tb .. 20 tb + 19, the type one-hot k = 80 .. 83 of G_hi.
+  auto build_g = [&](const float4 xi, const float4 xj) {
+    const float rx = xi.x - xj.x, ry = xi.y - xj.y, rz = xi.z - xj.z;
+    const float d = sqrtf(__fmaf_rn(rz, rz, __fmaf_rn(ry, ry, __fmul_rn(rx, rx))));
+    const int fi = node_flags(xi), fj = node_flags(xj);
+    const int t_e = ((fj & 1) ? 0 : 2) + ((fi & 1) ? 0 : 1);
+    uint32_t gv[10];
 #pragma unroll
-      for (int mp = 0; mp < 10; ++mp) {
-        const float u0 = d - rbf[2 * mp], u1 = d - rbf[2 * mp + 1];
-        float g0, g1;
-        asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(g0) : "f"(fmaf(c2 * u0, u0, 10.f)));
-        asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(g1) : "f"(fmaf(c2 * u1, u1, 10.f)));
-        uint32_t hi, lo;
-        split_pair(g0, g1, hi, lo);
-        gv[mp] = g_part ? lo : hi;
-      }
-      uint8_t* grow = smem + SM_G + (uint32_t)(2 * wg + g_part) * G_IMG + (uint32_t)(g_row >> 3) * WG_SBO + (uint32_t)(g_row & 7) * 16u;
-#pragma unroll
-      for (int c = 0; c < KG_LO / 8; ++c) {        // 16-byte core-matrix rows: f16 pairs 4 c .. 4 c + 3
-        uint4 w;
-        w.x = (t_e == (4 * c) / 10) ? gv[(4 * c) % 10] : 0u;
-        w.y = (t_e == (4 * c + 1) / 10) ? gv[(4 * c + 1) % 10] : 0u;
-        w.z = (t_e == (4 * c + 2) / 10) ? gv[(4 * c + 2) % 10] : 0u;
-        w.w = (t_e == (4 * c + 3) / 10) ? gv[(4 * c + 3) % 10] : 0u;
-        *reinterpret_cast<uint4*>(grow + 128u * c) = w;
-      }
-      if (g_part == 0) {        // k = 80 .. 95 exist in G_hi only: the type one-hot, then zeros
-        uint4 w = make_uint4(0u, 0u, 0u, 0u);
-        w.x = (t_e == 0) ? kHalfTypeOne : ((t_e == 1) ? (kHalfTypeOne << 16) : 0u);
-        w.y = (t_e == 2) ? kHalfTypeOne : ((t_e == 3) ? (kHalfTypeOne << 16) : 0u);
-        *reinterpret_cast<uint4*>(grow + 128u * 10) = w;
-        *reinterpret_cast<uint4*>(grow + 128u * 11) = make_uint4(0u, 0u, 0u, 0u);
-      }
+    for (int mp = 0; mp < 10; ++mp) {
+      const float u0 = d - rbf[2 * mp], u1 = d - rbf[2 * mp + 1];
+      float g0, g1;
+      asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(g0) : "f"(fmaf(c2 * u0, u0, 10.f)));
+      asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(g1) : "f"(fmaf(c2 * u1, u1, 10.f)));
+      uint32_t hi, lo;
+      split_pair(g0, g1, hi, lo);
+      gv[mp] = g_part ? lo : hi;
     }
-    fence_proxy_async();
-    warpgroup_sync(wg);
-    TC_STAMP(k, 0);
-
-    // ---- inputs of this thread's two accumulator rows
-    const int n = 4 * ((int)blockIdx.x + k * (int)gridDim.x) + slot;
-    const bool live = n < n_list;
-    const int i = tile_node(k, slot);
-    const int w_row = p.w_compact ? (n < n_list ? n : n_list - 1) : i;       // row of the w buffer: list position (H2X) or node id
-    const size_t eoff = (size_t)i * CBG_KMAX + e0;
-    const int jn0 = p.nbr[eoff], jn1 = p.nbr[eoff + 8];
-    float v[64];
-    {   // Pi[i] + Pj[j] in the accumulator layout
-      const float* pi = pi_plane + (size_t)i * CBG_H + 2 * qt;
-      const float* pj0 = pj_plane + (size_t)(jn0 >= 0 ? jn0 : i) * CBG_H + 2 * qt;
-      const float* pj1 = pj_plane + (size_t)(jn1 >= 0 ? jn1 : i) * CBG_H + 2 * qt;
+    uint8_t* grow = smem + SM_G + (uint32_t)(2 * wg + g_part) * G_IMG + (uint32_t)(g_row >> 3) * WG_SBO + (uint32_t)(g_row & 7) * 16u;
 #pragma unroll
-      for (int j = 0; j < 16; ++j) {
-        const float2 a = ldg2(pi + 8 * j), b0 = ldg2(pj0 + 8 * j), b1 = ldg2(pj1 + 8 * j);
-        v[4 * j] = a.x + b0.x; v[4 * j + 1] = a.y + b0.y; v[4 * j + 2] = a.x + b1.x; v[4 * j + 3] = a.y + b1.y;
-      }
+    for (int c = 0; c < KG_LO / 8; ++c) {        // 16-byte core-matrix rows: f16 pairs 4 c .. 4 c + 3
+      uint4 w;
+      w.x = (t_e == (4 * c) / 10) ? gv[(4 * c) % 10] : 0u;
+      w.y = (t_e == (4 * c + 1) / 10) ? gv[(4 * c + 1) % 10] : 0u;
+      w.z = (t_e == (4 * c + 2) / 10) ? gv[(4 * c + 2) % 10] : 0u;
+      w.w = (t_e == (4 * c + 3) / 10) ? gv[(4 * c + 3) % 10] : 0u;
+      *reinterpret_cast<uint4*>(grow + 128u * c) = w;
     }
-    // ---- MMA1: small terms first
-    float d[64];
+    if (g_part == 0) {        // k = 80 .. 95 exist in G_hi only: the type one-hot, then zeros
+      uint4 w = make_uint4(0u, 0u, 0u, 0u);
+      w.x = (t_e == 0) ? kHalfTypeOne : ((t_e == 1) ? (kHalfTypeOne << 16) : 0u);
+      w.y = (t_e == 2) ? kHalfTypeOne : ((t_e == 3) ? (kHalfTypeOne << 16) : 0u);
+      *reinterpret_cast<uint4*>(grow + 128u * 10) = w;
+      *reinterpret_cast<uint4*>(grow + 128u * 11) = make_uint4(0u, 0u, 0u, 0u);
+    }
+  };
+  // MMA1, issued and committed, not waited for: small terms first
+  auto issue_mma1 = [&](float (&d)[64]) {
     wgmma_fence();
 #pragma unroll
-    for (int ks = 0; ks < KG_LO / 16; ++ks) wgmma_f16_ss(d, dg_lo + 16u * ks, dw_hi + 16u * ks, ks > 0 ? 1u : 0u);
+    for (int ks = 0; ks < KG_LO / 16; ++ks) {
+      if (ks == 0) wgmma_f16_ss_first(d, dg_lo, dw_hi);
+      else wgmma_f16_ss(d, dg_lo + 16u * ks, dw_hi + 16u * ks, 1u);
+    }
 #pragma unroll
     for (int ks = 0; ks < KG / 16; ++ks) wgmma_f16_ss(d, dg_hi + 16u * ks, dw_lo + 16u * ks, 1u);
 #pragma unroll
     for (int ks = 0; ks < KG / 16; ++ks) wgmma_f16_ss(d, dg_hi + 16u * ks, dw_hi + 16u * ks, 1u);
     wgmma_commit();
+    wgmma_settle(d);
+  };
+  // Pi[i] + Pj[j] of this thread's two accumulator rows in the accumulator layout, columns 8 j + 2 qt, + 1
+  auto gather_p = [&](float (&v)[64], int j, int ti, int tj0, int tj1) {
+    const float2 a = ldg2(pi_plane + (size_t)ti * CBG_H + 2 * qt + 8 * j);
+    const float2 b0 = ldg2(pj_plane + (size_t)(tj0 >= 0 ? tj0 : ti) * CBG_H + 2 * qt + 8 * j);
+    const float2 b1 = ldg2(pj_plane + (size_t)(tj1 >= 0 ? tj1 : ti) * CBG_H + 2 * qt + 8 * j);
+    v[4 * j] = a.x + b0.x; v[4 * j + 1] = a.y + b0.y; v[4 * j + 2] = a.x + b1.x; v[4 * j + 3] = a.y + b1.y;
+  };
+
+  // ---- software pipeline over this CTA's tiles.  Per warpgroup, tile k:
+  //   wait MMA1(k), S1(k), issue MMA2(k) | load the coordinates of k+1, build G(k+1) while MMA2(k) runs | wait MMA2(k),
+  //   issue MMA1(k+1) | epilogue(k) while MMA1(k+1) runs (it issues the Pi + Pj gathers of k+1 as it frees registers)
+  // The G buffer is free once every warp of the warpgroup has completed MMA1(k) (MMA2 reads no G), and the s_epi slots once
+  // every warp has finished epilogue(k-1): one warpgroup barrier after the MMA2 issue orders both.
+  float d[64], v[64];        // MMA1 accumulator and Pi + Pj of the tile in flight
+  int ti = 0, tj0 = 0, tj1 = 0;                        // node / neighbours of this thread's accumulator rows, tile k
+  int ngi = 0, ngjn = 0, nti = 0, ntj0 = 0, ntj1 = 0;  // the same of tile k+1, and its G-row node / neighbour
+  if (n_my > 0) {          // prologue: tile 0 up to its MMA1 issue
+    int gi, gjn;
+    load_idx(0, gi, gjn, ti, tj0, tj1);
+    build_g(p.x4[gi], p.x4[gjn >= 0 ? gjn : gi]);
+    fence_proxy_async();
+    warpgroup_sync(wg);
+    issue_mma1(d);
+#pragma unroll
+    for (int j = 0; j < 16; ++j) gather_p(v, j, ti, tj0, tj1);
+  }
+  // one tile; `more` (a compile-time constant: the last tile is peeled) says whether a tile k+1 follows, so the compiler
+  // sees exactly where d and v are redefined and keeps neither live across the drain
+  auto tile = [&](const int k, auto more_c) {
+    constexpr bool more = decltype(more_c)::value;
+    if constexpr (more) load_idx(k + 1, ngi, ngjn, nti, ntj0, ntj1);     // dependent index loads: their latency hides behind MMA1(k)
     wgmma_wait0();
     wgmma_settle(d);
-    TC_STAMP(k, 1);
+    TC_STAMP(k, 0);
+    // ---- inputs of this thread's two accumulator rows
+    const int n = 4 * ((int)blockIdx.x + k * (int)gridDim.x) + slot;
+    const bool live = n < n_list;
+    const int i = ti;
+    const int w_row = p.w_compact ? (n < n_list ? n : n_list - 1) : i;       // row of the w buffer: list position (H2X) or node id
     // ---- S1: pre = acc + Pi + Pj -> LayerNorm -> ReLU -> (hi, lo) f16 A fragments.  The first Linear is centred over
     // the feature axis by the packer, so pre has zero mean and LayerNorm needs only the sum of squares.
     uint32_t a_hi[8][4], a_lo[8][4];
@@ -305,8 +333,51 @@ __global__ void __launch_bounds__(256, 1) x2h_tc_kernel(EdgeArgs p, TcWeights W)
         }
       }
     }
-    TC_STAMP(k, 2);
-    // ---- MMA2 (A from registers) and the epilogue
+    // ---- MMA2 (A from REGISTERS: a_hi / a_lo stay untouched until it completes), issued and committed
+    auto issue_mma2 = [&](auto& o) {
+      wgmma_fence();
+#pragma unroll
+      for (int ks = 0; ks < 8; ++ks) {
+        if constexpr (IS_XV) wgmma_f16_rs_n16(o, a_lo[ks], d1_hi + 16u * ks, ks > 0 ? 1u : 0u);
+        else wgmma_f16_rs(o, a_lo[ks], d1_hi + 16u * ks, ks > 0 ? 1u : 0u);
+      }
+#pragma unroll
+      for (int ks = 0; ks < 8; ++ks) {
+        if constexpr (IS_XV) wgmma_f16_rs_n16(o, a_hi[ks], d1_lo + 16u * ks, 1u);
+        else wgmma_f16_rs(o, a_hi[ks], d1_lo + 16u * ks, 1u);
+      }
+#pragma unroll
+      for (int ks = 0; ks < 8; ++ks) {
+        if constexpr (IS_XV) wgmma_f16_rs_n16(o, a_hi[ks], d1_hi + 16u * ks, 1u);
+        else wgmma_f16_rs(o, a_hi[ks], d1_hi + 16u * ks, 1u);
+      }
+      wgmma_commit();
+      wgmma_settle(o);
+      TC_STAMP(k, 1);
+    };
+    // ---- while MMA2(k) runs: G(k+1); then MMA2(k) complete, MMA1(k+1) issued
+    auto advance = [&](auto& o) {
+      if constexpr (more) {
+        const float4 xi = p.x4[ngi], xj = p.x4[ngjn >= 0 ? ngjn : ngi];
+        warpgroup_sync(wg);                            // MMA1(k) complete and epilogue(k-1) done in every warp
+        build_g(xi, xj);
+        fence_proxy_async();
+      } else {
+        warpgroup_sync(wg);                            // epilogue(k-1) done in every warp
+      }
+      wgmma_wait0();
+      wgmma_settle(o);
+      TC_STAMP(k, 2);
+      if constexpr (more) {
+        warpgroup_sync(wg);                            // G(k+1) complete
+        issue_mma1(d);
+        TC_STAMP(k, 3);
+      }
+    };
+    // ---- epilogue(k) from the MMA2 fragment, while MMA1(k+1) runs.  The Pi + Pj gathers of k+1 are issued column
+    // group by column group as the epilogue frees the fragment registers of the same group: they start early, and o and
+    // v are never both live in full
+    auto gather_next = [&](int j) { if constexpr (more) gather_p(v, j, nti, ntj0, ntj1); };
     if constexpr (MODE == MODE_K) {
       // attention weights: <q_i, k> per head (a head's 8 columns = one quad's registers), softmax over the node's 32
       // edges through shared memory, w = alpha * e_w
@@ -325,26 +396,18 @@ __global__ void __launch_bounds__(256, 1) x2h_tc_kernel(EdgeArgs p, TcWeights W)
         sc[j] = p.nbr[eo] >= 0 ? p.ew[eo] : 0.f;
       }
       float o[64];
-      wgmma_fence();
-#pragma unroll
-      for (int ks = 0; ks < 8; ++ks) wgmma_f16_rs(o, a_lo[ks], d1_hi + 16u * ks, ks > 0 ? 1u : 0u);
-#pragma unroll
-      for (int ks = 0; ks < 8; ++ks) wgmma_f16_rs(o, a_hi[ks], d1_lo + 16u * ks, 1u);
-#pragma unroll
-      for (int ks = 0; ks < 8; ++ks) wgmma_f16_rs(o, a_hi[ks], d1_hi + 16u * ks, 1u);
-      wgmma_commit();
-      wgmma_wait0();
-      wgmma_settle(o);
-      TC_STAMP(k, 3);
+      issue_mma2(o);
+      advance(o);
       float* s_sm = s_epi + slot * (32 * 17);              // [edge][17]: conflict-free rows
 #pragma unroll
       for (int j = 0; j < 16; ++j) {
         const float l0 = quad_sum(fmaf(o[4 * j + 1], qv[2 * j + 1], o[4 * j] * qv[2 * j]));
         const float l1 = quad_sum(fmaf(o[4 * j + 3], qv[2 * j + 1], o[4 * j + 2] * qv[2 * j]));
         if ((j & 3) == qt) {
-          s_sm[e0 * 17 + j] = jn0 >= 0 ? l0 * kInvOut : -INFINITY;
-          s_sm[(e0 + 8) * 17 + j] = jn1 >= 0 ? l1 * kInvOut : -INFINITY;
+          s_sm[e0 * 17 + j] = tj0 >= 0 ? l0 * kInvOut : -INFINITY;
+          s_sm[(e0 + 8) * 17 + j] = tj1 >= 0 ? l1 * kInvOut : -INFINITY;
         }
+        gather_next(j);
       }
       warpgroup_sync(wg);
       {
@@ -376,18 +439,13 @@ __global__ void __launch_bounds__(256, 1) x2h_tc_kernel(EdgeArgs p, TcWeights W)
           wv[h][4 * j] = t.x; wv[h][4 * j + 1] = t.y; wv[h][4 * j + 2] = t.z; wv[h][4 * j + 3] = t.w;
         }
       }
+      // this thread's two h_i values, read early: every node is listed once and no other thread writes its row
+      const int c = 2 * (32 * wp + lane);
+      float2* hp = reinterpret_cast<float2*>(p.h + (size_t)i * CBG_H + c);
+      const float2 hv = *hp;
       float o[64];
-      wgmma_fence();
-#pragma unroll
-      for (int ks = 0; ks < 8; ++ks) wgmma_f16_rs(o, a_lo[ks], d1_hi + 16u * ks, ks > 0 ? 1u : 0u);
-#pragma unroll
-      for (int ks = 0; ks < 8; ++ks) wgmma_f16_rs(o, a_hi[ks], d1_lo + 16u * ks, 1u);
-#pragma unroll
-      for (int ks = 0; ks < 8; ++ks) wgmma_f16_rs(o, a_hi[ks], d1_hi + 16u * ks, 1u);
-      wgmma_commit();
-      wgmma_wait0();
-      wgmma_settle(o);
-      TC_STAMP(k, 3);
+      issue_mma2(o);
+      advance(o);
       float* s_vr = s_epi + (slot * 2 + wp) * CBG_H;       // this warp's 16-edge partial sums
 #pragma unroll
       for (int j = 0; j < 16; ++j) {
@@ -395,13 +453,11 @@ __global__ void __launch_bounds__(256, 1) x2h_tc_kernel(EdgeArgs p, TcWeights W)
         const float sx = rows_sum(fmaf(fmaf(o[4 * j + 2], kInvOut, b1.x), wv[1][j], fmaf(o[4 * j], kInvOut, b1.x) * wv[0][j]));
         const float sy = rows_sum(fmaf(fmaf(o[4 * j + 3], kInvOut, b1.y), wv[1][j], fmaf(o[4 * j + 1], kInvOut, b1.y) * wv[0][j]));
         if ((j >> 1) == qg) *reinterpret_cast<float2*>(s_vr + 8 * j + 2 * qt) = make_float2(sx, sy);
+        gather_next(j);
       }
       warpgroup_sync(wg);
       if (live) {
-        const int c = 2 * (32 * wp + lane);
         const float* s0 = s_epi + (slot * 2) * CBG_H + c;
-        float2* hp = reinterpret_cast<float2*>(p.h + (size_t)i * CBG_H + c);
-        const float2 hv = *hp;
         *hp = make_float2(hv.x + (s0[0] + s0[CBG_H]), hv.y + (s0[1] + s0[CBG_H + 1]));
       }
     } else {
@@ -415,23 +471,16 @@ __global__ void __launch_bounds__(256, 1) x2h_tc_kernel(EdgeArgs p, TcWeights W)
           const float* wi = p.w + ((size_t)w_row * CBG_KMAX + e0 + 8 * h) * CBG_HEADS + 2 * qt;
           wx[h][0] = *reinterpret_cast<const float2*>(wi);
           wx[h][1] = *reinterpret_cast<const float2*>(wi + 8);
-          const int jn = h ? jn1 : jn0;       // padded slots: j = i, and their w is zero
+          const int jn = h ? tj1 : tj0;       // padded slots: j = i, and their w is zero
           const float4 xj = p.x4[jn >= 0 ? jn : i];
           rel[h][0] = xi.x - xj.x; rel[h][1] = xi.y - xj.y; rel[h][2] = xi.z - xj.z;
         }
       }
       float o[8];
-      wgmma_fence();
+      issue_mma2(o);
+      advance(o);
 #pragma unroll
-      for (int ks = 0; ks < 8; ++ks) wgmma_f16_rs_n16(o, a_lo[ks], d1_hi + 16u * ks, ks > 0 ? 1u : 0u);
-#pragma unroll
-      for (int ks = 0; ks < 8; ++ks) wgmma_f16_rs_n16(o, a_hi[ks], d1_lo + 16u * ks, 1u);
-#pragma unroll
-      for (int ks = 0; ks < 8; ++ks) wgmma_f16_rs_n16(o, a_hi[ks], d1_hi + 16u * ks, 1u);
-      wgmma_commit();
-      wgmma_wait0();
-      wgmma_settle(o);
-      TC_STAMP(k, 3);
+      for (int j = 0; j < 16; ++j) gather_next(j);
       float se[2];
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
@@ -457,7 +506,10 @@ __global__ void __launch_bounds__(256, 1) x2h_tc_kernel(EdgeArgs p, TcWeights W)
       }
     }
     TC_STAMP(k, 4);
-  }
+    ti = nti; tj0 = ntj0; tj1 = ntj1;
+  };
+  for (int k = 0; k + 1 < n_my; ++k) tile(k, std::true_type{});
+  if (n_my > 0) tile(n_my - 1, std::false_type{});
   TC_STAMP_CTA(2);
 }
 
