@@ -45,6 +45,10 @@ class EvalCoef(C.Structure):
 EVAL_MAX_REPLICAS = 64     # replicas per cbg_eval_loss_f32 call (csrc/cbg_kernels.cuh: CBG_EVAL_MAX_REPLICAS)
 
 
+class BpEvalCoef(C.Structure):
+    _fields_ = [('alphas_cumprod', C.c_float), ('beta', C.c_float), ('mask_prob', C.c_float)]
+
+
 class SbddCoef(C.Structure):
     _fields_ = [('a', C.c_float), ('b', C.c_float), ('s', C.c_float), ('mode', C.c_int32)]
 
@@ -92,6 +96,8 @@ SIGNATURES = {
     'cbg_eval_loss_f32': (_I32, [C.POINTER(SamplePlan), C.POINTER(EvalCoef), _I32, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     'cbg_sbdd_step_f32': (_I32, [C.POINTER(SamplePlan), C.POINTER(SbddCoef), _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     'cbg_bp_step_f32': (_I32, [C.POINTER(SamplePlan), _P, _I32, C.POINTER(BpCoef), _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
+    'cbg_bp_eval_loss_f32': (_I32, [C.POINTER(SamplePlan), _P, _I32, C.POINTER(BpEvalCoef), _I32, _P, _P, _P, _P, _P, _P,
+                                     _P, _P, _P, _P, _P]),
     'cbg_pocket_stats_f32': (_I32, [_P, _P, _I32, _P, _P, _I32, _P, _P, _P]),
     'cbg_sample_ligand_sizes': (_I32, [_P, _P, _I32, _I32, _P, _P, _P, _P, _P, _P]),
     'cbg_build_batch_f32': (_I32, [_P, _P]),

@@ -337,6 +337,53 @@ int run_core(const float* blob, int num_layers, const Workspace& ws, const int* 
   return 0;
 }
 
+// CoM head of DiffBP (CoMPredictor.forward, diffbp.py:80-101) after run_core on the same plan: the ligand rows of x4
+// get the step's INPUT coordinates x_t back, then the head's own edge gate and com_layers x H2X on the denoiser's final
+// h move the generated rows.  Afterwards the ligand rows of x4 hold x_com.  Shared by the sampling step and the
+// validation loss.
+int run_com_head(const cbg_sample_plan* plan, const float* com_blob, int com_layers, const Workspace& ws,
+                 const float* x_t, bool prune, cudaStream_t st) {
+  const long long n_nodes = plan->n_nodes;
+  const int n_gen = plan->n_gen, n_lig = plan->n_lig;
+  if (int rc = cbg_launch_scatter_x(x_t, plan->lig_node, n_lig, ws.x4, st)) return rc;
+  if (n_gen > 0 && com_layers > 0) {
+    if (int rc = cbg_launch_edge_gate_rows(com_blob, ws.x4, ws.nbr, plan->gen_node, n_gen, ws.ew, st)) return rc;
+    const bool pruned = prune && plan->num_layers > 0;      // run_core built ws.order / ws.cnt
+    const float* layers = com_blob + cbg_layout::kGlobalFloats;
+    for (int l = 0; l < com_layers; ++l) {
+      const float* L = layers + (size_t)l * cbg_layout::kLayerFloats;
+      NodeGemmArgs gj{};
+      gj.a = ws.h; gj.row_idx = nullptr; gj.n_rows = (int)n_nodes;
+      gj.wt = L + cbg_layout::layer_offset(CBG_LF_H2X_NODE_WT);
+      gj.bias = L + cbg_layout::layer_offset(CBG_LF_H2X_NODE_B);
+      gj.ldw = 640; gj.n_planes = 2; gj.has_q = 0;
+      gj.out[0] = ws.hplane[0]; gj.out[1] = ws.hplane[1];
+      gj.tc_planes = L + cbg_layout::layer_offset(CBG_LF_H2X_NODE_TC); gj.tc_first_plane = 0;
+      gj.tch_planes = L + cbg_layout::layer_offset(CBG_LF_H2X_NODE_TCH);
+      if (pruned) { gj.row_idx = ws.order; gj.n_rows_dev = ws.cnt + plan->num_layers; }   // generated atoms + neighbours
+      if (int rc = launch_node_gemm(gj, st)) return rc;
+      NodeGemmArgs gi{};
+      gi.a = ws.h; gi.row_idx = plan->gen_node; gi.n_rows = n_gen;
+      gi.wt = gj.wt + 256; gi.bias = gj.bias + 256;
+      gi.ldw = 640; gi.n_planes = 3; gi.has_q = 1;
+      gi.out[0] = ws.hplane[2]; gi.out[1] = ws.hplane[3]; gi.out[2] = nullptr;
+      gi.q_ln = L + cbg_layout::layer_offset(CBG_LF_H2X_Q_LN);
+      gi.q_w1t = L + cbg_layout::layer_offset(CBG_LF_H2X_Q_W1T);
+      gi.q_b1 = L + cbg_layout::layer_offset(CBG_LF_H2X_Q_B1);
+      gi.out_q = ws.hplane[4];
+      gi.tc_planes = gj.tc_planes; gi.tc_first_plane = 2; gi.tch_planes = gj.tch_planes;
+      if (int rc = launch_node_gemm(gi, st)) return rc;
+      EdgeArgs x{};
+      x.x4 = ws.x4; x.nbr = ws.nbr; x.ew = ws.ew;
+      x.pj_k = ws.hplane[0]; x.pj_v = ws.hplane[1]; x.pi_k = ws.hplane[2]; x.pi_v = ws.hplane[3]; x.q = ws.hplane[4];
+      x.layer = L; x.w = ws.hw; x.h = ws.h; x.node_idx = plan->gen_node; x.n_nodes = n_gen; x.dx = ws.dx;
+      if (int rc = cbg_launch_h2x(x, st)) return rc;
+      if (int rc = cbg_launch_apply_dx(ws.x4, plan->gen_node, ws.dx, n_gen, st)) return rc;
+    }
+  }
+  return 0;
+}
+
 // cached device scratch for the *_host entry points: one per DEVICE (the buffers belong to the device that was current
 // when they were allocated); the weight blob is re-uploaded whenever the caller's (version, size, host pointer) changes -
 // the version is a process-unique id handed out by the Python side, so two models never alias
@@ -830,42 +877,7 @@ int32_t cbg_bp_step_f32(const cbg_sample_plan* plan, const float* com_blob, int3
   if (int rc = cbg_launch_classifier(plan->blob, ws.h, plan->lig_node, n_lig, K, lg, st)) return rc;
   if (int rc = cbg_launch_gather_x(ws.x4, plan->lig_node, n_lig, xp, st)) return rc;
   // ---- CoM head (diffbp.py:80-101): same graph, own gate, H2X stack on the final h, starting from the INPUT x
-  if (int rc = cbg_launch_scatter_x(x_t, plan->lig_node, n_lig, ws.x4, st)) return rc;
-  if (n_gen > 0 && com_layers > 0) {
-    if (int rc = cbg_launch_edge_gate_rows(com_blob, ws.x4, ws.nbr, plan->gen_node, n_gen, ws.ew, st)) return rc;
-    const bool pruned = prune && plan->num_layers > 0;      // run_core built ws.order / ws.cnt
-    const float* layers = com_blob + cbg_layout::kGlobalFloats;
-    for (int l = 0; l < com_layers; ++l) {
-      const float* L = layers + (size_t)l * cbg_layout::kLayerFloats;
-      NodeGemmArgs gj{};
-      gj.a = ws.h; gj.row_idx = nullptr; gj.n_rows = (int)n_nodes;
-      gj.wt = L + cbg_layout::layer_offset(CBG_LF_H2X_NODE_WT);
-      gj.bias = L + cbg_layout::layer_offset(CBG_LF_H2X_NODE_B);
-      gj.ldw = 640; gj.n_planes = 2; gj.has_q = 0;
-      gj.out[0] = ws.hplane[0]; gj.out[1] = ws.hplane[1];
-      gj.tc_planes = L + cbg_layout::layer_offset(CBG_LF_H2X_NODE_TC); gj.tc_first_plane = 0;
-    gj.tch_planes = L + cbg_layout::layer_offset(CBG_LF_H2X_NODE_TCH);
-      if (pruned) { gj.row_idx = ws.order; gj.n_rows_dev = ws.cnt + plan->num_layers; }   // generated atoms + neighbours
-      if (int rc = launch_node_gemm(gj, st)) return rc;
-      NodeGemmArgs gi{};
-      gi.a = ws.h; gi.row_idx = plan->gen_node; gi.n_rows = n_gen;
-      gi.wt = gj.wt + 256; gi.bias = gj.bias + 256;
-      gi.ldw = 640; gi.n_planes = 3; gi.has_q = 1;
-      gi.out[0] = ws.hplane[2]; gi.out[1] = ws.hplane[3]; gi.out[2] = nullptr;
-      gi.q_ln = L + cbg_layout::layer_offset(CBG_LF_H2X_Q_LN);
-      gi.q_w1t = L + cbg_layout::layer_offset(CBG_LF_H2X_Q_W1T);
-      gi.q_b1 = L + cbg_layout::layer_offset(CBG_LF_H2X_Q_B1);
-      gi.out_q = ws.hplane[4];
-      gi.tc_planes = gj.tc_planes; gi.tc_first_plane = 2; gi.tch_planes = gj.tch_planes;
-      if (int rc = launch_node_gemm(gi, st)) return rc;
-      EdgeArgs x{};
-      x.x4 = ws.x4; x.nbr = ws.nbr; x.ew = ws.ew;
-      x.pj_k = ws.hplane[0]; x.pj_v = ws.hplane[1]; x.pi_k = ws.hplane[2]; x.pi_v = ws.hplane[3]; x.q = ws.hplane[4];
-      x.layer = L; x.w = ws.hw; x.h = ws.h; x.node_idx = plan->gen_node; x.n_nodes = n_gen; x.dx = ws.dx;
-      if (int rc = cbg_launch_h2x(x, st)) return rc;
-      if (int rc = cbg_launch_apply_dx(ws.x4, plan->gen_node, ws.dx, n_gen, st)) return rc;
-    }
-  }
+  if (int rc = run_com_head(plan, com_blob, com_layers, ws, x_t, prune, st)) return rc;
   BpArgs r{};
   r.x4 = ws.x4; r.graph_ptr = plan->graph_ptr; r.lig_node = plan->lig_node; r.n_lig = n_lig; r.num_classes = K;
   r.n_graphs = plan->n_graphs; r.x_pred = xp; r.logits = lg; r.x_t = x_t; r.c_t = c_t; r.gen = plan->gen_lig;
@@ -873,6 +885,51 @@ int32_t cbg_bp_step_f32(const cbg_sample_plan* plan, const float* com_blob, int3
   r.nonzero = coef->nonzero; r.prob = coef->change_prob; r.x_next = x_next; r.c_next = c_next;
   r.v_next = (long long*)v_next; r.eps_out = eps_out;
   return cbg_launch_bp_reverse(r, st);
+}
+
+int32_t cbg_bp_eval_loss_f32(const cbg_sample_plan* plan, const float* com_blob, int32_t com_layers,
+                             const cbg_bp_eval_coef* coefs, int32_t n_rep, const float* x0, const int64_t* v0,
+                             const float* pos_noise, const float* type_uniform, float* xt, int64_t* vt, uint8_t* mask,
+                             float* vec, float* c_pred, float* rep_loss, void* stream) {
+  if (!plan || !com_blob || !coefs || !x0 || !v0 || !pos_noise || !type_uniform || !xt || !vt || !mask || !vec || !c_pred ||
+      !rep_loss) {
+    cbg_set_error("cbg_bp_eval_loss_f32: null argument"); return 1;
+  }
+  if (com_layers < 0 || com_layers > 16) { cbg_set_error("com_layers=%d outside [0,16]", com_layers); return 1; }
+  if (n_rep < 1 || n_rep > CBG_EVAL_MAX_REPLICAS) { cbg_set_error("n_rep=%d outside [1,%d]", n_rep, CBG_EVAL_MAX_REPLICAS); return 1; }
+  if (plan->n_lig < n_rep || plan->n_lig % n_rep || plan->n_graphs % n_rep) {
+    cbg_set_error("plan (n_lig=%d, n_graphs=%d) is not %d replicas of one batch", plan->n_lig, plan->n_graphs, n_rep); return 1;
+  }
+  NvtxRange nvtx_eval("cbg:bp_eval_loss");
+  Workspace ws;
+  if (int rc = check_ws(plan->workspace, plan->workspace_bytes, plan->n_nodes, plan->n_gen, &ws)) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  const int K = plan->num_classes, n_lig = plan->n_lig;
+  if (K < 1 || K > CBG_MAXCLS) { cbg_set_error("num_classes=%d outside [1,%d]", K, CBG_MAXCLS); return 1; }
+  BpEvalArgs e{};
+  for (int r = 0; r < n_rep; ++r) e.coef.c[r] = BpEvalCoefDev{coefs[r].alphas_cumprod, coefs[r].beta, coefs[r].mask_prob};
+  e.n_rep = n_rep; e.n_lig = n_lig; e.n_graphs = plan->n_graphs; e.num_classes = K;
+  e.lig_node = plan->lig_node; e.graph_ptr = plan->graph_ptr; e.gen = plan->gen_lig;
+  e.x0 = x0; e.v0 = (const long long*)v0; e.pos_noise = pos_noise; e.type_u = type_uniform;
+  e.emb_wt = plan->emb_wt; e.h_lig_bias = plan->h_lig_bias;
+  e.x4 = ws.x4; e.h = ws.h; e.xt = xt; e.vt = (long long*)vt; e.mask = mask; e.vec = vec; e.c_pred = c_pred;
+  e.rep_loss = rep_loss;
+  // scratch: logits | denoiser output coordinates in the attention-weight buffer (as in cbg_bp_step_f32); the X2H
+  // planes are free once the denoiser is done (the CoM head uses the H2X planes)
+  float* lg = ws.w;
+  float* xp = ws.w + align256((size_t)n_lig * K * 4) / 4;
+  e.logits = lg; e.x_pred = xp;
+  e.xs = (float4*)ws.plane[0]; e.thr = (int2*)ws.plane[1]; e.graph_part = ws.plane[2];
+  CBG_CUDA_OK(cudaMemcpyAsync(ws.h, plan->h_static, (size_t)plan->n_nodes * CBG_H * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  if (int rc = cbg_launch_bp_eval_noise(e, st)) return rc;
+  const bool prune = plan->prune != 0 && prune_enabled();
+  if (int rc = run_core(plan->blob, plan->num_layers, ws, plan->graph_ptr, plan->n_graphs, plan->max_graph_nodes,
+                        plan->n_nodes, plan->gen_node, plan->n_gen, plan->mode, plan->k, plan->r_max, plan->rcache,
+                        plan->lig_node, n_lig, prune, st, plan->static_lists != 0)) return rc;
+  if (int rc = cbg_launch_classifier(plan->blob, ws.h, plan->lig_node, n_lig, K, lg, st)) return rc;
+  if (int rc = cbg_launch_gather_x(ws.x4, plan->lig_node, n_lig, xp, st)) return rc;
+  if (int rc = run_com_head(plan, com_blob, com_layers, ws, xt, prune, st)) return rc;
+  return cbg_launch_bp_eval_loss(e, st);
 }
 
 int32_t cbg_reverse_step_f32(const cbg_step_coef* coef, const float* x0_pred, const float* logits, const float* x_t,

@@ -237,6 +237,40 @@ struct BpArgs {
 };
 int cbg_launch_bp_reverse(const BpArgs& a, cudaStream_t st);
 
+// bp_eval.cu: DiffBP validation loss over R replicas of a batch (cbg_bp_eval_loss_f32), replica-major like EvalArgs.
+constexpr int CBG_BP_INTER_K = 48;       // interior loss: protein -> ligand kNN (diffbp.py:19)
+struct BpEvalCoefDev { float alphas_cumprod, beta, mask_prob; };    // same members as cbg_bp_eval_coef
+struct BpEvalCoefs { BpEvalCoefDev c[CBG_EVAL_MAX_REPLICAS]; };
+struct BpEvalArgs {
+  BpEvalCoefs coef;
+  int n_rep, n_lig, n_graphs, num_classes;   // n_lig / n_graphs: replicated totals
+  const int* lig_node;       // [n_lig] ascending composed node index
+  const int* graph_ptr;      // [n_graphs+1]
+  const unsigned char* gen;  // [n_lig] replicated ligand_gen_flag
+  const float* x0;           // [n_lig/n_rep,3]
+  const long long* v0;       // [n_lig/n_rep]
+  const float* pos_noise;    // [n_lig,3] raw normal draws
+  const float* type_u;       // [n_lig] uniform draws of the type mask
+  const float* emb_wt;       // [K,128]
+  const float* h_lig_bias;   // [n_lig,128]
+  const float* logits;       // [n_lig,K] classifier output
+  const float* x_pred;       // [n_lig,3] denoiser output coordinates
+  float4* x4;                // node coordinates + flags; after the CoM head the ligand rows hold x_com
+  float* h;                  // [N,128] node features
+  float* xt;                 // [n_lig,3]
+  long long* vt;             // [n_lig]
+  unsigned char* mask;       // [n_lig] type mask
+  float* vec;                // [n_rep, 8, n_lig/n_rep, 3]: eps_0, eps_pred, score_0, score_pred, then the _com four
+  float* c_pred;             // [n_lig,K]
+  float4* xs;                // [n_lig] scratch: posterior mean of x_{t-1} (interior loss)
+  int2* thr;                 // [N] scratch: per protein node, (d^2 bits, ligand index) of its 48th nearest ligand atom
+  float* graph_part;         // [n_graphs,8] scratch: per-graph means / counts / interior-loss sum
+  float* rep_loss;           // [n_rep,4]: pos, atom, com, inter
+};
+int cbg_launch_bp_eval_noise(const BpEvalArgs& a, cudaStream_t st);
+// bp_eval_loss_kernel (one CTA per graph) followed by bp_eval_reduce_kernel (one thread per replica)
+int cbg_launch_bp_eval_loss(const BpEvalArgs& a, cudaStream_t st);
+
 // batch.cu (row f3: device-side batch construction)
 int cbg_launch_pocket_stats(const float* prot_pos, const int* prot_ptr, int n_pockets, const float* ctx_pos,
                             const int* ctx_ptr, int centre_mode, float* space_size, float* centre, cudaStream_t st);

@@ -11,16 +11,20 @@ gates, receptive-field pruning) all apply to the denoiser part unchanged.
 
 Random numbers: ``torch.randn_like`` (positions) then ``torch.rand_like`` over [n_lig] (type change mask) per step,
 in the reference's order (diffusion_scheduler.py:158, 486), or injected for parity tests.
+
+The eval-mode ``forward(batch)`` (diffbp.py:133-230, the validation loss) runs the noised copies of the batch for all
+its timesteps through ONE C-ABI call (``cbg_bp_eval_loss_f32``, DESIGN.md section 14).
 """
 import ctypes as C
 
 import torch
 from torch import nn
+import torch.nn.functional as F
 
 from . import _lib
 from .modules import (GaussianSmearing, H2XAttention, MLP, _NoTorchPath, cfg_get, pack_denoiser_blob)
 from .schedulers import CTNVPTables
-from .targetdiff import BaseDiffB200, register_model
+from .targetdiff import BaseDiffB200, eval_t_values, register_model
 
 ABSORBING_STATE = 0      # repo/utils/molecule/constants.py:8
 
@@ -90,6 +94,98 @@ class DiffBPB200(BaseDiffB200):
                            beta=float(ps.host_table('betas')[t_idx]),
                            nonzero=0.0 if t_idx == 0 else 1.0,
                            change_prob=self.type_scheduler.change_prob(t_idx))
+
+    # ---- validation loss (DiffBP.forward with self.training == False) ----------------------------------------------
+    def forward(self, batch, pos_noise=None, type_uniform=None):
+        """DiffBP.forward (diffbp.py:133-171).  Eval mode only: returns ``(loss_dict, results)`` for the
+        ``eval_interval`` (default 10) timesteps ``np.linspace(0, T-1, eval_interval)`` truncated to integers, exactly
+        like the reference; see ``eval_losses``.  Training mode needs autograd through the denoiser and raises."""
+        if self.training:
+            raise NotImplementedError(f'{type(self).__name__}.forward in training mode needs autograd through the '
+                                      'denoiser, which the CUDA path does not provide: training is out of scope '
+                                      '(call model.eval() for the validation losses)')
+        t_values = eval_t_values(self.num_diffusion_timesteps, cfg_get(self.cfg, 'eval_interval', 10))
+        return self.eval_losses(batch, t_values, pos_noise=pos_noise, type_uniform=type_uniform)
+
+    def eval_coef(self, t_idx):
+        ps = self.pos_scheduler
+        mask_prob = torch.tensor([t_idx]).float().clamp(min=0.) / self.num_diffusion_timesteps    # fp32, like :462-466
+        return _lib.BpEvalCoef(alphas_cumprod=float(ps.host_table('alphas_cumprod')[t_idx]),
+                               beta=float(ps.host_table('betas')[t_idx]), mask_prob=float(mask_prob[0]))
+
+    @torch.no_grad()
+    def eval_losses(self, batch, t_values, pos_noise=None, type_uniform=None, max_nodes=None):
+        """Validation losses of ``batch`` at the timesteps ``t_values`` (DiffBP.get_loss, diffbp.py:173-230, once per t).
+        Returns ``(loss_dict, results)`` like the reference's eval-mode forward: ``loss_dict`` = {'pos', 'atom', 'com',
+        'inter'} as CPU 0-d float32 tensors (mean over t of the per-t losses), ``results`` one dict per t with the device
+        tensors eps_0, eps_pred, score_0, score_pred, mask_gen (the type mask), v0, vt (one-hot float), c_pred, and
+        eps_0_com, eps_pred_com, score_0_com, score_pred_com, mask_gen_com (the generation flag).  A t whose batch has no
+        generated atom gets NaN pos / com losses; a t without masked atoms (every t = 0) an atom loss of 0, like the
+        reference.
+
+        The denoiser is not conditioned on t, so the R = len(t_values) noised copies go through ONE denoiser pass as
+        R*B graphs, split over several launches above ``max_nodes`` composed nodes (default ``eval_max_nodes``) or 64
+        replicas; the split does not change any result bit.
+
+        ``pos_noise`` [R,n_lig,3] / ``type_uniform`` [R,n_lig] inject the draws; by default they are drawn with torch on
+        the model device in the reference's order (for each t: randn [n_lig,3], then rand [n_lig])."""
+        if not self.intersect_reg:
+            raise NotImplementedError('intersect_reg: False is not supported: the reference\'s DiffBP.get_loss reads the '
+                                      'interior loss unconditionally (diffbp.py:222-226) and raises UnboundLocalError')
+        t_values = [int(t) for t in t_values]
+        R, T, K = len(t_values), self.num_diffusion_timesteps, self.num_classes
+        if R == 0:
+            raise ValueError('t_values is empty')
+        if any(t < 0 or t >= T for t in t_values):
+            raise ValueError(f't_values must lie in [0, {T - 1}]')
+        dev = next(self.parameters()).device
+        if dev.type != 'cuda':
+            raise NotImplementedError(f'{type(self).__name__}.forward needs the model on a CUDA device: the validation '
+                                      'losses have no CPU implementation')
+        b, n_graphs = self._eval_batch(batch, dev)
+        if 'protein_gen_flag' in b and bool(b['protein_gen_flag'].any()):
+            raise NotImplementedError('the interior loss reads the pocket at its input coordinates: protein_gen_flag '
+                                      'must be all False')
+        x0 = b['ligand_pos'].float().contiguous()
+        v0 = b['ligand_atom_type'].long().contiguous()
+        gen = b['ligand_gen_flag'] if 'ligand_gen_flag' in b else b['ligand_lig_flag']
+        n_lig = x0.shape[0]
+        if pos_noise is None or type_uniform is None:
+            draws = [(torch.randn(n_lig, 3, device=dev), torch.rand(n_lig, device=dev)) for _ in range(R)]
+            pos_noise = torch.stack([d[0] for d in draws]) if pos_noise is None else pos_noise
+            type_uniform = torch.stack([d[1] for d in draws]) if type_uniform is None else type_uniform
+        pos_noise = pos_noise.to(dev, torch.float32).reshape(R, n_lig, 3).contiguous()
+        type_uniform = type_uniform.to(dev, torch.float32).reshape(R, n_lig).contiguous()
+
+        com_blob = self.com_head.packed_blob(dev)
+        xt = torch.empty(R, n_lig, 3, device=dev)
+        vt = torch.empty(R, n_lig, dtype=torch.int64, device=dev)
+        mask = torch.empty(R, n_lig, dtype=torch.uint8, device=dev)
+        vec = torch.empty(R, 8, n_lig, 3, device=dev)
+        c_pred = torch.empty(R, n_lig, K, device=dev)
+        rep_loss = torch.empty(R, 4, device=dev)
+        L = _lib.lib()
+        launches0 = L.cbg_launch_count()
+        for r0, r1, state in self._eval_launches(b, n_graphs, R, max_nodes):
+            n = r1 - r0
+            coefs = (_lib.BpEvalCoef * n)(*[self.eval_coef(t) for t in t_values[r0:r1]])
+            with torch.cuda.device(dev):
+                _lib.check(L.cbg_bp_eval_loss_f32(
+                    C.byref(state['plan']), com_blob.data_ptr(), self.com_head.num_layers, coefs, n, x0.data_ptr(),
+                    v0.data_ptr(), pos_noise[r0:r1].data_ptr(), type_uniform[r0:r1].data_ptr(), xt[r0:r1].data_ptr(),
+                    vt[r0:r1].data_ptr(), mask[r0:r1].data_ptr(), vec[r0:r1].data_ptr(), c_pred[r0:r1].data_ptr(),
+                    rep_loss[r0:r1].data_ptr(), _lib.stream_ptr(dev)))
+        self.last_launches = L.cbg_launch_count() - launches0
+        per_t = rep_loss.cpu()
+        # get_dict_mean (common.py:33-42): mean over t of the per-t scalars, as a CPU float32 tensor
+        loss_dict = {k: torch.mean(torch.tensor(per_t[:, i].tolist())) for i, k in enumerate(('pos', 'atom', 'com', 'inter'))}
+        vt_onehot = F.one_hot(vt, K).float()
+        # the reference's key order: pos_info, then atom_info (its mask_gen, the type mask, replaces gen), then com_info
+        results = [{'eps_0': vec[r, 0], 'eps_pred': vec[r, 1], 'score_0': vec[r, 2], 'score_pred': vec[r, 3],
+                    'mask_gen': mask[r].bool(), 'v0': v0, 'vt': vt_onehot[r], 'c_pred': c_pred[r],
+                    'eps_0_com': vec[r, 4], 'eps_pred_com': vec[r, 5], 'score_0_com': vec[r, 6],
+                    'score_pred_com': vec[r, 7], 'mask_gen_com': gen} for r in range(R)]
+        return loss_dict, results
 
     @torch.no_grad()
     def run_steps(self, state, t_seq, X, Cc, pos_noise=None, type_uniform=None, eps_out=None):

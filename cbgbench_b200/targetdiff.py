@@ -111,6 +111,7 @@ class BaseDiffB200(nn.Module):
     ``prepare`` (batch -> device plan)."""
 
     allow_rcache = True      # samplers whose pocket atoms move between steps (DiffSBDD) turn the R-cache off
+    eval_max_nodes = 1 << 20    # composed nodes per validation-loss launch (about 9 GB of workspace at ~8.5 KB/node)
 
     def __init__(self, cfg):
         super().__init__()
@@ -156,6 +157,30 @@ class BaseDiffB200(nn.Module):
     def forward(self, batch):
         raise NotImplementedError(f'{type(self).__name__} is a sampling build: the training / validation losses of this '
                                   'model are not implemented on the CUDA path (DESIGN.md section 9)')
+
+    # ---- validation losses: what the eval-mode forwards share (replica batching, DESIGN.md section 13) --------------
+    _EVAL_KEYS = ('ligand_pos', 'ligand_atom_type', 'protein_pos', 'protein_atom_feature', 'protein_aa_type',
+                  'ligand_lig_flag', 'protein_lig_flag', 'ligand_element_batch', 'protein_element_batch',
+                  'ligand_gen_flag', 'protein_gen_flag')
+
+    def _eval_batch(self, batch, dev):
+        """The batch's tensors on ``dev`` (dict or attribute batch) and its graph count."""
+        g = lambda k, d=None: batch.get(k, d) if hasattr(batch, 'get') else (batch[k] if k in batch else d)
+        b = {k: g(k).to(dev) for k in self._EVAL_KEYS if g(k) is not None}
+        if b['ligand_pos'].shape[0] == 0:
+            raise ValueError('the batch has no ligand atoms')
+        n_graphs = int(torch.cat([b['ligand_element_batch'], b['protein_element_batch']]).max()) + 1
+        return b, n_graphs
+
+    def _eval_launches(self, b, n_graphs, R, max_nodes):
+        """Yield (r0, r1, state): replicas r0 .. r1-1 prepared as one plan of (r1 - r0) * n_graphs graphs, at most 64
+        replicas and ``max_nodes`` composed nodes (default ``eval_max_nodes``) per plan."""
+        n_nodes = b['ligand_pos'].shape[0] + b['protein_pos'].shape[0]
+        budget = self.eval_max_nodes if max_nodes is None else int(max_nodes)
+        per_launch = max(1, min(_lib.EVAL_MAX_REPLICAS, budget // n_nodes))
+        for r0 in range(0, R, per_launch):
+            r1 = min(R, r0 + per_launch)
+            yield r0, r1, self.prepare(replicate_batch(b, r1 - r0, n_graphs))
 
     # ---- setup of the step-invariant state ------------------------------------------------
     @torch.no_grad()
@@ -274,8 +299,6 @@ class TargetDiffB200(BaseDiffB200):
             log_one_minus_alpha=float(ts.host_table('log_one_minus_alphas_v')[t_idx]))
 
     # ---- validation loss (TargetDiff.forward with self.training == False) -------------------------------------------
-    eval_max_nodes = 1 << 20    # composed nodes per cbg_eval_loss_f32 launch (about 9 GB of workspace at ~8.5 KB/node)
-
     def forward(self, batch, pos_noise=None, type_uniform=None):
         """TargetDiff.forward (targetdiff.py:41-80).  Eval mode only: returns ``(loss_dict, results)`` for the
         ``eval_interval`` (default 10) timesteps ``np.linspace(0, T-1, eval_interval)`` truncated to integers, exactly
@@ -325,19 +348,11 @@ class TargetDiffB200(BaseDiffB200):
         dev = next(self.parameters()).device
         if dev.type != 'cuda':
             raise RuntimeError(f'{type(self).__name__}.forward needs the model on a CUDA device (no CPU fallback)')
-        g = lambda k, d=None: batch.get(k, d) if hasattr(batch, 'get') else (batch[k] if k in batch else d)
-        keys = ['ligand_pos', 'ligand_atom_type', 'protein_pos', 'protein_atom_feature', 'protein_aa_type',
-                'ligand_lig_flag', 'protein_lig_flag', 'ligand_element_batch', 'protein_element_batch',
-                'ligand_gen_flag', 'protein_gen_flag']
-        b = {k: g(k).to(dev) for k in keys if g(k) is not None}
+        b, n_graphs = self._eval_batch(batch, dev)
         x0 = b['ligand_pos'].float().contiguous()
         v0 = b['ligand_atom_type'].long().contiguous()
         mask_gen = b['ligand_gen_flag'].bool() if 'ligand_gen_flag' in b else b['ligand_lig_flag'].bool()
         n_lig = x0.shape[0]
-        if n_lig == 0:
-            raise ValueError('the batch has no ligand atoms')
-        n_nodes = n_lig + b['protein_pos'].shape[0]
-        n_graphs = int(torch.cat([b['ligand_element_batch'], b['protein_element_batch']]).max()) + 1
         if pos_noise is None or type_uniform is None:
             draws = [(torch.randn(n_lig, 3, device=dev), torch.rand(n_lig, K, device=dev)) for _ in range(R)]
             pos_noise = torch.stack([d[0] for d in draws]) if pos_noise is None else pos_noise
@@ -350,14 +365,10 @@ class TargetDiffB200(BaseDiffB200):
         x_pred = torch.empty(R, n_lig, 3, device=dev)
         c_pred = torch.empty(R, n_lig, K, device=dev)
         rep_loss = torch.empty(R, 2, device=dev)
-        budget = self.eval_max_nodes if max_nodes is None else int(max_nodes)
-        per_launch = max(1, min(_lib.EVAL_MAX_REPLICAS, budget // n_nodes))
         L = _lib.lib()
         launches0 = L.cbg_launch_count()
-        for r0 in range(0, R, per_launch):
-            r1 = min(R, r0 + per_launch)
+        for r0, r1, state in self._eval_launches(b, n_graphs, R, max_nodes):
             n = r1 - r0
-            state = self.prepare(replicate_batch(b, n, n_graphs))
             coefs = (_lib.EvalCoef * n)(*[self.eval_coef(t) for t in t_values[r0:r1]])
             graph_loss = torch.empty(n * n_graphs, 2, device=dev)
             with torch.cuda.device(dev):

@@ -300,6 +300,34 @@ int32_t cbg_bp_step_f32(const cbg_sample_plan* plan, const float* com_blob, int3
                         float* eps_out /*[n_lig,3] or NULL: eps + eps_com*/, float* logits /*[n_lig,K] or NULL*/,
                         void* stream);
 
+/* ---- validation loss: DiffBP.forward in eval mode (diffbp.py:133-230) ------------------------------------------------
+ *
+ * Same replica layout as cbg_eval_loss_f32 (graph r*B + g and ligand atom r*(n_lig/n_rep) + a of the plan are graph g
+ * and atom a of the batch).  One call enqueues: forward noising of positions with the raw normal draw
+ * (CTNVPScheduler.forward_add_noise, zero_center=True) and the absorbing-state type mask (MaskTypeSchedule.
+ * forward_add_noise) -> the denoiser -> classifier -> the CoM head of cbg_bp_step_f32 on the noised coordinates ->
+ * per-graph position / CoM score losses, masked-type cross-entropy of softmax(logits) and the interior loss
+ * (diffbp.py:19-30: for each protein atom its min(48, n_lig_g) nearest ligand atoms of the graph at the posterior
+ * mean of x_{t-1}, nearest first, ties to the lower ligand index) -> per-replica reduction.  No atomics: repeated calls
+ * are bit-identical. */
+typedef struct cbg_bp_eval_coef {  /* one replica's timestep t */
+  float alphas_cumprod;            /* pos_scheduler.alphas_cumprod[t] */
+  float beta;                      /* pos_scheduler.betas[t] */
+  float mask_prob;                 /* float(t) / T in fp32: probability that a generated atom is masked */
+} cbg_bp_eval_coef;
+
+/* coefs: host array [n_rep], n_rep <= 64.  com_blob / com_layers as in cbg_bp_step_f32.  x0 / v0: the batch's
+ * ligand_pos [n_lig/n_rep,3] / ligand_atom_type.  Draws from the caller: pos_noise [n_rep, n_lig/n_rep, 3] (normal),
+ * type_uniform [n_rep, n_lig/n_rep] (uniform).  Outputs: xt [n_rep, n_lig/n_rep, 3]; vt / mask [n_rep, n_lig/n_rep]
+ * (the noised type and the type mask); vec [n_rep, 8, n_lig/n_rep, 3] = eps_0, eps_pred, score_0, score_pred,
+ * eps_0_com, eps_pred_com, score_0_com, score_pred_com (score = eps * sqrt(1 - alphas_cumprod)); c_pred = softmax(logits)
+ * [n_rep, n_lig/n_rep, K]; rep_loss [n_rep, 4] = pos, atom, com, inter (pos / com NaN when no atom is generated, atom 0
+ * when no atom is masked). */
+int32_t cbg_bp_eval_loss_f32(const cbg_sample_plan* plan, const float* com_blob, int32_t com_layers,
+                             const cbg_bp_eval_coef* coefs, int32_t n_rep, const float* x0, const int64_t* v0,
+                             const float* pos_noise, const float* type_uniform, float* xt, int64_t* vt, uint8_t* mask,
+                             float* vec, float* c_pred, float* rep_loss, void* stream);
+
 /* ---- SURVEY.md section 8 row f3: sampling-time transforms + batch construction on the device ------------------
  *
  * The reference builds a sampling batch by evaluating dataset[i] num_samples times (sample.py:177), i.e. by running
