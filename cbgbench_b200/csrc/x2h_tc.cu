@@ -19,9 +19,9 @@
 // persistent CTA (bulk copies, mbarrier).  Nothing of size [E, 128] touches HBM and no R-cache is needed: the only
 // per-edge gather is the 512-byte Pj row, read in the accumulator layout (a quad of lanes = one 32-byte sector of a row).
 // In that layout a row's 128 columns live in the 4 lanes of a quad, so LayerNorm is two shuffles, and a head's 8 columns
-// are one quad's registers, so <q_i, k> per head is two shuffles as well; the softmax over a node's 32 edges (2 warps)
-// and the sum over them go through a small shared-memory buffer.  The two warpgroups only share the weights: each walks
-// its own 2 nodes of every tile, and while one waits on its MMAs or gathers the other one computes.
+// are one quad's registers, so <q_i, k> per head is a reduction over the quad as well; the softmax over a node's 32
+// edges (2 warps) and the sum over them go through a small shared-memory buffer.  The two warpgroups only share the
+// weights: each walks its own 2 nodes of every tile, and while one waits on its MMAs or gathers the other one computes.
 //
 // H2X (repo/modules/attention/h2x_attention.py:34-73) runs on the same kernel over the list of generated nodes:
 //   launch 1  MODE_K with the xk / xq weights -> w = alpha * e_w (compact buffer, indexed by list position)
@@ -110,6 +110,28 @@ __device__ __forceinline__ float rows_sum(float v) {        // over the 8 row gr
   v += __shfl_xor_sync(CBG_FULL, v, 4);
   v += __shfl_xor_sync(CBG_FULL, v, 8);
   return v + __shfl_xor_sync(CBG_FULL, v, 16);
+}
+// Reduce-scatter of a[0 .. N) over the lanes that differ in lane bits LB .. LB + LEVELS - 1, for epilogues where each
+// sum is stored by one lane only.  Level l pairs the lanes as the butterfly's xor (1 << (LB + l)) does; each lane sends
+// the half of its values whose index bit IB differs from its lane bit LB + l and adds the partner's copy of the half it
+// keeps, own + partner as in the butterfly.  So every kept value is the same fp32 sum tree, bit for bit, that
+// quad_sum / rows_sum leave in every lane; which lane keeps which value only decides where its store comes from.  The kept
+// values are compacted in place (index bit IB removed, higher bits shift down): afterwards a lane holds a[0 .. N >> LEVELS),
+// the values whose original index bits IB .. IB + LEVELS - 1 equal its lane bits LB .. LB + LEVELS - 1.
+// N (1 - 2^-LEVELS) shuffles instead of the butterfly's N LEVELS; fully unrolled, constant indices: registers only.
+// (One level per instantiation, so that every loop has a constant trip count and the array stays in registers.)
+template <int IB, int LB, int LEVELS, int N, int LIVE = N>
+__device__ __forceinline__ void reduce_scatter(float (&a)[N], int lane) {
+  static_assert((LIVE >> LEVELS) << LEVELS == LIVE && (LIVE >> LEVELS) >= (1 << IB), "reduce_scatter shape");
+  const bool up = (lane >> LB) & 1;
+#pragma unroll
+  for (int o = 0; o < LIVE / 2; ++o) {      // o <= i0 < i1: the in-place write never clobbers a later read
+    const int i0 = ((o >> IB) << (IB + 1)) | (o & ((1 << IB) - 1)), i1 = i0 | (1 << IB);
+    const float give = up ? a[i0] : a[i1];
+    const float keep = up ? a[i1] : a[i0];
+    a[o] = keep + __shfl_xor_sync(CBG_FULL, give, 1 << LB);
+  }
+  if constexpr (LEVELS > 1) reduce_scatter<IB, LB + 1, LEVELS - 1, N, LIVE / 2>(a, lane);
 }
 __device__ __forceinline__ float2 ldg2(const float* p) { return __ldg(reinterpret_cast<const float2*>(p)); }
 
@@ -398,16 +420,22 @@ __global__ void __launch_bounds__(256, 1) x2h_tc_kernel(EdgeArgs p, TcWeights W)
       float o[64];
       issue_mma2(o);
       advance(o);
-      float* s_sm = s_epi + slot * (32 * 17);              // [edge][17]: conflict-free rows
+      float* s_sm = s_epi + slot * (32 * 17);              // [edge][17]: the softmax reads it without bank conflicts
+      // heads 4 m .. 4 m + 3 at a time: the quad's partial dot products are reduce-scattered over the quad, lane qt keeps
+      // head 4 m + qt of both rows (these stores have two-way bank conflicts; the rows stay padded to 17 for the softmax)
 #pragma unroll
-      for (int j = 0; j < 16; ++j) {
-        const float l0 = quad_sum(fmaf(o[4 * j + 1], qv[2 * j + 1], o[4 * j] * qv[2 * j]));
-        const float l1 = quad_sum(fmaf(o[4 * j + 3], qv[2 * j + 1], o[4 * j + 2] * qv[2 * j]));
-        if ((j & 3) == qt) {
-          s_sm[e0 * 17 + j] = tj0 >= 0 ? l0 * kInvOut : -INFINITY;
-          s_sm[(e0 + 8) * 17 + j] = tj1 >= 0 ? l1 * kInvOut : -INFINITY;
+      for (int m = 0; m < 4; ++m) {
+        float lg[8];                                       // [head 4 m + jj][row e0 | e0 + 8]
+#pragma unroll
+        for (int jj = 0; jj < 4; ++jj) {
+          const int j = 4 * m + jj;
+          lg[2 * jj] = fmaf(o[4 * j + 1], qv[2 * j + 1], o[4 * j] * qv[2 * j]);
+          lg[2 * jj + 1] = fmaf(o[4 * j + 3], qv[2 * j + 1], o[4 * j + 2] * qv[2 * j]);
+          gather_next(j);
         }
-        gather_next(j);
+        reduce_scatter<1, 0, 2>(lg, lane);                 // xor 1, xor 2: quad_sum's tree
+        s_sm[e0 * 17 + 4 * m + qt] = tj0 >= 0 ? lg[0] * kInvOut : -INFINITY;
+        s_sm[(e0 + 8) * 17 + 4 * m + qt] = tj1 >= 0 ? lg[1] * kInvOut : -INFINITY;
       }
       warpgroup_sync(wg);
       {
@@ -447,13 +475,21 @@ __global__ void __launch_bounds__(256, 1) x2h_tc_kernel(EdgeArgs p, TcWeights W)
       issue_mma2(o);
       advance(o);
       float* s_vr = s_epi + (slot * 2 + wp) * CBG_H;       // this warp's 16-edge partial sums
+      // columns 64 b .. 64 b + 63 at a time: the per-row terms are reduce-scattered over the warp's 8 row groups, lane qg
+      // keeps column group 8 b + qg (one conflict-free float2 row store per half)
 #pragma unroll
-      for (int j = 0; j < 16; ++j) {
-        const float2 b1 = *reinterpret_cast<const float2*>(s_b1 + 8 * j + 2 * qt);
-        const float sx = rows_sum(fmaf(fmaf(o[4 * j + 2], kInvOut, b1.x), wv[1][j], fmaf(o[4 * j], kInvOut, b1.x) * wv[0][j]));
-        const float sy = rows_sum(fmaf(fmaf(o[4 * j + 3], kInvOut, b1.y), wv[1][j], fmaf(o[4 * j + 1], kInvOut, b1.y) * wv[0][j]));
-        if ((j >> 1) == qg) *reinterpret_cast<float2*>(s_vr + 8 * j + 2 * qt) = make_float2(sx, sy);
-        gather_next(j);
+      for (int b = 0; b < 2; ++b) {
+        float s[16];                                       // [column group 8 b + jj][column 2 qt | 2 qt + 1]
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj) {
+          const int j = 8 * b + jj;
+          const float2 b1 = *reinterpret_cast<const float2*>(s_b1 + 8 * j + 2 * qt);
+          s[2 * jj] = fmaf(fmaf(o[4 * j + 2], kInvOut, b1.x), wv[1][j], fmaf(o[4 * j], kInvOut, b1.x) * wv[0][j]);
+          s[2 * jj + 1] = fmaf(fmaf(o[4 * j + 3], kInvOut, b1.y), wv[1][j], fmaf(o[4 * j + 1], kInvOut, b1.y) * wv[0][j]);
+          gather_next(j);
+        }
+        reduce_scatter<1, 2, 3>(s, lane);                  // xor 4, 8, 16: rows_sum's tree
+        *reinterpret_cast<float2*>(s_vr + 64 * b + 8 * qg + 2 * qt) = make_float2(s[0], s[1]);
       }
       warpgroup_sync(wg);
       if (live) {
