@@ -118,23 +118,65 @@ int check_ws(const void* workspace, size_t have, long long n_nodes, long long n_
   return 0;
 }
 
-// node GEMM implementation: wgmma f16 with the (hi, lo) split (default), CBG_NODE_GEMM=tf32 the 3xTF32
-// kernel, CBG_NODE_GEMM=simt the fp32 SIMT kernel
-int node_gemm_impl() {
-  static int impl = -1;
-  if (impl < 0) {
-    const char* e = getenv("CBG_NODE_GEMM");
-    impl = (e && strcmp(e, "simt") == 0) ? 0 : ((e && strcmp(e, "tf32") == 0) ? 1 : 2);
-  }
-  return impl;
+// The CBG_* switches of the orchestration, read from the environment once per process (on first use).  "0" turns a
+// default-on switch off.
+struct Switches {
+  int node_gemm;      // CBG_NODE_GEMM: simt 0 (fp32 SIMT), tf32 1 (3xTF32), anything else 2 (wgmma f16, (hi, lo) split)
+  bool overlap;       // CBG_OVERLAP: side streams (AuxStream) instead of the caller's stream alone
+  bool prune;         // CBG_PRUNE: receptive-field pruning of the sampling step (exact)
+  bool gate_compact;  // CBG_GATE_COMPACT: compact the moving edges before their gates (ws.w is free until the first X2H)
+  bool dyn_sched;     // CBG_DYN_SCHED: dynamic node scheduling of the X2H kernels (work counters), else round-robin
+  bool static_fast;   // CBG_STATIC_FAST: edge_setup fast path for nodes whose 32 in-edges are all static (R-cache)
+};
+bool env_on(const char* name) {
+  const char* e = getenv(name);
+  return !(e && strcmp(e, "0") == 0);
 }
+Switches& switches() {
+  static Switches s = [] {
+    const char* g = getenv("CBG_NODE_GEMM");
+    const int node_gemm = (g && strcmp(g, "simt") == 0) ? 0 : ((g && strcmp(g, "tf32") == 0) ? 1 : 2);
+    return Switches{node_gemm, env_on("CBG_OVERLAP"), env_on("CBG_PRUNE"), env_on("CBG_GATE_COMPACT"),
+                    env_on("CBG_DYN_SCHED"), env_on("CBG_STATIC_FAST")};
+  }();
+  return s;
+}
+
 int launch_node_gemm(const NodeGemmArgs& a, cudaStream_t st) {
-  const int impl = node_gemm_impl();
+  const int impl = switches().node_gemm;
   return impl == 2 ? cbg_launch_node_gemm_f16(a, st) : (impl == 1 ? cbg_launch_node_gemm_tc(a, st) : cbg_launch_node_gemm(a, st));
 }
 
-// Second stream for the H2X chain of layer l, which overlaps the X2H node GEMM of layer l+1
-// (that GEMM needs only h).  Fork/join with two events; CBG_OVERLAP=0 keeps everything on one stream.
+// The node projections of one sub-layer (cbg_layout.h): five planes pj_k, pj_v, pi_k, pi_v, q, the last one through
+// the q head (LN -> ReLU -> second Linear).  A launch computes all of them, the source planes Pj (0..1) or the
+// destination planes Pi / q (2..4).
+enum SubLayer { kX2H = 0, kH2X = 1 };
+enum class Planes { kAll, kSrc, kDst };
+NodeGemmArgs node_gemm_args(const float* L, SubLayer sub, Planes shape, const float* a, const int* row_idx, int n_rows,
+                            float* const planes[CBG_NPLANES]) {
+  auto field = [&](int x2h, int h2x) { return L + cbg_layout::layer_offset(sub == kX2H ? x2h : h2x); };
+  const int first = shape == Planes::kDst ? 2 : 0;
+  NodeGemmArgs g{};
+  g.a = a; g.row_idx = row_idx; g.n_rows = n_rows;
+  g.wt = field(CBG_LF_X2H_NODE_WT, CBG_LF_H2X_NODE_WT) + first * CBG_H;
+  g.bias = field(CBG_LF_X2H_NODE_B, CBG_LF_H2X_NODE_B) + first * CBG_H;
+  g.ldw = 640;
+  g.n_planes = shape == Planes::kAll ? 5 : (shape == Planes::kSrc ? 2 : 3);
+  g.has_q = shape != Planes::kSrc;
+  for (int p = 0; p < g.n_planes - g.has_q; ++p) g.out[p] = planes[first + p];
+  if (g.has_q) {
+    g.q_ln = field(CBG_LF_X2H_Q_LN, CBG_LF_H2X_Q_LN);
+    g.q_w1t = field(CBG_LF_X2H_Q_W1T, CBG_LF_H2X_Q_W1T);
+    g.q_b1 = field(CBG_LF_X2H_Q_B1, CBG_LF_H2X_Q_B1);
+    g.out_q = planes[4];
+  }
+  g.tc_planes = field(CBG_LF_X2H_NODE_TC, CBG_LF_H2X_NODE_TC); g.tc_first_plane = first;
+  g.tch_planes = field(CBG_LF_X2H_NODE_TCH, CBG_LF_H2X_NODE_TCH);
+  return g;
+}
+
+// Side streams of the denoiser pass: the H2X chain of layer l overlaps the X2H node GEMM of layer l+1 (that GEMM needs
+// only h).  Fork/join with events.
 struct AuxStream {
   cudaStream_t s2 = nullptr, s3 = nullptr, s4 = nullptr;   // H2X chain, X2H source-plane GEMM, H2X destination GEMM
   cudaEvent_t ev_h = nullptr, ev_x = nullptr, ev_h0 = nullptr, ev_p = nullptr, ev_gi = nullptr;
@@ -142,244 +184,190 @@ struct AuxStream {
 };
 constexpr int kMaxDevices = 64;
 AuxStream g_aux_dev[kMaxDevices];   // streams and events belong to a device: one set per device the caller uses
-AuxStream g_aux_off;                // state 0: what aux() returns when overlap is unavailable
-#define g_aux (*g_aux_cur)
-thread_local AuxStream* g_aux_cur = &g_aux_off;
 
-int aux_ready() {
+// The current device's side streams (created on first use), or nullptr when overlap is off or unavailable.
+AuxStream* aux_streams() {
   int dev = -1;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= kMaxDevices) { g_aux_cur = &g_aux_off; g_aux_off.state = 0; return 0; }
-  g_aux_cur = &g_aux_dev[dev];
-  if (g_aux.state >= 0) return g_aux.state;
-  const char* e = getenv("CBG_OVERLAP");
-  if (e && strcmp(e, "0") == 0) { g_aux.state = 0; return 0; }
-  if (cudaStreamCreateWithFlags(&g_aux.s2, cudaStreamNonBlocking) != cudaSuccess ||
-      cudaStreamCreateWithFlags(&g_aux.s3, cudaStreamNonBlocking) != cudaSuccess ||
-      cudaStreamCreateWithFlags(&g_aux.s4, cudaStreamNonBlocking) != cudaSuccess ||
-      cudaEventCreateWithFlags(&g_aux.ev_h, cudaEventDisableTiming) != cudaSuccess ||
-      cudaEventCreateWithFlags(&g_aux.ev_x, cudaEventDisableTiming) != cudaSuccess ||
-      cudaEventCreateWithFlags(&g_aux.ev_h0, cudaEventDisableTiming) != cudaSuccess ||
-      cudaEventCreateWithFlags(&g_aux.ev_p, cudaEventDisableTiming) != cudaSuccess ||
-      cudaEventCreateWithFlags(&g_aux.ev_gi, cudaEventDisableTiming) != cudaSuccess) {
-    g_aux.state = 0;
-    return 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= kMaxDevices) return nullptr;
+  AuxStream& a = g_aux_dev[dev];
+  if (a.state < 0) {
+    a.state = switches().overlap &&
+              cudaStreamCreateWithFlags(&a.s2, cudaStreamNonBlocking) == cudaSuccess &&
+              cudaStreamCreateWithFlags(&a.s3, cudaStreamNonBlocking) == cudaSuccess &&
+              cudaStreamCreateWithFlags(&a.s4, cudaStreamNonBlocking) == cudaSuccess &&
+              cudaEventCreateWithFlags(&a.ev_h, cudaEventDisableTiming) == cudaSuccess &&
+              cudaEventCreateWithFlags(&a.ev_x, cudaEventDisableTiming) == cudaSuccess &&
+              cudaEventCreateWithFlags(&a.ev_h0, cudaEventDisableTiming) == cudaSuccess &&
+              cudaEventCreateWithFlags(&a.ev_p, cudaEventDisableTiming) == cudaSuccess &&
+              cudaEventCreateWithFlags(&a.ev_gi, cudaEventDisableTiming) == cudaSuccess;
   }
-  g_aux.state = 1;
-  return 1;
+  return a.state ? &a : nullptr;
 }
 
-// receptive-field pruning of the sampling step (exact); CBG_PRUNE=0 turns it off
-bool prune_enabled() {
-  static int on = -1;
-  if (on < 0) {
-    const char* e = getenv("CBG_PRUNE");
-    on = (e && strcmp(e, "0") == 0) ? 0 : 1;
+// Receptive-field pruning of a plan's denoiser pass (only when the caller consumes nothing but the generated /
+// classified rows): layer l updates h only for the nodes that can still reach such a row through the remaining layers.
+bool plan_prunes(const cbg_sample_plan& p) {
+  return p.prune != 0 && switches().prune && p.num_layers > 0 && (p.n_gen > 0 || p.n_lig > 0);
+}
+
+// One H2X sub-layer on the current h and the layer-input x: source planes Pj for all nodes, or for the first
+// *src_rows_dev nodes of ws.order (pruned: the generated atoms and their neighbours), destination planes Pi / q for the
+// generated nodes, then their coordinate update.  With side streams the destination GEMM runs on aux->s4 beside the
+// source GEMM (both wait for the caller's fork) and the rest on st.
+int run_h2x(const float* L, const Workspace& ws, long long n_nodes, const int* gen_idx, int n_gen,
+            const int* src_rows_dev, const AuxStream* aux, cudaStream_t st) {
+  NodeGemmArgs gj = node_gemm_args(L, kH2X, Planes::kSrc, ws.h, src_rows_dev ? ws.order : nullptr, (int)n_nodes, ws.hplane);
+  gj.n_rows_dev = src_rows_dev;
+  if (int rc = launch_node_gemm(gj, st)) return rc;
+  const NodeGemmArgs gi = node_gemm_args(L, kH2X, Planes::kDst, ws.h, gen_idx, n_gen, ws.hplane);
+  if (int rc = launch_node_gemm(gi, aux ? aux->s4 : st)) return rc;
+  if (aux) {
+    CBG_CUDA_OK(cudaEventRecord(aux->ev_gi, aux->s4));
+    CBG_CUDA_OK(cudaStreamWaitEvent(st, aux->ev_gi, 0));
   }
-  return on != 0;
+  EdgeArgs x{};
+  x.x4 = ws.x4; x.nbr = ws.nbr; x.ew = ws.ew;
+  x.pj_k = ws.hplane[0]; x.pj_v = ws.hplane[1]; x.pi_k = ws.hplane[2]; x.pi_v = ws.hplane[3]; x.q = ws.hplane[4];
+  x.layer = L; x.h = ws.h; x.node_idx = gen_idx; x.n_nodes = n_gen; x.dx = ws.dx;
+  x.w = ws.hw;        // the X2H kernels of the next layer use ws.w while this chain runs
+  if (int rc = cbg_launch_h2x(x, st)) return rc;
+  return cbg_launch_apply_dx(ws.x4, gen_idx, ws.dx, n_gen, st);
 }
 
-// compact the moving edges before computing their gates (ws.w is free until the first X2H): CBG_GATE_COMPACT=0
-// keeps the in-place kernel
-bool gate_compact() {
-  static int on = -1;
-  if (on < 0) { const char* e = getenv("CBG_GATE_COMPACT"); on = (e && strcmp(e, "0") == 0) ? 0 : 1; }
-  return on != 0;
-}
-
-// fast path of edge_setup for nodes whose 32 in-edges are all static (needs the R-cache): CBG_STATIC_FAST=0 turns it off
-// dynamic node scheduling of the X2H kernels (work counters); CBG_DYN_SCHED=0 keeps the static round-robin
-int g_dyn_sched = -1;
-bool dyn_sched() {
-  if (g_dyn_sched < 0) { const char* e = getenv("CBG_DYN_SCHED"); g_dyn_sched = (e && strcmp(e, "0") == 0) ? 0 : 1; }
-  return g_dyn_sched != 0;
-}
-int g_static_fast = -1;
-bool static_fast_path() {
-  if (g_static_fast < 0) { const char* e = getenv("CBG_STATIC_FAST"); g_static_fast = (e && strcmp(e, "0") == 0) ? 0 : 1; }
-  return g_static_fast != 0;
-}
-
-// graph build + gate + layers on an initialised workspace (x4, h valid)
-int run_core(const float* blob, int num_layers, const Workspace& ws, const int* graph_ptr, int n_graphs,
-             int max_graph_nodes, long long n_nodes, const int* gen_idx, int n_gen, int mode, int k,
-             float r_max, const float* rcache, const int* cls_idx, int n_cls, bool prune, cudaStream_t st,
-             bool static_lists = false) {
-  static_lists = static_lists || rcache != nullptr;      // the R-cache is indexed by the static lists
+// The denoiser pass of a plan on an initialised workspace (x4, h valid): graph build, edge gate, the layers.  The
+// classified rows are the plan's ligand rows.
+int run_denoiser(const cbg_sample_plan& p, const Workspace& ws, cudaStream_t st) {
   // One set of side streams / fork-join events per device (g_aux_dev): two host threads enqueueing denoiser passes on the
   // same GPU must not interleave their cudaEventRecord / cudaStreamWaitEvent pairs.  Enqueueing is serialised here; the
   // GPU work itself still overlaps across the callers' streams.
   static std::mutex core_mutex;
   std::lock_guard<std::mutex> core_lock(core_mutex);
   NvtxRange nvtx_core("cbg:denoiser");
+  const long long n_nodes = p.n_nodes;
+  const int num_layers = p.num_layers, n_gen = p.n_gen;
+  const bool static_lists = p.static_lists != 0 || p.rcache != nullptr;   // the R-cache is indexed by the static lists
   if (n_nodes > 0x7fffffffLL / (CBG_KMAX * CBG_HEADS)) { cbg_set_error("n_nodes too large for 32-bit indexing"); return 1; }
-  if (int rc = cbg_launch_knn(ws.x4, graph_ptr, n_graphs, max_graph_nodes, mode, k, r_max, 0, static_lists ? ws.snbr : nullptr, ws.nbr, st)) return rc;
-  const float* layers = blob + cbg_layout::kGlobalFloats;
-  // Receptive-field pruning (only when the caller consumes nothing but the generated / classified rows):
-  // layer l updates h only for the nodes that can still reach such a row through the remaining layers.
-  prune = prune && num_layers > 0 && (n_gen > 0 || n_cls > 0);
-  const bool overlap = (n_gen > 0) && aux_ready();
-  const bool tickets = dyn_sched() && 2 * num_layers <= 64;
+  if (int rc = cbg_launch_knn(ws.x4, p.graph_ptr, p.n_graphs, p.max_graph_nodes, p.mode, p.k, p.r_max, 0,
+                              static_lists ? ws.snbr : nullptr, ws.nbr, st)) return rc;
+  const float* layers = p.blob + cbg_layout::kGlobalFloats;
+  const bool prune = plan_prunes(p);
+  AuxStream* const aux = n_gen > 0 ? aux_streams() : nullptr;
+  const bool tickets = switches().dyn_sched && 2 * num_layers <= 64;
   if (tickets) CBG_CUDA_OK(cudaMemsetAsync(ws.tickets, 0, 64 * sizeof(int), st));
   // the edge gate and the pruning BFS both need only the neighbour table: run them side by side
-  const bool fork_depth = prune && overlap;
+  const bool fork_depth = prune && aux;
   if (fork_depth) {
-    CBG_CUDA_OK(cudaEventRecord(g_aux.ev_h0, st));
-    CBG_CUDA_OK(cudaStreamWaitEvent(g_aux.s3, g_aux.ev_h0, 0));
+    CBG_CUDA_OK(cudaEventRecord(aux->ev_h0, st));
+    CBG_CUDA_OK(cudaStreamWaitEvent(aux->s3, aux->ev_h0, 0));
   }
   if (prune) {
-    if (int rc = cbg_launch_depth(ws.nbr, graph_ptr, n_graphs, max_graph_nodes, n_nodes, gen_idx, n_gen, cls_idx, n_cls,
-                                  num_layers, ws.depth, ws.order, ws.cnt, fork_depth ? g_aux.s3 : st)) return rc;
+    if (int rc = cbg_launch_depth(ws.nbr, p.graph_ptr, p.n_graphs, p.max_graph_nodes, n_nodes, p.gen_node, n_gen,
+                                  p.lig_node, p.n_lig, num_layers, ws.depth, ws.order, ws.cnt,
+                                  fork_depth ? aux->s3 : st)) return rc;
   }
-  if (fork_depth) CBG_CUDA_OK(cudaEventRecord(g_aux.ev_p, g_aux.s3));
-  if (int rc = cbg_launch_edge_gate(blob, ws.x4, ws.nbr, n_nodes, static_lists ? ws.sew : nullptr,
-                                    gate_compact() ? (int*)ws.w : nullptr, ws.ew, st, ws.fstat)) return rc;
-  if (fork_depth) CBG_CUDA_OK(cudaStreamWaitEvent(st, g_aux.ev_p, 0));
-  cudaStream_t sx = overlap ? g_aux.s2 : st;       // stream of the H2X chain
+  if (fork_depth) CBG_CUDA_OK(cudaEventRecord(aux->ev_p, aux->s3));
+  if (int rc = cbg_launch_edge_gate(p.blob, ws.x4, ws.nbr, n_nodes, static_lists ? ws.sew : nullptr,
+                                    switches().gate_compact ? (int*)ws.w : nullptr, ws.ew, st, ws.fstat)) return rc;
+  if (fork_depth) CBG_CUDA_OK(cudaStreamWaitEvent(st, aux->ev_p, 0));
+  cudaStream_t sx = aux ? aux->s2 : st;            // stream of the H2X chain
   bool x_pending = false;                          // an apply_dx on sx has not been joined yet
   for (int l = 0; l < num_layers; ++l) {
     const float* L = layers + (size_t)l * cbg_layout::kLayerFloats;
     NvtxRange nvtx_layer("cbg:layer");
     // ---- X2H: node planes, attention weights, aggregation (h updated in place)
-    NodeGemmArgs g{};
-    g.a = ws.h; g.row_idx = nullptr; g.n_rows = (int)n_nodes;
-    g.wt = L + cbg_layout::layer_offset(CBG_LF_X2H_NODE_WT);
-    g.bias = L + cbg_layout::layer_offset(CBG_LF_X2H_NODE_B);
-    g.ldw = 640; g.n_planes = 5; g.has_q = 1;
-    for (int p = 0; p < 4; ++p) g.out[p] = ws.plane[p];
-    g.out[4] = nullptr;
-    g.q_ln = L + cbg_layout::layer_offset(CBG_LF_X2H_Q_LN);
-    g.q_w1t = L + cbg_layout::layer_offset(CBG_LF_X2H_Q_W1T);
-    g.q_b1 = L + cbg_layout::layer_offset(CBG_LF_X2H_Q_B1);
-    g.out_q = ws.plane[4];
-    g.tc_planes = L + cbg_layout::layer_offset(CBG_LF_X2H_NODE_TC); g.tc_first_plane = 0;
-    g.tch_planes = L + cbg_layout::layer_offset(CBG_LF_X2H_NODE_TCH);
     if (!prune) {
+      const NodeGemmArgs g = node_gemm_args(L, kX2H, Planes::kAll, ws.h, nullptr, (int)n_nodes, ws.plane);
       if (int rc = launch_node_gemm(g, st)) return rc;          // reads h only: may overlap the previous H2X chain
-    } else if (node_gemm_impl() == 2) {
+    } else if (switches().node_gemm == 2) {
       // one launch: source planes Pj for every node a needed destination can gather (depth >= l-1), destination planes
       // Pi / q for the needed destinations only (depth >= l); both lists are prefixes of ws.order
-      NodeGemmArgs gm = g;
-      gm.row_idx = ws.order; gm.n_rows_dev = ws.cnt + l; gm.n_dst_dev = ws.cnt + l + 1;
-      if (int rc = launch_node_gemm(gm, st)) return rc;
+      NodeGemmArgs g = node_gemm_args(L, kX2H, Planes::kAll, ws.h, ws.order, (int)n_nodes, ws.plane);
+      g.n_rows_dev = ws.cnt + l; g.n_dst_dev = ws.cnt + l + 1;
+      if (int rc = launch_node_gemm(g, st)) return rc;
     } else {
-      NodeGemmArgs gp = g;
-      gp.row_idx = ws.order; gp.n_rows_dev = ws.cnt + l; gp.n_planes = 2; gp.has_q = 0;
-      const bool fork_p = overlap;          // the two X2H GEMMs only read h: run them side by side
-      if (fork_p) {
-        CBG_CUDA_OK(cudaEventRecord(g_aux.ev_h0, st));
-        CBG_CUDA_OK(cudaStreamWaitEvent(g_aux.s3, g_aux.ev_h0, 0));
+      NodeGemmArgs gp = node_gemm_args(L, kX2H, Planes::kSrc, ws.h, ws.order, (int)n_nodes, ws.plane);
+      gp.n_rows_dev = ws.cnt + l;
+      if (aux) {                            // the two X2H GEMMs only read h: run them side by side
+        CBG_CUDA_OK(cudaEventRecord(aux->ev_h0, st));
+        CBG_CUDA_OK(cudaStreamWaitEvent(aux->s3, aux->ev_h0, 0));
       }
-      if (int rc = launch_node_gemm(gp, fork_p ? g_aux.s3 : st)) return rc;
-      if (fork_p) CBG_CUDA_OK(cudaEventRecord(g_aux.ev_p, g_aux.s3));
-      NodeGemmArgs gd = g;
-      gd.row_idx = ws.order; gd.n_rows_dev = ws.cnt + l + 1;
-      gd.wt = g.wt + 256; gd.bias = g.bias + 256; gd.n_planes = 3; gd.tc_first_plane = 2;
-      gd.out[0] = ws.plane[2]; gd.out[1] = ws.plane[3]; gd.out[2] = nullptr;
+      if (int rc = launch_node_gemm(gp, aux ? aux->s3 : st)) return rc;
+      if (aux) CBG_CUDA_OK(cudaEventRecord(aux->ev_p, aux->s3));
+      NodeGemmArgs gd = node_gemm_args(L, kX2H, Planes::kDst, ws.h, ws.order, (int)n_nodes, ws.plane);
+      gd.n_rows_dev = ws.cnt + l + 1;
       if (int rc = launch_node_gemm(gd, st)) return rc;
-      if (fork_p) CBG_CUDA_OK(cudaStreamWaitEvent(st, g_aux.ev_p, 0));
+      if (aux) CBG_CUDA_OK(cudaStreamWaitEvent(st, aux->ev_p, 0));
     }
-    if (overlap && x_pending) { CBG_CUDA_OK(cudaStreamWaitEvent(st, g_aux.ev_x, 0)); x_pending = false; }
+    if (aux && x_pending) { CBG_CUDA_OK(cudaStreamWaitEvent(st, aux->ev_x, 0)); x_pending = false; }
     EdgeArgs e{};
     e.x4 = ws.x4; e.nbr = ws.nbr; e.ew = ws.ew;
     e.pj_k = ws.plane[0]; e.pj_v = ws.plane[1]; e.pi_k = ws.plane[2]; e.pi_v = ws.plane[3]; e.q = ws.plane[4];
     e.layer = L; e.w = ws.w; e.h = ws.h; e.node_idx = nullptr; e.n_nodes = (int)n_nodes; e.dx = nullptr;
     if (prune) { e.node_idx = ws.order; e.n_nodes_dev = ws.cnt + l + 1; }
     if (tickets) e.ticket = ws.tickets + 2 * l;
-    if (rcache) {
+    if (p.rcache) {
       const size_t per = (size_t)n_nodes * (CBG_KMAX * CBG_H);
-      e.rc_k = rcache + (size_t)(2 * l) * per;
-      e.rc_v = rcache + (size_t)(2 * l + 1) * per;
-      e.fstat = static_fast_path() ? ws.fstat : nullptr;
+      e.rc_k = p.rcache + (size_t)(2 * l) * per;
+      e.rc_v = p.rcache + (size_t)(2 * l + 1) * per;
+      e.fstat = switches().static_fast ? ws.fstat : nullptr;
     }
     if (int rc = cbg_launch_x2h(e, st)) return rc;
     if (n_gen <= 0) continue;   // nothing moves: H2X output is multiplied by gen_flag == 0
-    if (overlap) {
-      CBG_CUDA_OK(cudaEventRecord(g_aux.ev_h, st));
-      CBG_CUDA_OK(cudaStreamWaitEvent(sx, g_aux.ev_h, 0));
-      CBG_CUDA_OK(cudaStreamWaitEvent(g_aux.s4, g_aux.ev_h, 0));
+    if (aux) {
+      CBG_CUDA_OK(cudaEventRecord(aux->ev_h, st));
+      CBG_CUDA_OK(cudaStreamWaitEvent(sx, aux->ev_h, 0));
+      CBG_CUDA_OK(cudaStreamWaitEvent(aux->s4, aux->ev_h, 0));
     }
-    // ---- H2X (uses the NEW h and the layer-input x): Pj planes for all nodes, Pi/q for generated nodes
-    NodeGemmArgs gj{};
-    gj.a = ws.h; gj.row_idx = nullptr; gj.n_rows = (int)n_nodes;
-    gj.wt = L + cbg_layout::layer_offset(CBG_LF_H2X_NODE_WT);
-    gj.bias = L + cbg_layout::layer_offset(CBG_LF_H2X_NODE_B);
-    gj.ldw = 640; gj.n_planes = 2; gj.has_q = 0;
-    gj.out[0] = ws.hplane[0]; gj.out[1] = ws.hplane[1];
-    gj.tc_planes = L + cbg_layout::layer_offset(CBG_LF_H2X_NODE_TC); gj.tc_first_plane = 0;
-    gj.tch_planes = L + cbg_layout::layer_offset(CBG_LF_H2X_NODE_TCH);
-    if (prune) { gj.row_idx = ws.order; gj.n_rows_dev = ws.cnt + num_layers; }   // depth == top: generated atoms + neighbours
-    if (int rc = launch_node_gemm(gj, sx)) return rc;
-    NodeGemmArgs gi{};
-    gi.a = ws.h; gi.row_idx = gen_idx; gi.n_rows = n_gen;
-    gi.wt = gj.wt + 256; gi.bias = gj.bias + 256;
-    gi.ldw = 640; gi.n_planes = 3; gi.has_q = 1;
-    gi.out[0] = ws.hplane[2]; gi.out[1] = ws.hplane[3]; gi.out[2] = nullptr;
-    gi.q_ln = L + cbg_layout::layer_offset(CBG_LF_H2X_Q_LN);
-    gi.q_w1t = L + cbg_layout::layer_offset(CBG_LF_H2X_Q_W1T);
-    gi.q_b1 = L + cbg_layout::layer_offset(CBG_LF_H2X_Q_B1);
-    gi.out_q = ws.hplane[4];
-    gi.tc_planes = gj.tc_planes; gi.tc_first_plane = 2; gi.tch_planes = gj.tch_planes;
-    if (int rc = launch_node_gemm(gi, overlap ? g_aux.s4 : sx)) return rc;     // beside gj
-    if (overlap) {
-      CBG_CUDA_OK(cudaEventRecord(g_aux.ev_gi, g_aux.s4));
-      CBG_CUDA_OK(cudaStreamWaitEvent(sx, g_aux.ev_gi, 0));
-    }
-    EdgeArgs x = e;
-    x.pj_k = ws.hplane[0]; x.pj_v = ws.hplane[1]; x.pi_k = ws.hplane[2]; x.pi_v = ws.hplane[3]; x.q = ws.hplane[4];
-    x.node_idx = gen_idx; x.n_nodes = n_gen; x.n_nodes_dev = nullptr; x.dx = ws.dx; x.rc_k = nullptr; x.rc_v = nullptr; x.fstat = nullptr;
-    x.w = ws.hw;        // the X2H kernels of the next layer use ws.w while this chain runs
-    x.ticket = (tickets && num_layers <= 16) ? ws.tickets + 32 + l : nullptr;      // used by the pair kernel only (x2h: 0 .. 2L-1)
-    if (int rc = cbg_launch_h2x(x, sx)) return rc;
-    if (int rc = cbg_launch_apply_dx(ws.x4, gen_idx, ws.dx, n_gen, sx)) return rc;
-    if (overlap) { CBG_CUDA_OK(cudaEventRecord(g_aux.ev_x, sx)); x_pending = true; }
+    // ---- H2X (uses the NEW h and the layer-input x); pruned: Pj for depth == top (generated atoms + neighbours)
+    if (int rc = run_h2x(L, ws, n_nodes, p.gen_node, n_gen, prune ? ws.cnt + num_layers : nullptr, aux, sx)) return rc;
+    if (aux) { CBG_CUDA_OK(cudaEventRecord(aux->ev_x, sx)); x_pending = true; }
   }
-  if (overlap && x_pending) CBG_CUDA_OK(cudaStreamWaitEvent(st, g_aux.ev_x, 0));   // join
+  if (aux && x_pending) CBG_CUDA_OK(cudaStreamWaitEvent(st, aux->ev_x, 0));   // join
   return 0;
 }
 
-// CoM head of DiffBP (CoMPredictor.forward, diffbp.py:80-101) after run_core on the same plan: the ligand rows of x4
-// get the step's INPUT coordinates x_t back, then the head's own edge gate and com_layers x H2X on the denoiser's final
-// h move the generated rows.  Afterwards the ligand rows of x4 hold x_com.  Shared by the sampling step and the
-// validation loss.
-int run_com_head(const cbg_sample_plan* plan, const float* com_blob, int com_layers, const Workspace& ws,
-                 const float* x_t, bool prune, cudaStream_t st) {
-  const long long n_nodes = plan->n_nodes;
-  const int n_gen = plan->n_gen, n_lig = plan->n_lig;
-  if (int rc = cbg_launch_scatter_x(x_t, plan->lig_node, n_lig, ws.x4, st)) return rc;
-  if (n_gen > 0 && com_layers > 0) {
-    if (int rc = cbg_launch_edge_gate_rows(com_blob, ws.x4, ws.nbr, plan->gen_node, n_gen, ws.ew, st)) return rc;
-    const bool pruned = prune && plan->num_layers > 0;      // run_core built ws.order / ws.cnt
-    const float* layers = com_blob + cbg_layout::kGlobalFloats;
-    for (int l = 0; l < com_layers; ++l) {
-      const float* L = layers + (size_t)l * cbg_layout::kLayerFloats;
-      NodeGemmArgs gj{};
-      gj.a = ws.h; gj.row_idx = nullptr; gj.n_rows = (int)n_nodes;
-      gj.wt = L + cbg_layout::layer_offset(CBG_LF_H2X_NODE_WT);
-      gj.bias = L + cbg_layout::layer_offset(CBG_LF_H2X_NODE_B);
-      gj.ldw = 640; gj.n_planes = 2; gj.has_q = 0;
-      gj.out[0] = ws.hplane[0]; gj.out[1] = ws.hplane[1];
-      gj.tc_planes = L + cbg_layout::layer_offset(CBG_LF_H2X_NODE_TC); gj.tc_first_plane = 0;
-      gj.tch_planes = L + cbg_layout::layer_offset(CBG_LF_H2X_NODE_TCH);
-      if (pruned) { gj.row_idx = ws.order; gj.n_rows_dev = ws.cnt + plan->num_layers; }   // generated atoms + neighbours
-      if (int rc = launch_node_gemm(gj, st)) return rc;
-      NodeGemmArgs gi{};
-      gi.a = ws.h; gi.row_idx = plan->gen_node; gi.n_rows = n_gen;
-      gi.wt = gj.wt + 256; gi.bias = gj.bias + 256;
-      gi.ldw = 640; gi.n_planes = 3; gi.has_q = 1;
-      gi.out[0] = ws.hplane[2]; gi.out[1] = ws.hplane[3]; gi.out[2] = nullptr;
-      gi.q_ln = L + cbg_layout::layer_offset(CBG_LF_H2X_Q_LN);
-      gi.q_w1t = L + cbg_layout::layer_offset(CBG_LF_H2X_Q_W1T);
-      gi.q_b1 = L + cbg_layout::layer_offset(CBG_LF_H2X_Q_B1);
-      gi.out_q = ws.hplane[4];
-      gi.tc_planes = gj.tc_planes; gi.tc_first_plane = 2; gi.tch_planes = gj.tch_planes;
-      if (int rc = launch_node_gemm(gi, st)) return rc;
-      EdgeArgs x{};
-      x.x4 = ws.x4; x.nbr = ws.nbr; x.ew = ws.ew;
-      x.pj_k = ws.hplane[0]; x.pj_v = ws.hplane[1]; x.pi_k = ws.hplane[2]; x.pi_v = ws.hplane[3]; x.q = ws.hplane[4];
-      x.layer = L; x.w = ws.hw; x.h = ws.h; x.node_idx = plan->gen_node; x.n_nodes = n_gen; x.dx = ws.dx;
-      if (int rc = cbg_launch_h2x(x, st)) return rc;
-      if (int rc = cbg_launch_apply_dx(ws.x4, plan->gen_node, ws.dx, n_gen, st)) return rc;
-    }
+// DiffBP's denoiser pass and heads: run_denoiser, the classifier on the ligand rows into `logits`, their output
+// coordinates into x_pred, then the CoM head (CoMPredictor.forward, diffbp.py:80-101): the ligand rows of x4 get the
+// step's INPUT coordinates x_t back, then the head's own edge gate and com_layers x H2X on the denoiser's final h move
+// the generated rows.  Afterwards the ligand rows of x4 hold x_com.  Shared by the sampling step and the validation loss.
+int run_bp_denoiser(const cbg_sample_plan& p, const float* com_blob, int com_layers, const Workspace& ws,
+                    const float* x_t, float* logits, float* x_pred, cudaStream_t st) {
+  if (int rc = run_denoiser(p, ws, st)) return rc;
+  if (int rc = cbg_launch_classifier(p.blob, ws.h, p.lig_node, p.n_lig, p.num_classes, logits, st)) return rc;
+  if (int rc = cbg_launch_gather_x(ws.x4, p.lig_node, p.n_lig, x_pred, st)) return rc;
+  if (int rc = cbg_launch_scatter_x(x_t, p.lig_node, p.n_lig, ws.x4, st)) return rc;
+  if (p.n_gen <= 0 || com_layers <= 0) return 0;
+  if (int rc = cbg_launch_edge_gate_rows(com_blob, ws.x4, ws.nbr, p.gen_node, p.n_gen, ws.ew, st)) return rc;
+  const int* src_rows_dev = plan_prunes(p) ? ws.cnt + p.num_layers : nullptr;   // run_denoiser built ws.order / ws.cnt
+  const float* layers = com_blob + cbg_layout::kGlobalFloats;
+  for (int l = 0; l < com_layers; ++l) {
+    if (int rc = run_h2x(layers + (size_t)l * cbg_layout::kLayerFloats, ws, p.n_nodes, p.gen_node, p.n_gen, src_rows_dev,
+                         nullptr, st)) return rc;
+  }
+  return 0;
+}
+
+// DiffBP scratch in the attention-weight buffer (free after the layers): logits [n_lig,K] | output coordinates [n_lig,3]
+struct BpScratch { float* logits; float* x_pred; };
+BpScratch bp_scratch(const Workspace& ws, int n_lig, int num_classes) {
+  return {ws.w, ws.w + align256((size_t)n_lig * num_classes * 4) / 4};
+}
+
+// Prologue of the plan-driven entry points: the plan and the entry point's other required arguments (args_ok; null_msg
+// is the error otherwise), a workspace that fits the plan, a class count the classifier supports.
+int open_plan(const cbg_sample_plan* plan, bool args_ok, const char* null_msg, Workspace* ws) {
+  if (!plan || !args_ok) { cbg_set_error("%s", null_msg); return 1; }
+  if (int rc = check_ws(plan->workspace, plan->workspace_bytes, plan->n_nodes, plan->n_gen, ws)) return rc;
+  const int K = plan->num_classes;
+  if (K < 1 || K > CBG_MAXCLS) { cbg_set_error("num_classes=%d outside [1,%d]", K, CBG_MAXCLS); return 1; }
+  return 0;
+}
+
+// The validation losses run n_rep noised copies of one batch as one plan, replica-major.
+int check_replicas(const cbg_sample_plan& p, int n_rep) {
+  if (n_rep < 1 || n_rep > CBG_EVAL_MAX_REPLICAS) { cbg_set_error("n_rep=%d outside [1,%d]", n_rep, CBG_EVAL_MAX_REPLICAS); return 1; }
+  if (p.n_lig < n_rep || p.n_lig % n_rep || p.n_graphs % n_rep) {
+    cbg_set_error("plan (n_lig=%d, n_graphs=%d) is not %d replicas of one batch", p.n_lig, p.n_graphs, n_rep); return 1;
   }
   return 0;
 }
@@ -434,8 +422,8 @@ int32_t cbg_selftest_umma_f16(const void* a, const void* b, float* d, int32_t a_
   return cbg_launch_umma_selftest(a, b, d, a_from_smem, (cudaStream_t)stream);
 }
 int32_t cbg_set_option(const char* key, int32_t value) {
-  if (key && strcmp(key, "static_fast") == 0) { g_static_fast = value ? 1 : 0; return 0; }
-  if (key && strcmp(key, "dyn_sched") == 0) { g_dyn_sched = value ? 1 : 0; return 0; }
+  if (key && strcmp(key, "static_fast") == 0) { switches().static_fast = value != 0; return 0; }
+  if (key && strcmp(key, "dyn_sched") == 0) { switches().dyn_sched = value != 0; return 0; }
   if (key && strcmp(key, "x2h_trace_off") == 0) { cbg_x2h_tc_set_trace(nullptr, 0); return 0; }
   cbg_set_error("cbg_set_option: unknown key '%s'", key ? key : "(null)");
   return 1;
@@ -529,8 +517,13 @@ int32_t cbg_denoiser_forward_f32(const float* blob, int32_t num_layers, int32_t 
   cudaStream_t st = (cudaStream_t)stream;
   if (int rc = cbg_launch_pack_x4(x, lig_flag, gen_flag, n_nodes, ws.x4, st)) return rc;
   CBG_CUDA_OK(cudaMemcpyAsync(ws.h, h, (size_t)n_nodes * CBG_H * 4, cudaMemcpyDeviceToDevice, st));
-  const int L = (stop_after_layers >= 0 && stop_after_layers < num_layers) ? stop_after_layers : num_layers;
-  if (int rc = run_core(blob, L, ws, graph_ptr, n_graphs, max_graph_nodes, n_nodes, gen_idx, n_gen, mode, k, r_max, nullptr, nullptr, 0, false, st)) return rc;
+  // no classified rows, R-cache, pruning or static lists: every node's x and h are outputs
+  cbg_sample_plan p{};
+  p.blob = blob; p.num_classes = num_classes;
+  p.num_layers = (stop_after_layers >= 0 && stop_after_layers < num_layers) ? stop_after_layers : num_layers;
+  p.graph_ptr = graph_ptr; p.n_graphs = n_graphs; p.max_graph_nodes = max_graph_nodes; p.n_nodes = n_nodes;
+  p.gen_node = gen_idx; p.n_gen = n_gen; p.mode = mode; p.k = k; p.r_max = r_max;
+  if (int rc = run_denoiser(p, ws, st)) return rc;
   if (x_out) { if (int rc = cbg_launch_unpack_x(ws.x4, n_nodes, x_out, st)) return rc; }
   if (h_out) CBG_CUDA_OK(cudaMemcpyAsync(h_out, ws.h, (size_t)n_nodes * CBG_H * 4, cudaMemcpyDeviceToDevice, st));
   if (logits_out) {
@@ -611,21 +604,9 @@ int32_t cbg_denoiser_forward_host_f32(const float* blob_host, int64_t blob_float
 int32_t cbg_node_proj_f32(const float* blob_layer, int32_t sublayer, int32_t impl, const float* h,
                           const int32_t* row_idx, int32_t n_rows, int64_t n_nodes, float* planes, void* stream) {
   if (sublayer < 0 || sublayer > 1 || (impl != 0 && impl != 1 && impl != 2 && impl != 11 && impl != 12 && impl != 14)) { cbg_set_error("bad sublayer/impl"); return 1; }
-  const float* L = blob_layer;
-  NodeGemmArgs g{};
-  g.a = h; g.row_idx = row_idx; g.n_rows = n_rows;
-  g.wt = L + cbg_layout::layer_offset(sublayer ? CBG_LF_H2X_NODE_WT : CBG_LF_X2H_NODE_WT);
-  g.bias = L + cbg_layout::layer_offset(sublayer ? CBG_LF_H2X_NODE_B : CBG_LF_X2H_NODE_B);
-  g.ldw = 640; g.n_planes = 5; g.has_q = 1;
-  for (int p = 0; p < 4; ++p) g.out[p] = planes + (size_t)p * n_nodes * CBG_H;
-  g.out[4] = nullptr;
-  g.q_ln = L + cbg_layout::layer_offset(sublayer ? CBG_LF_H2X_Q_LN : CBG_LF_X2H_Q_LN);
-  g.q_w1t = L + cbg_layout::layer_offset(sublayer ? CBG_LF_H2X_Q_W1T : CBG_LF_X2H_Q_W1T);
-  g.q_b1 = L + cbg_layout::layer_offset(sublayer ? CBG_LF_H2X_Q_B1 : CBG_LF_X2H_Q_B1);
-  g.out_q = planes + (size_t)4 * n_nodes * CBG_H;
-  g.tc_planes = L + cbg_layout::layer_offset(sublayer ? CBG_LF_H2X_NODE_TC : CBG_LF_X2H_NODE_TC);
-  g.tch_planes = L + cbg_layout::layer_offset(sublayer ? CBG_LF_H2X_NODE_TCH : CBG_LF_X2H_NODE_TCH);
-  g.tc_first_plane = 0;
+  float* out[CBG_NPLANES];
+  for (int p = 0; p < CBG_NPLANES; ++p) out[p] = planes + (size_t)p * n_nodes * CBG_H;
+  const NodeGemmArgs g = node_gemm_args(blob_layer, (SubLayer)sublayer, Planes::kAll, h, row_idx, n_rows, out);
   if (impl == 0) return cbg_launch_node_gemm(g, (cudaStream_t)stream);
   if (impl == 2) return cbg_launch_node_gemm_f16(g, (cudaStream_t)stream);
   return cbg_launch_node_gemm_tc(g, (cudaStream_t)stream, impl == 12 ? 2 : (impl == 14 ? 4 : (impl == 11 ? 1 : 0)));
@@ -667,18 +648,14 @@ int32_t cbg_sample_prune_counts_host(const cbg_sample_plan* plan, int32_t* count
 int32_t cbg_sample_step_f32(const cbg_sample_plan* plan, const cbg_step_coef* coef, const float* x_t,
                             const float* c_t, const float* pos_noise, const float* type_uniform, float* x_next,
                             float* c_next, int64_t* v_next, float* x0_pred, float* logits, void* stream) {
-  if (!plan || !coef) { cbg_set_error("null plan/coef"); return 1; }
-  NvtxRange nvtx_step("cbg:sample_step");
   Workspace ws;
-  if (int rc = check_ws(plan->workspace, plan->workspace_bytes, plan->n_nodes, plan->n_gen, &ws)) return rc;
+  if (int rc = open_plan(plan, coef != nullptr, "null plan/coef", &ws)) return rc;
+  NvtxRange nvtx_step("cbg:sample_step");
   cudaStream_t st = (cudaStream_t)stream;
   const int K = plan->num_classes;
-  if (K < 1 || K > CBG_MAXCLS) { cbg_set_error("num_classes=%d outside [1,%d]", K, CBG_MAXCLS); return 1; }
   if (int rc = cbg_launch_step_init(x_t, c_t, plan->lig_node, plan->n_lig, K, plan->emb_wt, plan->h_lig_bias,
                                     plan->h_static, plan->n_nodes, ws.x4, ws.h, st)) return rc;
-  if (int rc = run_core(plan->blob, plan->num_layers, ws, plan->graph_ptr, plan->n_graphs, plan->max_graph_nodes,
-                        plan->n_nodes, plan->gen_node, plan->n_gen, plan->mode, plan->k, plan->r_max, plan->rcache,
-                        plan->lig_node, plan->n_lig, plan->prune != 0 && prune_enabled(), st, plan->static_lists != 0)) return rc;
+  if (int rc = run_denoiser(*plan, ws, st)) return rc;
   // classifier on ligand rows only (SURVEY.md A11); logits scratch lives in the w buffer (free after the layers)
   float* lg = logits ? logits : ws.w;
   if (int rc = cbg_launch_classifier(plan->blob, ws.h, plan->lig_node, plan->n_lig, K, lg, st)) return rc;
@@ -738,7 +715,8 @@ void destroy_graph(StepGraph* g) {
 int32_t cbg_sample_step_graph_f32(const cbg_sample_plan* plan, const cbg_step_coef* coef, const float* x_t,
                                   const float* c_t, const float* pos_noise, const float* type_uniform, float* x_next,
                                   float* c_next, int64_t* v_next, void* stream) {
-  if (!plan || !coef) { cbg_set_error("null plan/coef"); return 1; }
+  Workspace ws;
+  if (int rc = open_plan(plan, coef != nullptr, "null plan/coef", &ws)) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   int dev = -1;
   CBG_CUDA_OK(cudaGetDevice(&dev));
@@ -764,8 +742,6 @@ int32_t cbg_sample_step_graph_f32(const cbg_sample_plan* plan, const cbg_step_co
     g->warm += 1;
     return cbg_sample_step_f32(plan, coef, x_t, c_t, pos_noise, type_uniform, x_next, c_next, v_next, nullptr, nullptr, stream);
   }
-  Workspace ws;
-  if (int rc = check_ws(plan->workspace, plan->workspace_bytes, plan->n_nodes, plan->n_gen, &ws)) return rc;
   const int K = plan->num_classes;
   if (!g->exec) {
     CBG_CUDA_OK(cudaMallocHost((void**)&g->pinned, sizeof(StepIO) * kIoRing));
@@ -778,9 +754,7 @@ int32_t cbg_sample_step_graph_f32(const cbg_sample_plan* plan, const cbg_step_co
     CBG_CUDA_OK(cudaStreamBeginCapture(cs, cudaStreamCaptureModeRelaxed));
     int rc = cbg_launch_step_init_io(ws.io, plan->lig_node, plan->n_lig, K, plan->emb_wt, plan->h_lig_bias, plan->h_static,
                                      plan->n_nodes, ws.x4, ws.h, cs);
-    if (!rc) rc = run_core(plan->blob, plan->num_layers, ws, plan->graph_ptr, plan->n_graphs, plan->max_graph_nodes,
-                           plan->n_nodes, plan->gen_node, plan->n_gen, plan->mode, plan->k, plan->r_max, plan->rcache,
-                           plan->lig_node, plan->n_lig, plan->prune != 0 && prune_enabled(), cs, plan->static_lists != 0);
+    if (!rc) rc = run_denoiser(*plan, ws, cs);
     if (!rc) rc = cbg_launch_classifier(plan->blob, ws.h, plan->lig_node, plan->n_lig, K, ws.w, cs);
     if (!rc) {
       ReverseArgs r{};
@@ -827,19 +801,15 @@ int64_t cbg_sample_step_graph_nodes(const cbg_sample_plan* plan, void* stream) {
 int32_t cbg_sbdd_step_f32(const cbg_sample_plan* plan, const cbg_sbdd_coef* coef, const float* x_t, const float* c_t,
                           const float* x_noise, const float* c_noise, float* x_next, float* c_next,
                           float* x_pred, float* logits, void* stream) {
-  if (!plan || !coef) { cbg_set_error("null plan/coef"); return 1; }
+  Workspace ws;
+  if (int rc = open_plan(plan, coef != nullptr, "null plan/coef", &ws)) return rc;
   if (plan->rcache || plan->static_lists) { cbg_set_error("DiffSBDD moves the pocket every step: the plan must not carry static lists / an R-cache"); return 1; }
   if (coef->mode != 0 && coef->mode != 1) { cbg_set_error("cbg_sbdd_coef.mode must be 0 or 1"); return 1; }
-  Workspace ws;
-  if (int rc = check_ws(plan->workspace, plan->workspace_bytes, plan->n_nodes, plan->n_gen, &ws)) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   const int K = plan->num_classes;
-  if (K < 1 || K > CBG_MAXCLS) { cbg_set_error("num_classes=%d outside [1,%d]", K, CBG_MAXCLS); return 1; }
   if (int rc = cbg_launch_step_init(x_t, c_t, plan->lig_node, plan->n_lig, K, plan->emb_wt, plan->h_lig_bias,
                                     plan->h_static, plan->n_nodes, ws.x4, ws.h, st)) return rc;
-  if (int rc = run_core(plan->blob, plan->num_layers, ws, plan->graph_ptr, plan->n_graphs, plan->max_graph_nodes,
-                        plan->n_nodes, plan->gen_node, plan->n_gen, plan->mode, plan->k, plan->r_max, nullptr,
-                        plan->lig_node, plan->n_lig, plan->prune != 0 && prune_enabled(), st)) return rc;
+  if (int rc = run_denoiser(*plan, ws, st)) return rc;
   float* lg = logits ? logits : ws.w;
   if (int rc = cbg_launch_classifier(plan->blob, ws.h, plan->lig_node, plan->n_lig, K, lg, st)) return rc;
   if (x_pred) {
@@ -856,31 +826,19 @@ int32_t cbg_sbdd_step_f32(const cbg_sample_plan* plan, const cbg_sbdd_coef* coef
 int32_t cbg_bp_step_f32(const cbg_sample_plan* plan, const float* com_blob, int32_t com_layers, const cbg_bp_coef* coef,
                         const float* x_t, const float* c_t, const float* pos_noise, const float* type_uniform,
                         float* x_next, float* c_next, int64_t* v_next, float* eps_out, float* logits, void* stream) {
-  if (!plan || !coef || !com_blob) { cbg_set_error("null plan/coef/com_blob"); return 1; }
-  if (com_layers < 0 || com_layers > 16) { cbg_set_error("com_layers=%d outside [0,16]", com_layers); return 1; }
   Workspace ws;
-  if (int rc = check_ws(plan->workspace, plan->workspace_bytes, plan->n_nodes, plan->n_gen, &ws)) return rc;
+  if (int rc = open_plan(plan, coef && com_blob, "null plan/coef/com_blob", &ws)) return rc;
+  if (com_layers < 0 || com_layers > 16) { cbg_set_error("com_layers=%d outside [0,16]", com_layers); return 1; }
   cudaStream_t st = (cudaStream_t)stream;
-  const int K = plan->num_classes;
-  if (K < 1 || K > CBG_MAXCLS) { cbg_set_error("num_classes=%d outside [1,%d]", K, CBG_MAXCLS); return 1; }
-  const long long n_nodes = plan->n_nodes;
-  const int n_gen = plan->n_gen, n_lig = plan->n_lig;
+  const int K = plan->num_classes, n_lig = plan->n_lig;
   if (int rc = cbg_launch_step_init(x_t, c_t, plan->lig_node, n_lig, K, plan->emb_wt, plan->h_lig_bias,
-                                    plan->h_static, n_nodes, ws.x4, ws.h, st)) return rc;
-  const bool prune = plan->prune != 0 && prune_enabled();
-  if (int rc = run_core(plan->blob, plan->num_layers, ws, plan->graph_ptr, plan->n_graphs, plan->max_graph_nodes,
-                        n_nodes, plan->gen_node, n_gen, plan->mode, plan->k, plan->r_max, plan->rcache,
-                        plan->lig_node, n_lig, prune, st, plan->static_lists != 0)) return rc;
-  // scratch in the attention-weight buffer (free after the layers): logits | denoiser output coordinates
-  float* lg = logits ? logits : ws.w;
-  float* xp = ws.w + align256((size_t)n_lig * K * 4) / 4;
-  if (int rc = cbg_launch_classifier(plan->blob, ws.h, plan->lig_node, n_lig, K, lg, st)) return rc;
-  if (int rc = cbg_launch_gather_x(ws.x4, plan->lig_node, n_lig, xp, st)) return rc;
-  // ---- CoM head (diffbp.py:80-101): same graph, own gate, H2X stack on the final h, starting from the INPUT x
-  if (int rc = run_com_head(plan, com_blob, com_layers, ws, x_t, prune, st)) return rc;
+                                    plan->h_static, plan->n_nodes, ws.x4, ws.h, st)) return rc;
+  const BpScratch s = bp_scratch(ws, n_lig, K);
+  float* lg = logits ? logits : s.logits;
+  if (int rc = run_bp_denoiser(*plan, com_blob, com_layers, ws, x_t, lg, s.x_pred, st)) return rc;
   BpArgs r{};
   r.x4 = ws.x4; r.graph_ptr = plan->graph_ptr; r.lig_node = plan->lig_node; r.n_lig = n_lig; r.num_classes = K;
-  r.n_graphs = plan->n_graphs; r.x_pred = xp; r.logits = lg; r.x_t = x_t; r.c_t = c_t; r.gen = plan->gen_lig;
+  r.n_graphs = plan->n_graphs; r.x_pred = s.x_pred; r.logits = lg; r.x_t = x_t; r.c_t = c_t; r.gen = plan->gen_lig;
   r.pos_noise = pos_noise; r.type_u = type_uniform; r.abar = coef->alpha_cumprod; r.beta = coef->beta;
   r.nonzero = coef->nonzero; r.prob = coef->change_prob; r.x_next = x_next; r.c_next = c_next;
   r.v_next = (long long*)v_next; r.eps_out = eps_out;
@@ -891,21 +849,14 @@ int32_t cbg_bp_eval_loss_f32(const cbg_sample_plan* plan, const float* com_blob,
                              const cbg_bp_eval_coef* coefs, int32_t n_rep, const float* x0, const int64_t* v0,
                              const float* pos_noise, const float* type_uniform, float* xt, int64_t* vt, uint8_t* mask,
                              float* vec, float* c_pred, float* rep_loss, void* stream) {
-  if (!plan || !com_blob || !coefs || !x0 || !v0 || !pos_noise || !type_uniform || !xt || !vt || !mask || !vec || !c_pred ||
-      !rep_loss) {
-    cbg_set_error("cbg_bp_eval_loss_f32: null argument"); return 1;
-  }
-  if (com_layers < 0 || com_layers > 16) { cbg_set_error("com_layers=%d outside [0,16]", com_layers); return 1; }
-  if (n_rep < 1 || n_rep > CBG_EVAL_MAX_REPLICAS) { cbg_set_error("n_rep=%d outside [1,%d]", n_rep, CBG_EVAL_MAX_REPLICAS); return 1; }
-  if (plan->n_lig < n_rep || plan->n_lig % n_rep || plan->n_graphs % n_rep) {
-    cbg_set_error("plan (n_lig=%d, n_graphs=%d) is not %d replicas of one batch", plan->n_lig, plan->n_graphs, n_rep); return 1;
-  }
-  NvtxRange nvtx_eval("cbg:bp_eval_loss");
   Workspace ws;
-  if (int rc = check_ws(plan->workspace, plan->workspace_bytes, plan->n_nodes, plan->n_gen, &ws)) return rc;
+  if (int rc = open_plan(plan, com_blob && coefs && x0 && v0 && pos_noise && type_uniform && xt && vt && mask && vec &&
+                         c_pred && rep_loss, "cbg_bp_eval_loss_f32: null argument", &ws)) return rc;
+  if (com_layers < 0 || com_layers > 16) { cbg_set_error("com_layers=%d outside [0,16]", com_layers); return 1; }
+  if (int rc = check_replicas(*plan, n_rep)) return rc;
+  NvtxRange nvtx_eval("cbg:bp_eval_loss");
   cudaStream_t st = (cudaStream_t)stream;
   const int K = plan->num_classes, n_lig = plan->n_lig;
-  if (K < 1 || K > CBG_MAXCLS) { cbg_set_error("num_classes=%d outside [1,%d]", K, CBG_MAXCLS); return 1; }
   BpEvalArgs e{};
   for (int r = 0; r < n_rep; ++r) e.coef.c[r] = BpEvalCoefDev{coefs[r].alphas_cumprod, coefs[r].beta, coefs[r].mask_prob};
   e.n_rep = n_rep; e.n_lig = n_lig; e.n_graphs = plan->n_graphs; e.num_classes = K;
@@ -914,21 +865,13 @@ int32_t cbg_bp_eval_loss_f32(const cbg_sample_plan* plan, const float* com_blob,
   e.emb_wt = plan->emb_wt; e.h_lig_bias = plan->h_lig_bias;
   e.x4 = ws.x4; e.h = ws.h; e.xt = xt; e.vt = (long long*)vt; e.mask = mask; e.vec = vec; e.c_pred = c_pred;
   e.rep_loss = rep_loss;
-  // scratch: logits | denoiser output coordinates in the attention-weight buffer (as in cbg_bp_step_f32); the X2H
-  // planes are free once the denoiser is done (the CoM head uses the H2X planes)
-  float* lg = ws.w;
-  float* xp = ws.w + align256((size_t)n_lig * K * 4) / 4;
-  e.logits = lg; e.x_pred = xp;
+  // scratch: the X2H planes are free once the denoiser is done (the CoM head uses the H2X planes)
+  const BpScratch s = bp_scratch(ws, n_lig, K);
+  e.logits = s.logits; e.x_pred = s.x_pred;
   e.xs = (float4*)ws.plane[0]; e.thr = (int2*)ws.plane[1]; e.graph_part = ws.plane[2];
   CBG_CUDA_OK(cudaMemcpyAsync(ws.h, plan->h_static, (size_t)plan->n_nodes * CBG_H * sizeof(float), cudaMemcpyDeviceToDevice, st));
   if (int rc = cbg_launch_bp_eval_noise(e, st)) return rc;
-  const bool prune = plan->prune != 0 && prune_enabled();
-  if (int rc = run_core(plan->blob, plan->num_layers, ws, plan->graph_ptr, plan->n_graphs, plan->max_graph_nodes,
-                        plan->n_nodes, plan->gen_node, plan->n_gen, plan->mode, plan->k, plan->r_max, plan->rcache,
-                        plan->lig_node, n_lig, prune, st, plan->static_lists != 0)) return rc;
-  if (int rc = cbg_launch_classifier(plan->blob, ws.h, plan->lig_node, n_lig, K, lg, st)) return rc;
-  if (int rc = cbg_launch_gather_x(ws.x4, plan->lig_node, n_lig, xp, st)) return rc;
-  if (int rc = run_com_head(plan, com_blob, com_layers, ws, xt, prune, st)) return rc;
+  if (int rc = run_bp_denoiser(*plan, com_blob, com_layers, ws, xt, s.logits, s.x_pred, st)) return rc;
   return cbg_launch_bp_eval_loss(e, st);
 }
 
@@ -951,19 +894,13 @@ int32_t cbg_reverse_step_f32(const cbg_step_coef* coef, const float* x0_pred, co
 int32_t cbg_eval_loss_f32(const cbg_sample_plan* plan, const cbg_eval_coef* coefs, int32_t n_rep, const float* x0,
                           const int64_t* v0, const float* pos_noise, const float* type_uniform, float* xt, int64_t* vt,
                           float* x_pred, float* c_pred, float* graph_loss, float* rep_loss, void* stream) {
-  if (!plan || !coefs || !x0 || !v0 || !pos_noise || !type_uniform || !xt || !vt || !x_pred || !c_pred || !graph_loss || !rep_loss) {
-    cbg_set_error("cbg_eval_loss_f32: null argument"); return 1;
-  }
-  if (n_rep < 1 || n_rep > CBG_EVAL_MAX_REPLICAS) { cbg_set_error("n_rep=%d outside [1,%d]", n_rep, CBG_EVAL_MAX_REPLICAS); return 1; }
-  if (plan->n_lig < n_rep || plan->n_lig % n_rep || plan->n_graphs % n_rep) {
-    cbg_set_error("plan (n_lig=%d, n_graphs=%d) is not %d replicas of one batch", plan->n_lig, plan->n_graphs, n_rep); return 1;
-  }
-  NvtxRange nvtx_eval("cbg:eval_loss");
   Workspace ws;
-  if (int rc = check_ws(plan->workspace, plan->workspace_bytes, plan->n_nodes, plan->n_gen, &ws)) return rc;
+  if (int rc = open_plan(plan, coefs && x0 && v0 && pos_noise && type_uniform && xt && vt && x_pred && c_pred && graph_loss &&
+                         rep_loss, "cbg_eval_loss_f32: null argument", &ws)) return rc;
+  if (int rc = check_replicas(*plan, n_rep)) return rc;
+  NvtxRange nvtx_eval("cbg:eval_loss");
   cudaStream_t st = (cudaStream_t)stream;
   const int K = plan->num_classes;
-  if (K < 1 || K > CBG_MAXCLS) { cbg_set_error("num_classes=%d outside [1,%d]", K, CBG_MAXCLS); return 1; }
   EvalArgs e{};
   for (int r = 0; r < n_rep; ++r) {
     const cbg_eval_coef& c = coefs[r];
@@ -980,9 +917,7 @@ int32_t cbg_eval_loss_f32(const cbg_sample_plan* plan, const cbg_eval_coef* coef
   e.graph_loss = graph_loss; e.rep_loss = rep_loss;
   CBG_CUDA_OK(cudaMemcpyAsync(ws.h, plan->h_static, (size_t)plan->n_nodes * CBG_H * sizeof(float), cudaMemcpyDeviceToDevice, st));
   if (int rc = cbg_launch_eval_noise(e, st)) return rc;
-  if (int rc = run_core(plan->blob, plan->num_layers, ws, plan->graph_ptr, plan->n_graphs, plan->max_graph_nodes,
-                        plan->n_nodes, plan->gen_node, plan->n_gen, plan->mode, plan->k, plan->r_max, plan->rcache,
-                        plan->lig_node, plan->n_lig, plan->prune != 0 && prune_enabled(), st, plan->static_lists != 0)) return rc;
+  if (int rc = run_denoiser(*plan, ws, st)) return rc;
   if (int rc = cbg_launch_classifier(plan->blob, ws.h, plan->lig_node, plan->n_lig, K, ws.w, st)) return rc;
   return cbg_launch_eval_loss(e, st);
 }

@@ -149,7 +149,7 @@ __global__ void __launch_bounds__(256, 2) node_gemm_kernel(NodeGemmArgs p) {
 
 int cbg_launch_node_gemm(const NodeGemmArgs& a, cudaStream_t st) {
   if (a.n_rows <= 0) return 0;
-  // the merged source/destination launch (n_dst_dev) is an f16-kernel feature: run_core gives this kernel two launches
+  // the merged source/destination launch (n_dst_dev) is an f16-kernel feature: run_denoiser gives this kernel two launches
   if (a.n_dst_dev) { cbg_set_error("fp32 SIMT node GEMM: n_dst_dev is not supported"); return 1; }
   static bool attr_dev[CBG_MAX_DEVICES] = {};
   bool& attr_set = cbg_dev_flag(attr_dev);

@@ -254,7 +254,7 @@ int launch_tc(const NodeGemmArgs& a, cudaStream_t st) {
 int cbg_launch_node_gemm_tc(const NodeGemmArgs& a, cudaStream_t st, int cluster) {
   if (a.n_rows <= 0) return 0;
   if (!a.tc_planes) { cbg_set_error("tensor-core node GEMM needs the pre-split weight planes"); return 1; }
-  // the merged source/destination launch (n_dst_dev) is an f16-kernel feature: run_core gives this kernel two launches
+  // the merged source/destination launch (n_dst_dev) is an f16-kernel feature: run_denoiser gives this kernel two launches
   if (a.n_dst_dev) { cbg_set_error("3xTF32 node GEMM: n_dst_dev is not supported"); return 1; }
   static int cl_env = -1;
   if (cl_env < 0) {

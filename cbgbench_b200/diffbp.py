@@ -24,7 +24,7 @@ import torch.nn.functional as F
 from . import _lib
 from .modules import (GaussianSmearing, H2XAttention, MLP, _NoTorchPath, cfg_get, pack_denoiser_blob)
 from .schedulers import CTNVPTables
-from .targetdiff import BaseDiffB200, eval_t_values, register_model
+from .targetdiff import BaseDiffB200, register_model
 
 ABSORBING_STATE = 0      # repo/utils/molecule/constants.py:8
 
@@ -95,18 +95,7 @@ class DiffBPB200(BaseDiffB200):
                            nonzero=0.0 if t_idx == 0 else 1.0,
                            change_prob=self.type_scheduler.change_prob(t_idx))
 
-    # ---- validation loss (DiffBP.forward with self.training == False) ----------------------------------------------
-    def forward(self, batch, pos_noise=None, type_uniform=None):
-        """DiffBP.forward (diffbp.py:133-171).  Eval mode only: returns ``(loss_dict, results)`` for the
-        ``eval_interval`` (default 10) timesteps ``np.linspace(0, T-1, eval_interval)`` truncated to integers, exactly
-        like the reference; see ``eval_losses``.  Training mode needs autograd through the denoiser and raises."""
-        if self.training:
-            raise NotImplementedError(f'{type(self).__name__}.forward in training mode needs autograd through the '
-                                      'denoiser, which the CUDA path does not provide: training is out of scope '
-                                      '(call model.eval() for the validation losses)')
-        t_values = eval_t_values(self.num_diffusion_timesteps, cfg_get(self.cfg, 'eval_interval', 10))
-        return self.eval_losses(batch, t_values, pos_noise=pos_noise, type_uniform=type_uniform)
-
+    # ---- validation loss (DiffBP.forward with self.training == False, diffbp.py:133-171) ---------------------------
     def eval_coef(self, t_idx):
         ps = self.pos_scheduler
         mask_prob = torch.tensor([t_idx]).float().clamp(min=0.) / self.num_diffusion_timesteps    # fp32, like :462-466
@@ -132,12 +121,8 @@ class DiffBPB200(BaseDiffB200):
         if not self.intersect_reg:
             raise NotImplementedError('intersect_reg: False is not supported: the reference\'s DiffBP.get_loss reads the '
                                       'interior loss unconditionally (diffbp.py:222-226) and raises UnboundLocalError')
-        t_values = [int(t) for t in t_values]
-        R, T, K = len(t_values), self.num_diffusion_timesteps, self.num_classes
-        if R == 0:
-            raise ValueError('t_values is empty')
-        if any(t < 0 or t >= T for t in t_values):
-            raise ValueError(f't_values must lie in [0, {T - 1}]')
+        t_values = self._eval_t_values(t_values)
+        R, K = len(t_values), self.num_classes
         dev = next(self.parameters()).device
         if dev.type != 'cuda':
             raise NotImplementedError(f'{type(self).__name__}.forward needs the model on a CUDA device: the validation '
@@ -150,12 +135,7 @@ class DiffBPB200(BaseDiffB200):
         v0 = b['ligand_atom_type'].long().contiguous()
         gen = b['ligand_gen_flag'] if 'ligand_gen_flag' in b else b['ligand_lig_flag']
         n_lig = x0.shape[0]
-        if pos_noise is None or type_uniform is None:
-            draws = [(torch.randn(n_lig, 3, device=dev), torch.rand(n_lig, device=dev)) for _ in range(R)]
-            pos_noise = torch.stack([d[0] for d in draws]) if pos_noise is None else pos_noise
-            type_uniform = torch.stack([d[1] for d in draws]) if type_uniform is None else type_uniform
-        pos_noise = pos_noise.to(dev, torch.float32).reshape(R, n_lig, 3).contiguous()
-        type_uniform = type_uniform.to(dev, torch.float32).reshape(R, n_lig).contiguous()
+        pos_noise, type_uniform = self._eval_noise(R, dev, pos_noise, type_uniform, (n_lig,))
 
         com_blob = self.com_head.packed_blob(dev)
         xt = torch.empty(R, n_lig, 3, device=dev)
@@ -221,26 +201,11 @@ class DiffBPB200(BaseDiffB200):
 
         ``pos_noise[t]`` [n_lig,3] / ``type_uniform[t]`` [n_lig] inject the random numbers; ``num_steps`` stops early;
         ``traj_mode='final'`` keeps only traj[0] and traj[-1]; ``eps_out`` (dict) receives eps + eps_com per step."""
-        T, K = self.num_diffusion_timesteps, self.num_classes
+        T = self.num_diffusion_timesteps
         state = self.prepare(batch)
-        dev, n_lig = state['device'], state['n_lig']
-        X = torch.empty((T + 1, n_lig, 3), dtype=torch.float32, device=dev)
-        Cc = torch.empty((T + 1, n_lig, K), dtype=torch.float32, device=dev)
-        X[T].copy_(state['x_lig'])
-        Cc[T].copy_(state['c_lig'])
+        X, Cc = self._traj_buffers(state['device'], state['x_lig'], state['c_lig'])
         t_seq = list(reversed(range(T)))
         if num_steps is not None:
             t_seq = t_seq[:num_steps]
         self.run_steps(state, t_seq, X, Cc, pos_noise, type_uniform, eps_out)
-        bl = state['batch_idx_lig']
-        t_last = t_seq[-1]
-        traj = {}
-        bl_cpu = bl.cpu()
-        if traj_mode == 'full':
-            Xh, Ch = X[t_last + 1:].cpu(), Cc[t_last + 1:].cpu()
-            for t in range(t_last, T):
-                traj[t] = (Xh[t - t_last], Ch[t - t_last], bl_cpu)
-        else:
-            traj[t_last] = (X[t_last + 1].cpu(), Cc[t_last + 1].cpu(), bl_cpu)
-        traj[t_last - 1] = (X[t_last].clone(), Cc[t_last].clone(), bl)
-        return traj
+        return self._traj(X, Cc, state['batch_idx_lig'], t_seq[-1], traj_mode)

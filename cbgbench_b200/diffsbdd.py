@@ -58,7 +58,7 @@ class DiffSBDDB200(BaseDiffB200):
         """Initial state (diffsbdd.py:255-262) + device plan.  Ligand ~ N(pocket mean, I) projected to zero ligand
         COM - the projection translates the pocket as well; type features ~ N(0, I).  Returns the state dict of
         ``prepare`` plus the trajectory buffers X [T+1,n_lig,3] / C [T+1,n_lig,K] (slot t+1 = state entering step t)."""
-        T, K = self.num_diffusion_timesteps, self.num_classes
+        K = self.num_classes
         dev = next(self.parameters()).device
         if dev.type != 'cuda':
             raise RuntimeError('DiffSBDDB200.sample needs the model on a CUDA device (no CPU fallback)')
@@ -75,11 +75,7 @@ class DiffSBDDB200(BaseDiffB200):
         x_lig = (x_lig - mean[bl]).contiguous()
         x_rec = x_rec - mean[br]
         state = self.prepare(batch, device=dev, protein_feature_scale=TYPE_NORM, protein_pos=x_rec)
-        X = torch.empty((T + 1, n_lig, 3), dtype=torch.float32, device=dev)
-        Cc = torch.empty((T + 1, n_lig, K), dtype=torch.float32, device=dev)
-        X[T].copy_(x_lig)
-        Cc[T].copy_(eps_c)
-        state['X'], state['C'] = X, Cc
+        state['X'], state['C'] = self._traj_buffers(dev, x_lig, eps_c)
         return state
 
     @torch.no_grad()
@@ -137,7 +133,6 @@ class DiffSBDDB200(BaseDiffB200):
         ``traj_mode='final'`` keeps only traj[0] and traj[-1]."""
         T = self.num_diffusion_timesteps
         state = self.begin(batch, noise)
-        X, Cc, bl = state['X'], state['C'], state['batch_idx_lig']
         t_seq = list(reversed(range(T)))
         if num_steps is not None:
             t_seq = t_seq[:num_steps]
@@ -148,15 +143,7 @@ class DiffSBDDB200(BaseDiffB200):
         if t_last == 0:
             x_fin, c_fin = self.finish(state, noise)
         self.last_launches = launches
-        traj = {}
-        bl_cpu = bl.cpu()
-        if traj_mode == 'full':
-            Xh, Ch = X[t_last + 1:].cpu(), Cc[t_last + 1:].cpu()
-            for t in range(t_last, T):
-                traj[t] = (Xh[t - t_last], Ch[t - t_last], bl_cpu)
-        else:
-            traj[t_last] = (X[t_last + 1].cpu(), Cc[t_last + 1].cpu(), bl_cpu)
-        traj[t_last - 1] = (X[t_last].clone(), Cc[t_last].clone(), bl)
+        traj = self._traj(state['X'], state['C'], state['batch_idx_lig'], t_last, traj_mode)
         if x_fin is not None:
-            traj[0] = (x_fin.cpu(), c_fin.cpu(), bl_cpu)
+            traj[0] = (x_fin.cpu(), c_fin.cpu(), traj[0][2])
         return traj

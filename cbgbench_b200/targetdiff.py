@@ -154,11 +154,69 @@ class BaseDiffB200(nn.Module):
             raise RuntimeError('stale sampling state: prepare() was called again on this model (its device workspace now '
                                'belongs to the newer batch); finish one batch before preparing the next, or use a second model')
 
-    def forward(self, batch):
-        raise NotImplementedError(f'{type(self).__name__} is a sampling build: the training / validation losses of this '
-                                  'model are not implemented on the CUDA path (DESIGN.md section 9)')
+    # ---- the trajectory of ``sample`` ----------------------------------------------------------------------------
+    def _traj_buffers(self, dev, x_init, c_init):
+        """Device trajectory X [T+1,n_lig,3] / Cc [T+1,n_lig,K]: slot t+1 is the state entering step t, slot t its
+        result; slot T holds the initial state."""
+        T, n_lig = self.num_diffusion_timesteps, x_init.shape[0]
+        X = torch.empty((T + 1, n_lig, 3), dtype=torch.float32, device=dev)
+        Cc = torch.empty((T + 1, n_lig, self.num_classes), dtype=torch.float32, device=dev)
+        X[T].copy_(x_init)
+        Cc[T].copy_(c_init)
+        return X, Cc
+
+    def _traj(self, X, Cc, bl, t_last, traj_mode):
+        """``traj`` of the reference's sample: {t: (x_lig, c_lig, batch_idx_lig)} for t = T-1 ... t_last (on the CPU,
+        one copy; only t_last when ``traj_mode`` is not 'full') and t_last - 1 (on the device)."""
+        T = self.num_diffusion_timesteps
+        traj = {}
+        bl_cpu = bl.cpu()
+        if traj_mode == 'full':
+            Xh, Ch = X[t_last + 1:].cpu(), Cc[t_last + 1:].cpu()
+            for t in range(t_last, T):
+                traj[t] = (Xh[t - t_last], Ch[t - t_last], bl_cpu)
+        else:
+            traj[t_last] = (X[t_last + 1].cpu(), Cc[t_last + 1].cpu(), bl_cpu)
+        traj[t_last - 1] = (X[t_last].clone(), Cc[t_last].clone(), bl)
+        return traj
 
     # ---- validation losses: what the eval-mode forwards share (replica batching, DESIGN.md section 13) --------------
+    def forward(self, batch, pos_noise=None, type_uniform=None):
+        """The reference's forward in eval mode: ``(loss_dict, results)`` of ``eval_losses`` for the ``eval_interval``
+        (default 10) timesteps ``np.linspace(0, T-1, eval_interval)`` truncated to integers, exactly like the reference.
+        Training mode needs autograd through the denoiser and raises; so does a sampler without ``eval_losses``."""
+        if not hasattr(self, 'eval_losses'):
+            raise NotImplementedError(f'{type(self).__name__} is a sampling build: the training / validation losses of '
+                                      'this model are not implemented on the CUDA path (DESIGN.md section 9)')
+        if self.training:
+            raise NotImplementedError(f'{type(self).__name__}.forward in training mode needs autograd through the '
+                                      'denoiser, which the CUDA path does not provide: training is out of scope '
+                                      '(call model.eval() for the validation losses)')
+        t_values = eval_t_values(self.num_diffusion_timesteps, cfg_get(self.cfg, 'eval_interval', 10))
+        return self.eval_losses(batch, t_values, pos_noise=pos_noise, type_uniform=type_uniform)
+
+    def _eval_t_values(self, t_values):
+        t_values = [int(t) for t in t_values]
+        T = self.num_diffusion_timesteps
+        if not t_values:
+            raise ValueError('t_values is empty')
+        if any(t < 0 or t >= T for t in t_values):
+            raise ValueError(f't_values must lie in [0, {T - 1}]')
+        return t_values
+
+    @staticmethod
+    def _eval_noise(R, dev, pos_noise, type_uniform, type_shape):
+        """pos_noise [R,n_lig,3] / type_uniform [R,*type_shape] on ``dev``; what is not injected is drawn in the
+        reference's order (for each of the R timesteps: randn [n_lig,3], then rand type_shape)."""
+        n_lig = type_shape[0]
+        if pos_noise is None or type_uniform is None:
+            draws = [(torch.randn(n_lig, 3, device=dev), torch.rand(*type_shape, device=dev)) for _ in range(R)]
+            pos_noise = torch.stack([d[0] for d in draws]) if pos_noise is None else pos_noise
+            type_uniform = torch.stack([d[1] for d in draws]) if type_uniform is None else type_uniform
+        pos_noise = pos_noise.to(dev, torch.float32).reshape(R, n_lig, 3).contiguous()
+        type_uniform = type_uniform.to(dev, torch.float32).reshape(R, *type_shape).contiguous()
+        return pos_noise, type_uniform
+
     _EVAL_KEYS = ('ligand_pos', 'ligand_atom_type', 'protein_pos', 'protein_atom_feature', 'protein_aa_type',
                   'ligand_lig_flag', 'protein_lig_flag', 'ligand_element_batch', 'protein_element_batch',
                   'ligand_gen_flag', 'protein_gen_flag')
@@ -298,18 +356,7 @@ class TargetDiffB200(BaseDiffB200):
             log_alpha=float(ts.host_table('log_alphas_v')[t_idx]),
             log_one_minus_alpha=float(ts.host_table('log_one_minus_alphas_v')[t_idx]))
 
-    # ---- validation loss (TargetDiff.forward with self.training == False) -------------------------------------------
-    def forward(self, batch, pos_noise=None, type_uniform=None):
-        """TargetDiff.forward (targetdiff.py:41-80).  Eval mode only: returns ``(loss_dict, results)`` for the
-        ``eval_interval`` (default 10) timesteps ``np.linspace(0, T-1, eval_interval)`` truncated to integers, exactly
-        like the reference; see ``eval_losses``.  Training mode needs autograd through the denoiser and raises."""
-        if self.training:
-            raise NotImplementedError(f'{type(self).__name__}.forward in training mode needs autograd through the '
-                                      'denoiser, which the CUDA path does not provide: training is out of scope '
-                                      '(call model.eval() for the validation losses)')
-        t_values = eval_t_values(self.num_diffusion_timesteps, cfg_get(self.cfg, 'eval_interval', 10))
-        return self.eval_losses(batch, t_values, pos_noise=pos_noise, type_uniform=type_uniform)
-
+    # ---- validation loss (TargetDiff.forward with self.training == False, targetdiff.py:41-80) ----------------------
     def eval_coef(self, t_idx):
         ps, ts = self.pos_scheduler, self.type_scheduler
         tm1 = max(t_idx - 1, 0)
@@ -339,12 +386,8 @@ class TargetDiffB200(BaseDiffB200):
 
         ``pos_noise`` [R,n_lig,3] / ``type_uniform`` [R,n_lig,K] inject the draws; by default they are drawn with torch on
         the model device in the reference's order (for each t: randn [n_lig,3], then rand [n_lig,K])."""
-        t_values = [int(t) for t in t_values]
-        R, T, K = len(t_values), self.num_diffusion_timesteps, self.num_classes
-        if R == 0:
-            raise ValueError('t_values is empty')
-        if any(t < 0 or t >= T for t in t_values):
-            raise ValueError(f't_values must lie in [0, {T - 1}]')
+        t_values = self._eval_t_values(t_values)
+        R, K = len(t_values), self.num_classes
         dev = next(self.parameters()).device
         if dev.type != 'cuda':
             raise RuntimeError(f'{type(self).__name__}.forward needs the model on a CUDA device (no CPU fallback)')
@@ -353,12 +396,7 @@ class TargetDiffB200(BaseDiffB200):
         v0 = b['ligand_atom_type'].long().contiguous()
         mask_gen = b['ligand_gen_flag'].bool() if 'ligand_gen_flag' in b else b['ligand_lig_flag'].bool()
         n_lig = x0.shape[0]
-        if pos_noise is None or type_uniform is None:
-            draws = [(torch.randn(n_lig, 3, device=dev), torch.rand(n_lig, K, device=dev)) for _ in range(R)]
-            pos_noise = torch.stack([d[0] for d in draws]) if pos_noise is None else pos_noise
-            type_uniform = torch.stack([d[1] for d in draws]) if type_uniform is None else type_uniform
-        pos_noise = pos_noise.to(dev, torch.float32).reshape(R, n_lig, 3).contiguous()
-        type_uniform = type_uniform.to(dev, torch.float32).reshape(R, n_lig, K).contiguous()
+        pos_noise, type_uniform = self._eval_noise(R, dev, pos_noise, type_uniform, (n_lig, K))
 
         xt = torch.empty(R, n_lig, 3, device=dev)
         vt = torch.empty(R, n_lig, dtype=torch.int64, device=dev)
@@ -444,25 +482,9 @@ class TargetDiffB200(BaseDiffB200):
         ``traj_mode='final'`` keeps only traj[0] and traj[-1]."""
         T = self.num_diffusion_timesteps
         state = self.prepare(batch)
-        dev, n_lig, K = state['device'], state['n_lig'], self.num_classes
-        X = torch.empty((T + 1, n_lig, 3), dtype=torch.float32, device=dev)
-        Cc = torch.empty((T + 1, n_lig, K), dtype=torch.float32, device=dev)
-        X[T].copy_(state['x_lig'])
-        Cc[T].copy_(state['c_lig'])
+        X, Cc = self._traj_buffers(state['device'], state['x_lig'], state['c_lig'])
         t_seq = list(reversed(range(T)))
         if num_steps is not None:
             t_seq = t_seq[:num_steps]
         self.run_steps(state, t_seq, X, Cc, pos_noise=pos_noise, type_uniform=type_uniform)
-        bl = state['batch_idx_lig']
-        t_last = t_seq[-1]
-        traj = {}
-        if traj_mode == 'full':
-            Xh = X[t_last + 1:].cpu()
-            Ch = Cc[t_last + 1:].cpu()
-            bl_cpu = bl.cpu()
-            for t in range(t_last, T):
-                traj[t] = (Xh[t - t_last], Ch[t - t_last], bl_cpu)
-        else:
-            traj[t_last] = (X[t_last + 1].cpu(), Cc[t_last + 1].cpu(), bl.cpu())
-        traj[t_last - 1] = (X[t_last].clone(), Cc[t_last].clone(), bl)
-        return traj
+        return self._traj(X, Cc, state['batch_idx_lig'], t_seq[-1], traj_mode)

@@ -101,12 +101,17 @@ def test_training_mode_forward_raises():
         model(synthetic.make_batch([20], [5], seed=1))
 
 
-@pytest.mark.parametrize('kind', ['diffsbdd', 'diffbp'])
-def test_other_samplers_forward_still_raise(kind):
+def test_diffsbdd_forward_is_a_sampling_build():
     from cbgbench_b200.targetdiff import get_model
-    cfg = synthetic.diffsbdd_config(num_steps=10) if kind == 'diffsbdd' else synthetic.diffbp_config(num_steps=10)
-    model = get_model(cfg).eval()
-    with pytest.raises(NotImplementedError):
+    model = get_model(synthetic.diffsbdd_config(num_steps=10)).eval()
+    with pytest.raises(NotImplementedError, match='sampling build'):
+        model(synthetic.make_batch([20], [5], seed=1))
+
+
+def test_diffbp_forward_on_a_cpu_model_raises():
+    from cbgbench_b200.targetdiff import get_model
+    model = get_model(synthetic.diffbp_config(num_steps=10)).eval()
+    with pytest.raises(NotImplementedError, match='CUDA device'):
         model(synthetic.make_batch([20], [5], seed=1))
 
 
