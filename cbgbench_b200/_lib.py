@@ -49,6 +49,13 @@ class BpEvalCoef(C.Structure):
     _fields_ = [('alphas_cumprod', C.c_float), ('beta', C.c_float), ('mask_prob', C.c_float)]
 
 
+class SbddEvalCoef(C.Structure):
+    _fields_ = [(name, C.c_float) for name in (
+        'pos_alpha_t', 'pos_sigma_t', 'type_alpha_t', 'type_sigma_t', 'pos_alpha_0', 'pos_sigma_0', 'type_alpha_0',
+        'type_sigma_0', 'pos_t_weight', 'type_t_weight', 'pos_log_const', 'type_log_const', 'pos_alpha_T', 'type_alpha_T',
+        'pos_log_inv_sigma_T', 'type_log_inv_sigma_T', 'pos_sigma2_T', 'type_sigma2_T')]
+
+
 class SbddCoef(C.Structure):
     _fields_ = [('a', C.c_float), ('b', C.c_float), ('s', C.c_float), ('mode', C.c_int32)]
 
@@ -98,6 +105,8 @@ SIGNATURES = {
     'cbg_bp_step_f32': (_I32, [C.POINTER(SamplePlan), _P, _I32, C.POINTER(BpCoef), _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     'cbg_bp_eval_loss_f32': (_I32, [C.POINTER(SamplePlan), _P, _I32, C.POINTER(BpEvalCoef), _I32, _P, _P, _P, _P, _P, _P,
                                      _P, _P, _P, _P, _P]),
+    'cbg_sbdd_eval_loss_f32': (_I32, [C.POINTER(SamplePlan), C.POINTER(SbddEvalCoef), _I32, _P, _P, _P, _P, _P, _P, _P, _P,
+                                       _P, _P, _P, _P]),
     'cbg_pocket_stats_f32': (_I32, [_P, _P, _I32, _P, _P, _I32, _P, _P, _P]),
     'cbg_sample_ligand_sizes': (_I32, [_P, _P, _I32, _I32, _P, _P, _P, _P, _P, _P]),
     'cbg_build_batch_f32': (_I32, [_P, _P]),

@@ -363,9 +363,12 @@ int open_plan(const cbg_sample_plan* plan, bool args_ok, const char* null_msg, W
   return 0;
 }
 
-// The validation losses run n_rep noised copies of one batch as one plan, replica-major.
-int check_replicas(const cbg_sample_plan& p, int n_rep) {
-  if (n_rep < 1 || n_rep > CBG_EVAL_MAX_REPLICAS) { cbg_set_error("n_rep=%d outside [1,%d]", n_rep, CBG_EVAL_MAX_REPLICAS); return 1; }
+// The validation losses run noised copies of one batch as one plan, replica-major: n_t timesteps of `copies` replicas
+// each (n_rep = n_t * copies, at most CBG_EVAL_MAX_REPLICAS).
+int check_replicas(const cbg_sample_plan& p, int n_t, int copies = 1) {
+  const int max_t = CBG_EVAL_MAX_REPLICAS / copies;
+  if (n_t < 1 || n_t > max_t) { cbg_set_error("%s=%d outside [1,%d]", copies == 1 ? "n_rep" : "n_t", n_t, max_t); return 1; }
+  const int n_rep = n_t * copies;
   if (p.n_lig < n_rep || p.n_lig % n_rep || p.n_graphs % n_rep) {
     cbg_set_error("plan (n_lig=%d, n_graphs=%d) is not %d replicas of one batch", p.n_lig, p.n_graphs, n_rep); return 1;
   }
@@ -920,6 +923,41 @@ int32_t cbg_eval_loss_f32(const cbg_sample_plan* plan, const cbg_eval_coef* coef
   if (int rc = run_denoiser(*plan, ws, st)) return rc;
   if (int rc = cbg_launch_classifier(plan->blob, ws.h, plan->lig_node, plan->n_lig, K, ws.w, st)) return rc;
   return cbg_launch_eval_loss(e, st);
+}
+
+int32_t cbg_sbdd_eval_loss_f32(const cbg_sample_plan* plan, const cbg_sbdd_eval_coef* coefs, int32_t n_t,
+                               const float* x0, const int64_t* v0, const float* x_rec, const float* x_t_noise,
+                               const float* c_t_noise, const float* x_0_noise, const float* c_0_noise, float* vec_pos,
+                               float* vec_atom, float* terms, float* t_loss, void* stream) {
+  Workspace ws;
+  if (int rc = open_plan(plan, coefs && x0 && v0 && x_t_noise && c_t_noise && x_0_noise && c_0_noise && vec_pos && vec_atom &&
+                         terms && t_loss && (x_rec || plan->n_nodes == plan->n_lig), "cbg_sbdd_eval_loss_f32: null argument", &ws)) return rc;
+  if (plan->rcache || plan->static_lists) { cbg_set_error("DiffSBDD moves the pocket with every noised copy: the plan must not carry static lists / an R-cache"); return 1; }
+  if (int rc = check_replicas(*plan, n_t, 2)) return rc;
+  if ((plan->n_nodes - plan->n_lig) % (2 * n_t)) { cbg_set_error("plan (n_nodes=%lld) is not %d replicas of one batch", (long long)plan->n_nodes, 2 * n_t); return 1; }
+  NvtxRange nvtx_eval("cbg:sbdd_eval_loss");
+  cudaStream_t st = (cudaStream_t)stream;
+  const int K = plan->num_classes;
+  SbddEvalArgs e{};
+  for (int j = 0; j < n_t; ++j) {
+    const cbg_sbdd_eval_coef& c = coefs[j];
+    e.coef.c[j] = SbddEvalCoefDev{c.pos_alpha_t, c.pos_sigma_t, c.type_alpha_t, c.type_sigma_t, c.pos_alpha_0, c.pos_sigma_0,
+                                  c.type_alpha_0, c.type_sigma_0, c.pos_t_weight, c.type_t_weight, c.pos_log_const,
+                                  c.type_log_const, c.pos_alpha_T, c.type_alpha_T, c.pos_log_inv_sigma_T,
+                                  c.type_log_inv_sigma_T, c.pos_sigma2_T, c.type_sigma2_T};
+  }
+  e.n_t = n_t; e.n_lig = plan->n_lig; e.n_graphs = plan->n_graphs; e.num_classes = K; e.n_nodes = plan->n_nodes;
+  e.lig_node = plan->lig_node; e.graph_ptr = plan->graph_ptr; e.gen = plan->gen_lig;
+  e.x0 = x0; e.v0 = (const long long*)v0; e.x_rec = x_rec;
+  e.x_t_noise = x_t_noise; e.c_t_noise = c_t_noise; e.x_0_noise = x_0_noise; e.c_0_noise = c_0_noise;
+  e.emb_wt = plan->emb_wt; e.h_lig_bias = plan->h_lig_bias;
+  e.logits = ws.w;                  // classifier scratch: the attention-weight buffer is free after the layers
+  e.x4 = ws.x4; e.h = ws.h; e.vec_pos = vec_pos; e.vec_atom = vec_atom; e.terms = terms; e.t_loss = t_loss;
+  CBG_CUDA_OK(cudaMemcpyAsync(ws.h, plan->h_static, (size_t)plan->n_nodes * CBG_H * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  if (int rc = cbg_launch_sbdd_eval_noise(e, st)) return rc;
+  if (int rc = run_denoiser(*plan, ws, st)) return rc;
+  if (int rc = cbg_launch_classifier(plan->blob, ws.h, plan->lig_node, plan->n_lig, K, ws.w, st)) return rc;
+  return cbg_launch_sbdd_eval_loss(e, st);
 }
 
 // ---- row f3: device-side batch construction ---------------------------------------------------------------------

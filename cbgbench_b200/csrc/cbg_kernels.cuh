@@ -271,6 +271,46 @@ int cbg_launch_bp_eval_noise(const BpEvalArgs& a, cudaStream_t st);
 // bp_eval_loss_kernel (one CTA per graph) followed by bp_eval_reduce_kernel (one thread per replica)
 int cbg_launch_bp_eval_loss(const BpEvalArgs& a, cudaStream_t st);
 
+// sbdd_eval.cu: DiffSBDD validation loss over n_t timesteps of a batch (cbg_sbdd_eval_loss_f32).  The plan holds 2 n_t
+// replicas, replica-major like EvalArgs: replica 2j is timestep j noised at t_j, replica 2j+1 timestep j noised at 0.
+struct SbddEvalCoefDev {   // same members as cbg_sbdd_eval_coef (include/cbg_b200.h)
+  float pos_alpha_t, pos_sigma_t, type_alpha_t, type_sigma_t;
+  float pos_alpha_0, pos_sigma_0, type_alpha_0, type_sigma_0;
+  float pos_t_weight, type_t_weight;
+  float pos_log_const, type_log_const;
+  float pos_alpha_T, type_alpha_T;
+  float pos_log_inv_sigma_T, type_log_inv_sigma_T;
+  float pos_sigma2_T, type_sigma2_T;
+};
+struct SbddEvalCoefs { SbddEvalCoefDev c[CBG_EVAL_MAX_REPLICAS / 2]; };
+struct SbddEvalArgs {
+  SbddEvalCoefs coef;
+  int n_t, n_lig, n_graphs, num_classes;   // n_lig / n_graphs: replicated totals (2 n_t replicas)
+  long long n_nodes;
+  const int* lig_node;       // [n_lig] ascending composed node index
+  const int* graph_ptr;      // [n_graphs+1]
+  const unsigned char* gen;  // [n_lig] replicated ligand_gen_flag
+  const float* x0;           // [n1,3] the batch's ligand_pos (n1 = n_lig / (2 n_t))
+  const long long* v0;       // [n1]
+  const float* x_rec;        // [n_rec1,3] the batch's protein_pos
+  const float* x_t_noise;    // [n_t,n1,3] / [n_t,n1,K] / [n_t,n1,3] / [n_t,n1,K]: the four draws of each timestep
+  const float* c_t_noise;
+  const float* x_0_noise;
+  const float* c_0_noise;
+  const float* emb_wt;       // [K,128]
+  const float* h_lig_bias;   // [n_lig,128]
+  const float* logits;       // [n_lig,K] classifier output
+  float4* x4;                // node coordinates + flags; after the denoiser the ligand rows hold x_pred
+  float* h;                  // [N,128] node features
+  float* vec_pos;            // [n_t,3,n1,3]: eps_pred, score_0, score_pred of the positions
+  float* vec_atom;           // [n_t,3,n1,K]: the same of the types
+  float* terms;              // [n_t,B,6]: pos_t, pos_0, pos_kl, atom_t, atom_0, atom_kl per graph of the batch
+  float* t_loss;             // [n_t,2]: pos, atom
+};
+int cbg_launch_sbdd_eval_noise(const SbddEvalArgs& a, cudaStream_t st);
+// sbdd_eval_loss_kernel (one CTA per (timestep, graph)) followed by sbdd_eval_reduce_kernel (one thread per timestep)
+int cbg_launch_sbdd_eval_loss(const SbddEvalArgs& a, cudaStream_t st);
+
 // batch.cu (row f3: device-side batch construction)
 int cbg_launch_pocket_stats(const float* prot_pos, const int* prot_ptr, int n_pockets, const float* ctx_pos,
                             const int* ctx_ptr, int centre_mode, float* space_size, float* centre, cudaStream_t st);

@@ -15,16 +15,28 @@ Reference quirks reproduced (oracle/diffusion_sbdd.py lists them): the denoiser'
 the final ``c_lig`` is 4 x the last state, not the freshly sampled one; gen_flag is ignored by the reverse step.
 Random numbers: ``torch.randn`` on the model device in the reference's order (x then c: init, every step, final
 stage), or injected through ``noise`` for parity tests.
+
+The eval-mode ``forward(batch)`` (diffsbdd.py:48-191, the validation loss) noises every timestep twice, at t and at 0,
+and runs all these copies through ONE C-ABI call (``cbg_sbdd_eval_loss_f32``, DESIGN.md section 15).
 """
 import ctypes as C
 
+import numpy as np
 import torch
 
 from . import _lib
+from .modules import cfg_get
 from .schedulers import DiffsbddVariationalTables
 from .targetdiff import BaseDiffB200, register_model
 
 TYPE_NORM = 4.0      # normalize_type / unnormalize_type (diffsbdd.py:95-96, 210-211)
+EVAL_NOISE_KEYS = ('x_t', 'c_t', 'x_0', 'c_0')     # the four draws of one eval timestep, in the reference's order
+
+
+def eval_t_values(num_timesteps, eval_interval=10):
+    """Timesteps of DiffSBDD's eval-mode forward (diffsbdd.py:71-77): ``np.linspace(1, T, eval_interval)``, each
+    truncated by ``torch.tensor([t] * B).long()``.  T = 1000 gives [1, 112, 223, ..., 889, 1000]: t = T is included."""
+    return [int(t) for t in np.linspace(1, num_timesteps, eval_interval).astype(np.int64)]
 
 
 @register_model('diffsbdd')
@@ -38,6 +50,96 @@ class DiffSBDDB200(BaseDiffB200):
         self.type_scheduler = DiffsbddVariationalTables(self.num_diffusion_timesteps, type=gen.atom_schedule.type)
         self._build_networks(cfg)
         self.intersect_reg = cfg.get('intersect_reg', True) if hasattr(cfg, 'get') else True
+
+    # ---- validation loss (DiffSBDD.forward with self.training == False, diffsbdd.py:48-191) --------------------------
+    def forward(self, batch, noise=None):
+        """The reference's forward in eval mode: ``(loss_dict, results)`` of ``eval_losses`` for the ``eval_interval``
+        (default 10) timesteps ``np.linspace(1, T, eval_interval)`` truncated to integers, exactly like the reference.
+        Training mode needs autograd through the denoiser and raises."""
+        self._check_eval_mode()
+        t_values = eval_t_values(self.num_diffusion_timesteps, cfg_get(self.cfg, 'eval_interval', 10))
+        return self.eval_losses(batch, t_values, noise=noise)
+
+    def eval_coef(self, t):
+        """Host scalars of timestep t (integer in [1, T]) with the reference's fp32 torch expressions: s = (t - 1) / T and
+        t / T as in get_loss, gamma at 0 (t_zeros) and at 1 (kl_prior's ones)."""
+        T = self.num_diffusion_timesteps
+        tt = torch.tensor([t], dtype=torch.int64)
+        alpha = lambda g: torch.sqrt(torch.sigmoid(-g))
+        sigma = lambda g: torch.sqrt(torch.sigmoid(g))
+        v = {}
+        for pre, tab in (('pos', self.pos_scheduler), ('type', self.type_scheduler)):
+            g_s, g_t, g_0, g_T = (tab.gamma_at(x) for x in ((tt - 1) / T, tt / T, torch.zeros(1), torch.ones(1)))
+            s_T = sigma(g_T)
+            v.update({f'{pre}_alpha_t': alpha(g_t), f'{pre}_sigma_t': sigma(g_t),
+                      f'{pre}_alpha_0': alpha(g_0), f'{pre}_sigma_0': sigma(g_0),
+                      f'{pre}_t_weight': -T * 0.5 * (1 - torch.exp(-(g_s - g_t))),               # :883-887
+                      f'{pre}_log_const': -(0.5 * g_0) - 0.5 * np.log(2 * np.pi),               # :680-692
+                      f'{pre}_alpha_T': alpha(g_T),
+                      f'{pre}_log_inv_sigma_T': torch.log(torch.ones_like(s_T) / s_T),          # gaussian_KL, :695-704
+                      f'{pre}_sigma2_T': s_T ** 2})
+        return _lib.SbddEvalCoef(**{k: float(x[0]) for k, x in v.items()})
+
+    @torch.no_grad()
+    def eval_losses(self, batch, t_values, noise=None, max_nodes=None):
+        """Validation losses of ``batch`` at the timesteps ``t_values`` (integers in [1, T]; DiffSBDD.get_loss in eval
+        mode, diffsbdd.py:87-191, once per t).  Returns ``(loss_dict, results)`` like the reference's eval-mode forward:
+        ``loss_dict`` = {'pos', 'atom'} as CPU 0-d float32 tensors (mean over t of the per-t losses), ``results`` one
+        dict per t with the device tensors eps_0_pos (the position draw at t), eps_pred_pos (the denoiser's output
+        coordinates), score_0_pos, score_pred_pos (both times sigma_t), mask_gen_pos (the generation flag), and the same
+        five ``_atom`` keys of the types (eps_pred_atom = the classifier's logits).  ``last_terms`` then holds the
+        per-graph terms [n_t, B, 6] (pos_t, pos_0, pos_kl, atom_t, atom_0, atom_kl; B = last ligand graph id + 1).
+
+        Each t is noised twice, at t and at 0.  The denoiser is not conditioned on t, so the 2 R copies go through ONE
+        denoiser pass as 2 R * B graphs, split over several launches above ``max_nodes`` composed nodes (default
+        ``eval_max_nodes``, a timestep counting twice) or 32 timesteps; the split does not change any result bit.
+
+        ``noise`` = {'x_t', 'c_t', 'x_0', 'c_0'} of [R, n_lig, 3 | K] injects the draws; by default they are drawn with
+        torch on the model device in the reference's order (for each t: randn [n_lig,3], [n_lig,K], [n_lig,3],
+        [n_lig,K])."""
+        t_values = self._eval_t_values(t_values, first=1)
+        R, K = len(t_values), self.num_classes
+        dev = next(self.parameters()).device
+        if dev.type != 'cuda':
+            raise NotImplementedError(f'{type(self).__name__}.forward needs the model on a CUDA device: on the CPU '
+                                      f'{type(self).__name__} is a sampling build without a validation-loss implementation')
+        b, n_graphs = self._eval_batch(batch, dev)
+        x0 = b['ligand_pos'].float().contiguous()
+        v0 = b['ligand_atom_type'].long().contiguous()
+        x_rec = b['protein_pos'].float().contiguous()
+        gen = b['ligand_gen_flag'] if 'ligand_gen_flag' in b else b['ligand_lig_flag']
+        n_lig = x0.shape[0]
+        dims = {'x_t': 3, 'c_t': K, 'x_0': 3, 'c_0': K}
+        if noise is None:
+            draws = [[torch.randn(n_lig, dims[k], device=dev) for k in EVAL_NOISE_KEYS] for _ in range(R)]
+            noise = {k: torch.stack([d[i] for d in draws]) for i, k in enumerate(EVAL_NOISE_KEYS)}
+        noise = {k: noise[k].to(dev, torch.float32).reshape(R, n_lig, dims[k]).contiguous() for k in EVAL_NOISE_KEYS}
+
+        vec_pos = torch.empty(R, 3, n_lig, 3, device=dev)
+        vec_atom = torch.empty(R, 3, n_lig, K, device=dev)
+        terms = torch.empty(R, n_graphs, 6, device=dev)
+        t_loss = torch.empty(R, 2, device=dev)
+        L = _lib.lib()
+        launches0 = L.cbg_launch_count()
+        for r0, r1, state in self._eval_launches(b, n_graphs, R, max_nodes, copies=2, protein_feature_scale=TYPE_NORM):
+            n = r1 - r0
+            coefs = (_lib.SbddEvalCoef * n)(*[self.eval_coef(t) for t in t_values[r0:r1]])
+            with torch.cuda.device(dev):
+                _lib.check(L.cbg_sbdd_eval_loss_f32(
+                    C.byref(state['plan']), coefs, n, x0.data_ptr(), v0.data_ptr(), x_rec.data_ptr() if x_rec.numel() else None,
+                    *[noise[k][r0:r1].data_ptr() for k in EVAL_NOISE_KEYS], vec_pos[r0:r1].data_ptr(),
+                    vec_atom[r0:r1].data_ptr(), terms[r0:r1].data_ptr(), t_loss[r0:r1].data_ptr(), _lib.stream_ptr(dev)))
+        self.last_launches = L.cbg_launch_count() - launches0
+        self.last_terms = terms[:, :int(b['ligand_element_batch'].max()) + 1]
+        per_t = t_loss.cpu()
+        # get_dict_mean (common.py:33-42): mean over t of the per-t scalars, as a CPU float32 tensor
+        loss_dict = {k: torch.mean(torch.tensor(per_t[:, i].tolist())) for i, k in enumerate(('pos', 'atom'))}
+        # the reference's key order: pos_info, then atom_info (get_score_loss, diffusion_scheduler.py:944-961)
+        results = [{'eps_0_pos': noise['x_t'][r], 'eps_pred_pos': vec_pos[r, 0], 'score_0_pos': vec_pos[r, 1],
+                    'score_pred_pos': vec_pos[r, 2], 'mask_gen_pos': gen,
+                    'eps_0_atom': noise['c_t'][r], 'eps_pred_atom': vec_atom[r, 0], 'score_0_atom': vec_atom[r, 1],
+                    'score_pred_atom': vec_atom[r, 2], 'mask_gen_atom': gen} for r in range(R)]
+        return loss_dict, results
 
     @staticmethod
     def _segment_mean(x, idx, n):

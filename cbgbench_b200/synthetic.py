@@ -99,6 +99,14 @@ def make_sbdd_noise(num_steps, n_lig, num_classes=13, seed=7):
             'final_x': f(n_lig, 3), 'final_c': f(n_lig, num_classes)}
 
 
+def make_sbdd_eval_noise(num_t, n_lig, num_classes=13, seed=7):
+    """Injected normal draws of one eval-mode DiffSBDD.forward over ``num_t`` timesteps: {'x_t', 'c_t', 'x_0', 'c_0'} of
+    [num_t, n_lig, 3 | K] (per t the reference draws positions at t, types at t, positions at 0, types at 0)."""
+    rs = np.random.RandomState(seed)
+    f = lambda d: torch.from_numpy(rs.normal(size=(num_t, n_lig, d)).astype(np.float32))
+    return {'x_t': f(3), 'c_t': f(num_classes), 'x_0': f(3), 'c_0': f(num_classes)}
+
+
 def make_batch(n_prot, n_lig, seed=2024, num_classes=13, gen_mode='denovo', protein_sigma=8.0):
     """Flat ragged batch with the reference's keys (SURVEY.md section 8b).
 
@@ -181,7 +189,7 @@ def seeded_state_dict(model, seed=0, skip_prefixes=('pos_scheduler.', 'type_sche
     return out
 
 
-__all__ = ['Cfg', 'targetdiff_config', 'diffsbdd_config', 'make_sbdd_noise', 'diffbp_config', 'make_bp_noise', 'make_batch', 'make_noise', 'seeded_state_dict', 'cfg_get']
+__all__ = ['Cfg', 'targetdiff_config', 'diffsbdd_config', 'make_sbdd_noise', 'make_sbdd_eval_noise', 'diffbp_config', 'make_bp_noise', 'make_batch', 'make_noise', 'seeded_state_dict', 'cfg_get']
 
 
 # ---- SURVEY.md section 8 row f4: IPATransformer (D3FG encoder) -----------------------------------------------------------

@@ -184,24 +184,25 @@ class BaseDiffB200(nn.Module):
     def forward(self, batch, pos_noise=None, type_uniform=None):
         """The reference's forward in eval mode: ``(loss_dict, results)`` of ``eval_losses`` for the ``eval_interval``
         (default 10) timesteps ``np.linspace(0, T-1, eval_interval)`` truncated to integers, exactly like the reference.
-        Training mode needs autograd through the denoiser and raises; so does a sampler without ``eval_losses``."""
-        if not hasattr(self, 'eval_losses'):
-            raise NotImplementedError(f'{type(self).__name__} is a sampling build: the training / validation losses of '
-                                      'this model are not implemented on the CUDA path (DESIGN.md section 9)')
+        Training mode needs autograd through the denoiser and raises."""
+        self._check_eval_mode()
+        t_values = eval_t_values(self.num_diffusion_timesteps, cfg_get(self.cfg, 'eval_interval', 10))
+        return self.eval_losses(batch, t_values, pos_noise=pos_noise, type_uniform=type_uniform)
+
+    def _check_eval_mode(self):
         if self.training:
             raise NotImplementedError(f'{type(self).__name__}.forward in training mode needs autograd through the '
                                       'denoiser, which the CUDA path does not provide: training is out of scope '
                                       '(call model.eval() for the validation losses)')
-        t_values = eval_t_values(self.num_diffusion_timesteps, cfg_get(self.cfg, 'eval_interval', 10))
-        return self.eval_losses(batch, t_values, pos_noise=pos_noise, type_uniform=type_uniform)
 
-    def _eval_t_values(self, t_values):
+    def _eval_t_values(self, t_values, first=0):
+        """``t_values`` as ints, each in [first, T - 1 + first]."""
         t_values = [int(t) for t in t_values]
         T = self.num_diffusion_timesteps
         if not t_values:
             raise ValueError('t_values is empty')
-        if any(t < 0 or t >= T for t in t_values):
-            raise ValueError(f't_values must lie in [0, {T - 1}]')
+        if any(t < first or t > T - 1 + first for t in t_values):
+            raise ValueError(f't_values must lie in [{first}, {T - 1 + first}]')
         return t_values
 
     @staticmethod
@@ -230,15 +231,16 @@ class BaseDiffB200(nn.Module):
         n_graphs = int(torch.cat([b['ligand_element_batch'], b['protein_element_batch']]).max()) + 1
         return b, n_graphs
 
-    def _eval_launches(self, b, n_graphs, R, max_nodes):
-        """Yield (r0, r1, state): replicas r0 .. r1-1 prepared as one plan of (r1 - r0) * n_graphs graphs, at most 64
-        replicas and ``max_nodes`` composed nodes (default ``eval_max_nodes``) per plan."""
+    def _eval_launches(self, b, n_graphs, R, max_nodes, copies=1, **prepare_kw):
+        """Yield (r0, r1, state): timesteps r0 .. r1-1, ``copies`` noised copies each, prepared as one plan of
+        (r1 - r0) * copies * n_graphs graphs, at most 64 replicas and ``max_nodes`` composed nodes (default
+        ``eval_max_nodes``) per plan.  ``prepare_kw`` goes to ``prepare``."""
         n_nodes = b['ligand_pos'].shape[0] + b['protein_pos'].shape[0]
         budget = self.eval_max_nodes if max_nodes is None else int(max_nodes)
-        per_launch = max(1, min(_lib.EVAL_MAX_REPLICAS, budget // n_nodes))
+        per_launch = max(1, min(_lib.EVAL_MAX_REPLICAS // copies, budget // (copies * n_nodes)))
         for r0 in range(0, R, per_launch):
             r1 = min(R, r0 + per_launch)
-            yield r0, r1, self.prepare(replicate_batch(b, r1 - r0, n_graphs))
+            yield r0, r1, self.prepare(replicate_batch(b, (r1 - r0) * copies, n_graphs), **prepare_kw)
 
     # ---- setup of the step-invariant state ------------------------------------------------
     @torch.no_grad()

@@ -328,6 +328,43 @@ int32_t cbg_bp_eval_loss_f32(const cbg_sample_plan* plan, const float* com_blob,
                              const float* pos_noise, const float* type_uniform, float* xt, int64_t* vt, uint8_t* mask,
                              float* vec, float* c_pred, float* rep_loss, void* stream);
 
+/* ---- validation loss: DiffSBDD.forward in eval mode (diffsbdd.py:48-191) ----------------------------------------------
+ *
+ * Every timestep t of the batch is noised twice, at t and at 0, and both copies go through the denoiser.  The plan holds
+ * 2 n_t replicas of the batch (graph r*B + g and ligand atom r*(n_lig/(2 n_t)) + a are graph g and atom a): replica 2j
+ * is timestep j at t_j, replica 2j+1 timestep j at 0.  No static lists or R-cache: the pocket moves with each copy.
+ * One call enqueues: remove_mean_batch of the clean ligand and pocket, forward_pos_center_noise (the noisy ligand's mean
+ * over all its atoms is removed from the generated atoms and the pocket; the other ligand atoms stay at their centred
+ * clean positions) and forward_type_add_noise of the types onehot / 4 (diffusion_scheduler.py:706-775) -> the denoiser
+ * -> classifier -> per (timestep, graph) the six terms of get_score_loss in eval mode (:897-920), the denoiser's ligand
+ * output coordinates acting as the position noise prediction and the logits as the type noise prediction -> the per-t
+ * means.  No atomics: repeated calls are bit-identical.  Every scalar below is the reference's fp32 torch expression. */
+typedef struct cbg_sbdd_eval_coef {  /* one timestep t (gamma_t = gamma[round(t/T * T)], s = (t-1)/T) */
+  float pos_alpha_t, pos_sigma_t;    /* sqrt(sigmoid(-gamma_t)), sqrt(sigmoid(gamma_t)) of pos_scheduler */
+  float type_alpha_t, type_sigma_t;  /* the same of type_scheduler */
+  float pos_alpha_0, pos_sigma_0;    /* at t = 0 */
+  float type_alpha_0, type_sigma_0;
+  float pos_t_weight;                /* -T * 0.5 * (1 - exp(-(gamma_s - gamma_t))) */
+  float type_t_weight;
+  float pos_log_const;               /* -0.5 * gamma_0 - 0.5 * log(2 pi) */
+  float type_log_const;
+  float pos_alpha_T, type_alpha_T;   /* at t = 1 (the prior) */
+  float pos_log_inv_sigma_T;         /* log(1 / sigma_T) */
+  float type_log_inv_sigma_T;
+  float pos_sigma2_T, type_sigma2_T; /* sigma_T ** 2 */
+} cbg_sbdd_eval_coef;
+
+/* coefs: host array [n_t], n_t <= 32.  x0 / v0 / x_rec: the batch's ligand_pos [n1,3] / ligand_atom_type [n1] /
+ * protein_pos [n_rec1,3] (NULL when the batch has no protein atoms), n1 = n_lig / (2 n_t).  Draws from the caller (normal):
+ * x_t_noise [n_t,n1,3], c_t_noise [n_t,n1,K] (the copy at t), x_0_noise, c_0_noise (the copy at 0).  Outputs:
+ * vec_pos [n_t,3,n1,3] = eps_pred, score_0, score_pred of the positions (score = eps * sigma_t), vec_atom [n_t,3,n1,K]
+ * the same of the types; terms [n_t,B,6] = pos_t, pos_0, pos_kl, atom_t, atom_0, atom_kl of every graph of the batch
+ * (B = n_graphs / (2 n_t)); t_loss [n_t,2] = pos, atom: the mean over the graphs up to the last one with ligand atoms. */
+int32_t cbg_sbdd_eval_loss_f32(const cbg_sample_plan* plan, const cbg_sbdd_eval_coef* coefs, int32_t n_t,
+                               const float* x0, const int64_t* v0, const float* x_rec, const float* x_t_noise,
+                               const float* c_t_noise, const float* x_0_noise, const float* c_0_noise, float* vec_pos,
+                               float* vec_atom, float* terms, float* t_loss, void* stream);
+
 /* ---- SURVEY.md section 8 row f3: sampling-time transforms + batch construction on the device ------------------
  *
  * The reference builds a sampling batch by evaluating dataset[i] num_samples times (sample.py:177), i.e. by running
