@@ -3,14 +3,24 @@
 // sub-layer; reference: x2h_attention.py:58-83, h2x_attention.py:42-62, common.py:151-171), half the tensor-core time
 // and half the operand bytes of the 3xTF32 version at the same accuracy class (cbg_tc.cuh).
 //
-// One CTA = one 128-row tile = two consumer warpgroups of 64 rows (wgmma M = 64) + a copy warp.  A (rows of h, scaled by
-// 16) is split once per CTA into hi/lo f16 tiles in shared memory (canonical K-major layout, read through wgmma
-// descriptors); the weight planes (scaled by 256) are pre-split and pre-laid-out by the packer in 64-wide K chunks
+// One CTA = one 128-row tile = two consumer warpgroups of 64 rows (wgmma M = 64) + a copy warp.  A (rows of h, each
+// scaled by its own power of two) is split once per CTA into hi/lo f16 tiles in shared memory (canonical K-major layout,
+// read through wgmma descriptors); the weight planes (scaled by 256) are pre-split and pre-laid-out by the packer in 64-wide K chunks
 // (hi | lo = 32 KB) and stream through a 3-stage ring with cp.async.bulk + mbarrier.  Each warpgroup holds the
 // 64 x 128 fp32 accumulator of its rows in registers and runs the epilogue from them: a quad of lanes owns 8 consecutive
 // columns of a row, so the plane rows go to global memory as full 32-byte sectors with no staging.  LayerNorm + ReLU
 // of the q MLP is done in registers (row sums over the quad) and written to a second (hi | lo) A tile for the second
 // Linear; only the owning warpgroup reads those rows back, so that hand-over is a warpgroup barrier.
+//
+// Operand windows.  The split keeps ~2^-22 relative accuracy only while hi stays below the f16 maximum (65504) and lo
+// stays a normal f16 (>= 2^-14), so every operand is scaled by a power of two into that window:
+//   - W (packer, x256): |W| < 256 is checked when the blob is packed (modules.py raises ValueError above it).
+//   - q hidden after LayerNorm + ReLU (x16): bounded by sqrt(127) max|gamma| + max|beta|, checked by the packer.
+//   - h (run time, per row): h is data, so no fixed scale fits every input.  Row r is scaled by 2^e_r with
+//     max|h_r| 2^e_r in [2^10, 2^11) (e_r clamped to [-126, 118] so that both 2^e_r and 2^(-8 - e_r) are normal fp32,
+//     e_r = 0 for a zero row), and the epilogue of the GEMMs that read this tile multiplies by 2^(-8 - e_r).  Both
+//     scales are powers of two, so the scaling adds no rounding.  The staging threads r and r + 128 each reduce the
+//     max over their half of row r and exchange it through shared memory behind a named barrier of the 256 threads.
 #include "cbg_kernels.cuh"
 #include "cbg_tc.cuh"
 
@@ -28,23 +38,34 @@ constexpr uint32_t B_STAGE = 2 * B_CHUNK;
 constexpr uint32_t SM_A_HI = 0;                            // rows of h (hi at +0, lo at +A_TILE)
 constexpr uint32_t SM_Q = 2 * A_TILE;                      // relu(LN(q hidden)), same (hi | lo) layout
 constexpr uint32_t SM_B0 = 4 * A_TILE;
-constexpr uint32_t SM_BARS = SM_B0 + STAGES * B_STAGE;
+constexpr uint32_t SM_ROWMAX = SM_B0 + STAGES * B_STAGE;   // [2][128] fp32: max|h| over each half of a row of the tile
+constexpr uint32_t SM_BARS = SM_ROWMAX + 2 * TM * 4;
 constexpr uint32_t SM_TOTAL = SM_BARS + 64;
 static_assert(SM_TOTAL <= 232448, "shared memory budget");
 constexpr uint32_t A_SBO = (CBG_H / 8) * 128, B_SBO = (KC / 8) * 128, LBO = 128;
-constexpr float kScaleA = 16.f;                // h (and the LayerNorm'ed q hidden) in the A tiles
-constexpr float kInvAcc = 1.f / 4096.f;        // weights are scaled by 256 (packer): accumulator at 2^12
+constexpr float kScaleQ = 16.f;                // the LayerNorm'ed q hidden in its A tile (bounded by the packer)
+constexpr float kInvAcc = 1.f / 4096.f;        // q tile x16, weights x256 (packer): accumulator at 2^12
+constexpr int kBarStage = 3;                   // named barrier of the 256 A-staging threads (1, 2: warpgroup_sync)
+
+// e_r of a row whose max |h| is m: m 2^e_r in [2^10, 2^11), clamped to [-126, 118] (2^e_r and 2^(-8 - e_r) normal
+// fp32; this clamp also covers subnormal, inf and NaN maxima), 0 for a zero row
+__device__ __forceinline__ int row_exp(float m) {
+  if (m == 0.f) return 0;
+  const int e = 137 - (int)((__float_as_uint(m) >> 23) & 0xffu);
+  return e < -126 ? -126 : (e > 118 ? 118 : e);
+}
+__device__ __forceinline__ float exp2i(int e) { return __uint_as_float((uint32_t)(e + 127) << 23); }   // normal range only
 
 // byte offset of elements (row, k .. k+7) inside an A tile (k a multiple of 8: one 16-byte core-matrix row)
 __device__ __forceinline__ uint32_t a_off8(int row, int k8) {
   return (uint32_t)(row >> 3) * A_SBO + (uint32_t)k8 * 128u + (uint32_t)(row & 7) * 16u;
 }
-__device__ __forceinline__ void store_split8(uint8_t* tile, int row, int k8, const float4 a, const float4 b) {
+__device__ __forceinline__ void store_split8(uint8_t* tile, int row, int k8, const float4 a, const float4 b, float sc) {
   uint4 hi, lo;
-  split_pair(a.x * kScaleA, a.y * kScaleA, hi.x, lo.x);
-  split_pair(a.z * kScaleA, a.w * kScaleA, hi.y, lo.y);
-  split_pair(b.x * kScaleA, b.y * kScaleA, hi.z, lo.z);
-  split_pair(b.z * kScaleA, b.w * kScaleA, hi.w, lo.w);
+  split_pair(a.x * sc, a.y * sc, hi.x, lo.x);
+  split_pair(a.z * sc, a.w * sc, hi.y, lo.y);
+  split_pair(b.x * sc, b.y * sc, hi.z, lo.z);
+  split_pair(b.z * sc, b.w * sc, hi.w, lo.w);
   const uint32_t off = a_off8(row, k8);
   *reinterpret_cast<uint4*>(tile + off) = hi;
   *reinterpret_cast<uint4*>(tile + A_TILE + off) = lo;
@@ -134,8 +155,16 @@ __global__ void __launch_bounds__(288, 1) node_gemm_f16_kernel(const __grid_cons
       v[2 * j] = live ? ldg4(arow + 8 * k8) : z;
       v[2 * j + 1] = live ? ldg4(arow + 8 * k8 + 4) : z;
     }
+    // per-row scale: max |h| over this thread's half of the row, combined with the other half's through shared memory
+    float m = 0.f;
 #pragma unroll
-    for (int j = 0; j < 8; ++j) store_split8(smem + SM_A_HI, r, (tid >> 7) + 2 * j, v[2 * j], v[2 * j + 1]);
+    for (int j = 0; j < 16; ++j) m = fmaxf(m, fmaxf(fmaxf(fabsf(v[j].x), fabsf(v[j].y)), fmaxf(fabsf(v[j].z), fabsf(v[j].w))));
+    float* rowmax = reinterpret_cast<float*>(smem + SM_ROWMAX);
+    rowmax[tid] = m;
+    asm volatile("bar.sync %0, 256;" ::"r"(kBarStage) : "memory");
+    const float sc = exp2i(row_exp(fmaxf(rowmax[r], rowmax[r + TM])));
+#pragma unroll
+    for (int j = 0; j < 8; ++j) store_split8(smem + SM_A_HI, r, (tid >> 7) + 2 * j, v[2 * j], v[2 * j + 1], sc);
     fence_proxy_async();
   }
   __syncthreads();
@@ -157,10 +186,13 @@ __global__ void __launch_bounds__(288, 1) node_gemm_f16_kernel(const __grid_cons
   const int wg = warp >> 2, qg = lane >> 2, qt = lane & 3;
   const int r_lo = 64 * wg + 16 * (warp & 3) + qg;            // this thread's accumulator rows: r_lo and r_lo + 8
   int node[2];
+  float inv_acc_h[2];                                           // 2^(-8 - e_r): accumulators of the GEMMs that read h
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     const int grow = row0 + r_lo + 8 * h;
     node[h] = (grow < n_rows) ? (p.row_idx ? p.row_idx[grow] : grow) : -1;
+    const float* rowmax = reinterpret_cast<const float*>(smem + SM_ROWMAX);
+    inv_acc_h[h] = exp2i(-8 - row_exp(fmaxf(rowmax[r_lo + 8 * h], rowmax[r_lo + 8 * h + TM])));
   }
   for (int g = 0; g < sc.n_gemm; ++g) {
     const int kind = sc.kind(g), rel = sc.rel(p, g);
@@ -197,10 +229,11 @@ __global__ void __launch_bounds__(288, 1) node_gemm_f16_kernel(const __grid_cons
       for (int h = 0; h < 2; ++h) {
         if (node[h] < 0 || row0 + r_lo + 8 * h >= row_lim) continue;
         float* o = out + (size_t)node[h] * CBG_H + 2 * qt;
+        const float inv = kind == 2 ? kInvAcc : inv_acc_h[h];
 #pragma unroll
         for (int j = 0; j < 16; ++j) {
           const float2 b = __ldg(reinterpret_cast<const float2*>(bias + 8 * j + 2 * qt));
-          *reinterpret_cast<float2*>(o + 8 * j) = make_float2(fmaf(d[4 * j + 2 * h], kInvAcc, b.x), fmaf(d[4 * j + 2 * h + 1], kInvAcc, b.y));
+          *reinterpret_cast<float2*>(o + 8 * j) = make_float2(fmaf(d[4 * j + 2 * h], inv, b.x), fmaf(d[4 * j + 2 * h + 1], inv, b.y));
         }
       }
     } else {
@@ -211,10 +244,10 @@ __global__ void __launch_bounds__(288, 1) node_gemm_f16_kernel(const __grid_cons
 #pragma unroll
       for (int j = 0; j < 16; ++j) {
         const float2 b = __ldg(reinterpret_cast<const float2*>(bias + 8 * j + 2 * qt));
-        d[4 * j] = fmaf(d[4 * j], kInvAcc, b.x);
-        d[4 * j + 1] = fmaf(d[4 * j + 1], kInvAcc, b.y);
-        d[4 * j + 2] = fmaf(d[4 * j + 2], kInvAcc, b.x);
-        d[4 * j + 3] = fmaf(d[4 * j + 3], kInvAcc, b.y);
+        d[4 * j] = fmaf(d[4 * j], inv_acc_h[0], b.x);
+        d[4 * j + 1] = fmaf(d[4 * j + 1], inv_acc_h[0], b.y);
+        d[4 * j + 2] = fmaf(d[4 * j + 2], inv_acc_h[1], b.x);
+        d[4 * j + 3] = fmaf(d[4 * j + 3], inv_acc_h[1], b.y);
         s0 += d[4 * j] + d[4 * j + 1];
         s1 += d[4 * j + 2] + d[4 * j + 3];
       }
@@ -238,7 +271,7 @@ __global__ void __launch_bounds__(288, 1) node_gemm_f16_kernel(const __grid_cons
           const float a0 = fmaxf(fmaf(d[4 * j + 2 * h] * rs, gm.x, bt.x), 0.f);
           const float a1 = fmaxf(fmaf(d[4 * j + 2 * h + 1] * rs, gm.y, bt.y), 0.f);
           uint32_t hi, lo;
-          split_pair(a0 * kScaleA, a1 * kScaleA, hi, lo);
+          split_pair(a0 * kScaleQ, a1 * kScaleQ, hi, lo);
           const uint32_t off = a_off8(r_lo + 8 * h, j) + 4u * (uint32_t)qt;
           *reinterpret_cast<uint32_t*>(smem + SM_Q + off) = hi;
           *reinterpret_cast<uint32_t*>(smem + SM_Q + A_TILE + off) = lo;

@@ -129,20 +129,38 @@ def tc_weight_plane(w):
     return torch.from_numpy(out.reshape(-1)).to(torch.float64)
 
 
-def tc_f16_image(w):
-    """[n][K k] matrix (n = 128, or 16 for the H2X value head; float64, already scaled by its power of two) -> the (hi | lo) f16 operand images of the
-    wgmma X2H kernels (csrc/x2h_tc.cu): w ~= hi + lo, each image in the canonical K-major / no-swizzle layout
-    for 16-bit types (8-row x 8-element core matrices, 128 B apart along K, K/8 * 128 B between 8-row groups).
-    Returns the raw bits as an int32 tensor (two f16 per word)."""
+def tc_f16_image(w, what='weight image', scale=1.0):
+    """[n][K k] matrix (n = 128, or 16 for the H2X value head; float64, already scaled by ``scale``, its power of two) ->
+    the (hi | lo) f16 operand images of the wgmma kernels (csrc/x2h_tc.cu, csrc/node_gemm_f16.cu): w ~= hi + lo, each
+    image in the canonical K-major / no-swizzle layout for 16-bit types (8-row x 8-element core matrices, 128 B apart
+    along K, K/8 * 128 B between 8-row groups).  Returns the raw bits as an int32 tensor (two f16 per word).
+    Raises ValueError (naming ``what``) when a scaled weight leaves the f16 range: hi would be inf and every product
+    that reads it NaN."""
     import numpy as np
     w = np.asarray(w, dtype=np.float64)
     n, k = w.shape
     assert n % 8 == 0 and k % 16 == 0
-    hi = w.astype(np.float16)
-    lo = (w - hi.astype(np.float64)).astype(np.float16)
+    with np.errstate(over='ignore', invalid='ignore'):
+        hi = w.astype(np.float16)
+        lo = (w - hi.astype(np.float64)).astype(np.float16)
+    if not (np.isfinite(hi).all() and np.isfinite(lo).all()):
+        big = float(np.nanmax(np.abs(w))) / scale if np.isfinite(w).any() else float('nan')
+        raise ValueError(f'{what}: max |w| = {big:.6g} does not fit the f16 tensor-core image (|w| x {scale:g} must stay '
+                         f'below {F16_MAX:g}, i.e. |w| < {F16_MAX / scale:.6g}), or a weight is not finite')
     imgs = [m.reshape(n // 8, 8, k // 8, 8).transpose(0, 2, 1, 3).reshape(-1) for m in (hi, lo)]
-    assert np.isfinite(np.concatenate(imgs).astype(np.float32)).all(), 'f16 overflow in a tensor-core weight image'
     return torch.from_numpy(np.concatenate(imgs).view(np.int32).copy())
+
+
+def check_ln_activation_bound(ln_params, scale, what):
+    """relu(LayerNorm(x) * gamma + beta) over 128 features is bounded by sqrt(127) max|gamma| + max|beta| (no normalised
+    feature exceeds sqrt(n - 1)).  The wgmma kernels split these activations into f16 (hi, lo) after multiplying by
+    ``scale``; raise ValueError (naming ``what``) when the scaled bound reaches the f16 maximum."""
+    g, b = ln_params[:HIDDEN], ln_params[HIDDEN:]
+    bound = math.sqrt(HIDDEN - 1) * float(g.abs().max()) + float(b.abs().max())
+    if not bound * scale < F16_MAX:
+        raise ValueError(f'{what}: LayerNorm activation bound sqrt(127) max|gamma| + max|beta| = {bound:.6g} times '
+                         f'{scale:g} reaches the f16 maximum {F16_MAX:g} of the tensor-core operand '
+                         f'(the bound must stay below {F16_MAX / scale:.6g})')
 
 
 # power-of-two scales of the f16 images (must match csrc/x2h_tc.cu)
@@ -150,6 +168,9 @@ TC_SCALE_WG = 16.0
 TC_SCALE_W1 = 64.0
 TC_KG = 96
 TC_SCALE_NODE = 256.0       # node GEMM weight planes (csrc/node_gemm_f16.cu)
+TC_SCALE_ACT = 64.0         # LayerNorm + ReLU activations of the edge MLPs (csrc/x2h_tc.cu)
+TC_SCALE_Q = 16.0           # LayerNorm + ReLU activations of the q MLP (csrc/node_gemm_f16.cu)
+F16_MAX = 65504.0
 
 
 def pack_denoiser_blob(sd, prefix, num_layers, num_classes, com_head=False):
@@ -235,20 +256,28 @@ def pack_denoiser_blob(sd, prefix, num_layers, num_classes, com_head=False):
             tc = [w0k[:, 212:340], w0v[:, 212:340], w0k[:, 84:212], w0v[:, 84:212],
                   _t(sd[sp + qname + '.net.0.weight']), _t(sd[sp + qname + '.net.3.weight']) * inv_sqrt_dh]
             put(base, lf, f'{tag}_NODE_TC', torch.cat([tc_weight_plane(m.to(torch.float32)) for m in tc]))
-            put_raw(base, lf, f'{tag}_NODE_TCH', torch.cat([tc_f16_image((m[:, 64 * c: 64 * c + 64] * TC_SCALE_NODE).numpy())
-                                                             for m in tc for c in range(2)]))
+            where = f'layer {l} {tag}'
+            put_raw(base, lf, f'{tag}_NODE_TCH', torch.cat([tc_f16_image((m[:, 64 * c: 64 * c + 64] * TC_SCALE_NODE).numpy(),
+                                                                         f'{where}_NODE_TCH', TC_SCALE_NODE)
+                                                            for m in tc for c in range(2)]))
             put(base, lf, f'{tag}_NODE_B', node_b)
-            put(base, lf, f'{tag}_Q_LN', torch.cat([_t(sd[sp + qname + '.net.1.weight']), _t(sd[sp + qname + '.net.1.bias'])]))
+            q_ln = torch.cat([_t(sd[sp + qname + '.net.1.weight']), _t(sd[sp + qname + '.net.1.bias'])])
+            check_ln_activation_bound(q_ln, TC_SCALE_Q, f'{where}_Q_LN')
+            put(base, lf, f'{tag}_Q_LN', q_ln)
             put(base, lf, f'{tag}_Q_W1T', (_t(sd[sp + qname + '.net.3.weight']) * inv_sqrt_dh).t().contiguous())
             put(base, lf, f'{tag}_Q_B1', _t(sd[sp + qname + '.net.3.bias']) * inv_sqrt_dh)
             rbf = rbf_field(sd[sp + 'distance_expansion.offset'])
             put(base, lf, f'{tag}_K_WRF', wrf_k)
             put(base, lf, f'{tag}_K_C', c_k)
-            put(base, lf, f'{tag}_K_LN', torch.cat([_t(sd[sp + kname + '.net.1.weight']), _t(sd[sp + kname + '.net.1.bias'])]))
+            k_ln = torch.cat([_t(sd[sp + kname + '.net.1.weight']), _t(sd[sp + kname + '.net.1.bias'])])
+            v_ln = torch.cat([_t(sd[sp + vname + '.net.1.weight']), _t(sd[sp + vname + '.net.1.bias'])])
+            check_ln_activation_bound(k_ln, TC_SCALE_ACT, f'{where}_K_LN')
+            check_ln_activation_bound(v_ln, TC_SCALE_ACT, f'{where}_V_LN')
+            put(base, lf, f'{tag}_K_LN', k_ln)
             put(base, lf, f'{tag}_K_W1', _t(sd[sp + kname + '.net.3.weight']))
             put(base, lf, f'{tag}_V_WRF', wrf_v)
             put(base, lf, f'{tag}_V_C', c_v)
-            put(base, lf, f'{tag}_V_LN', torch.cat([_t(sd[sp + vname + '.net.1.weight']), _t(sd[sp + vname + '.net.1.bias'])]))
+            put(base, lf, f'{tag}_V_LN', v_ln)
             put(base, lf, f'{tag}_V_W1', _t(sd[sp + vname + '.net.3.weight']))
             put(base, lf, f'{tag}_V_B1', _t(sd[sp + vname + '.net.3.bias']))
             if tag == 'X2H':
@@ -262,8 +291,8 @@ def pack_denoiser_blob(sd, prefix, num_layers, num_classes, com_head=False):
                 wg = torch.zeros(HIDDEN, TC_KG, dtype=torch.float64)     # [f][k]: k = 20 t + m | 80 + t | Pi columns
                 wg[:, 0:80] = w0[:, 4:84]
                 wg[:, 80:84] = w0[:, 0:4]
-                put_raw(base, lf, f'{tag}_{kv}_TCWG', tc_f16_image((wg * TC_SCALE_WG).numpy()))
-                put_raw(base, lf, f'{tag}_{kv}_TCW1', tc_f16_image((w1 * TC_SCALE_W1).numpy()))
+                put_raw(base, lf, f'{tag}_{kv}_TCWG', tc_f16_image((wg * TC_SCALE_WG).numpy(), f'{where}_{kv}_TCWG', TC_SCALE_WG))
+                put_raw(base, lf, f'{tag}_{kv}_TCW1', tc_f16_image((w1 * TC_SCALE_W1).numpy(), f'{where}_{kv}_TCW1', TC_SCALE_W1))
     blob32 = blob.to(torch.float32)
     bits = blob32.view(torch.int32)
     for off, b in raw:
