@@ -64,6 +64,27 @@ class BpCoef(C.Structure):
     _fields_ = [('alpha_cumprod', C.c_float), ('beta', C.c_float), ('nonzero', C.c_float), ('change_prob', C.c_float)]
 
 
+class FgPlan(C.Structure):
+    _fields_ = [
+        ('blob', C.c_void_p), ('hidden', C.c_int32), ('num_sublayers', C.c_int32), ('num_blocks', C.c_int32),
+        ('num_classes', C.c_int32), ('k', C.c_int32),
+        ('graph_ptr', C.c_void_p), ('n_graphs', C.c_int32), ('max_graph_nodes', C.c_int32), ('n_nodes', C.c_int64),
+        ('lig_flag', C.c_void_p), ('gen_flag', C.c_void_p), ('lig_node', C.c_void_p), ('gen_lig', C.c_void_p),
+        ('n_lig', C.c_int32), ('x', C.c_void_p), ('o', C.c_void_p), ('h', C.c_void_p),
+        ('fg_emb_t', C.c_void_p), ('fg_emb_b', C.c_void_p), ('lig_indicator', C.c_void_p),
+        ('angle_x', C.c_void_p), ('angle_cdf', C.c_void_p), ('n_bins', C.c_int32),
+        ('workspace', C.c_void_p), ('workspace_bytes', C.c_int64),
+    ]
+
+
+class FgCoef(C.Structure):
+    _fields_ = [('t', C.c_int32), ('pos_beta', C.c_float), ('pos_sigma', C.c_float),
+                ('pos_sqrt_one_minus_beta', C.c_float), ('pos_noise_scale', C.c_float), ('rot_std', C.c_float),
+                ('rot_gaussian', C.c_int32), ('rot_noise', C.c_int32),
+                ('log_alphas_cumprod_prev', C.c_float), ('log_one_minus_alphas_cumprod_prev', C.c_float),
+                ('log_alpha', C.c_float), ('log_one_minus_alpha', C.c_float)]
+
+
 _P, _I32, _I64, _F, _SZ = C.c_void_p, C.c_int32, C.c_int64, C.c_float, C.c_size_t
 
 # name -> (restype, argtypes); must list every symbol of include/cbg_b200.h
@@ -123,6 +144,8 @@ SIGNATURES = {
     'cbg_ipa_workspace_bytes': (_I64, [_I64, _I32]),
     'cbg_ipa_forward_f32': (_I32, [_P, _I32, _I32, _I32, _I32, _P, _P, _P, _P, _I32, _I32, _P, _P, _I64, _I32,
                                    _P, _P, _P, _P, _P, _P, _I64, _P]),
+    'cbg_fg_workspace_bytes': (_I64, [_I64, _I32, _I32]),
+    'cbg_fg_step_f32': (_I32, [C.POINTER(FgPlan), FgCoef, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     'cbg_reverse_step_f32': (_I32, [C.POINTER(StepCoef), _P, _P, _P, _P, _P, _P, _P, _I32, _I32, _P, _P, _P, _P]),
 }
 

@@ -324,3 +324,38 @@ int cbg_launch_build_batch(const float* prot_pos, const int* prot_element, const
                            float* o_prot_pos, float* o_prot_feat, long long* o_prot_aa, long long* o_prot_batch,
                            float* o_prot_tr, float* o_lig_pos, long long* o_lig_type, long long* o_lig_batch,
                            unsigned char* o_lig_ctx, unsigned char* o_lig_gen, cudaStream_t st);
+
+// ipa.cu (row f4): the IPATransformer forward behind cbg_ipa_forward_f32, arguments already validated; ws holds
+// cbg_ipa_workspace_bytes(N, hidden) bytes, 256-byte aligned
+int cbg_ipa_launch(const float* blob, int hidden, int num_sublayers, int num_blocks, int num_classes, const float* x,
+                   const float* o, const float* h_in, const int* graph_ptr, int n_graphs, int max_graph_nodes,
+                   const unsigned char* lig_flag, const unsigned char* gen_flag, int N, int k, float* eps_pos, float* h_out,
+                   float* o_next, float* R_next, float* logits, char* ws, cudaStream_t st);
+
+// ---- SO(3) maps of repo/models/utils/so3.py in fp32, used by ipa.cu (heads) and fg.cu (D3FG orientation step) ----------
+__device__ __forceinline__ void mat3_mul(const float* A, const float* B, float* C) {
+#pragma unroll
+  for (int r = 0; r < 3; ++r)
+#pragma unroll
+    for (int c = 0; c < 3; ++c) C[3 * r + c] = A[3 * r] * B[c] + A[3 * r + 1] * B[3 + c] + A[3 * r + 2] * B[6 + c];
+}
+// R = exp_skewsym(so3vec_to_skewsym(w))   so3.py:33-57
+__device__ __forceinline__ void so3vec_to_rotation(float wx, float wy, float wz, float* R) {
+  const float S[9] = {0.f, wz, -wy, -wz, 0.f, wx, wy, -wx, 0.f};
+  const float xn = sqrtf(wx * wx + wy * wy + wz * wz);
+  const float bb = (sinf(xn) + 1e-8f) / (xn + 1e-8f);
+  const float cb = (1.f - cosf(xn) + 1e-8f) / (xn * xn + 2e-8f);
+  float S2[9];
+  mat3_mul(S, S, S2);
+#pragma unroll
+  for (int e = 0; e < 9; ++e) R[e] = ((e % 4 == 0) ? 1.f : 0.f) + bb * S[e] + cb * S2[e];
+}
+// w = skewsym_to_so3vec(log_rotation(R))   so3.py:10-31, 60-63 (no-grad branch: cos clamped at -1)
+__device__ __forceinline__ void rotation_to_so3vec(const float* R, float* w) {
+  const float tr = R[0] + R[4] + R[8];
+  const float cos_t = fmaxf((tr - 1.f) * 0.5f, -1.f);
+  const float sin_t = sqrtf(1.f - cos_t * cos_t);
+  const float theta = acosf(cos_t);
+  const float coef = (theta + 1e-8f) / (2.f * sin_t + 2e-8f);
+  w[0] = coef * (R[5] - R[7]); w[1] = coef * (R[6] - R[2]); w[2] = coef * (R[1] - R[3]);
+}

@@ -20,6 +20,7 @@
 #define CBG_KMAX      32   // neighbour-table width (k <= 32)
 #define CBG_GATE_H   160   // dist_emb MLP hidden = 8 * num_r_gaussian
 #define CBG_MAXCLS    16   // classifier rows are padded to 16 (num_classes <= 16)
+#define CBG_IPA_MAXCLS 32  // IPATransformer type head (csrc/ipa.cu): rows padded to 32 (D3FG: 28 functional-group types)
 #define CBG_NPLANES    5   // node projection planes per sub-layer: Pj_k, Pj_v, Pi_k, Pi_v, q_hidden
 #define CBG_NODE_SRC_PLANES 2   // the first two are gathered by edges from the SOURCE node, the rest belong to the destination
 

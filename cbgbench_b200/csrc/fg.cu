@@ -1,0 +1,210 @@
+// D3FG sampling step (`difffg` / `difffg_v2`, repo/models/diffusion/difffg.py:174-246), DESIGN.md section 16.
+//
+// One call per reverse step t:
+//   fg_embed_kernel    ligand rows of the composed arrays from the state: x = xc, o = o_t and
+//                      h = ligand_fg_emb(onehot49(argmax c_t)) + ligand_indicator(1)   (context_emb.py:95-128)
+//   cbg_ipa_launch     the IPATransformer on the composed graph (csrc/ipa.cu)
+//   fg_reverse_kernel  one warp per functional group: CTNVPScheduler.backward_remove_noise (score form,
+//                      diffusion_scheduler.py:144-165), RotVPScheduler.backward_remove_noise (:558-574, so3.py:111-146)
+//                      and TypeVPScheduler.backward_remove_noise (:367-378); lane k holds class k.
+// The protein rows are step-invariant and written once per batch by the host.  No atomics: a step is bit-reproducible.
+#include <math.h>
+#include "../../include/cbg_b200.h"
+#include "cbg_kernels.cuh"
+
+namespace {
+
+__device__ __forceinline__ float fg_log_add_exp(float a, float b) {      // categorical.py: log_add_exp
+  const float m = fmaxf(a, b);
+  return m + logf(expf(a - m) + expf(b - m));
+}
+
+__device__ __forceinline__ float fg_warp_max(float v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(CBG_FULL, v, o));
+  return v;
+}
+
+__device__ __forceinline__ float fg_warp_sum(float v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(CBG_FULL, v, o);
+  return v;
+}
+
+// torch.argmax over the lanes: the largest value, the lowest index among equal values
+__device__ __forceinline__ int fg_warp_argmax(float v, int idx) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const float ov = __shfl_xor_sync(CBG_FULL, v, o);
+    const int oi = __shfl_xor_sync(CBG_FULL, idx, o);
+    if (ov > v || (ov == v && oi < idx)) { v = ov; idx = oi; }
+  }
+  return idx;
+}
+
+__global__ void __launch_bounds__(256) fg_embed_kernel(cbg_fg_plan p, const float* __restrict__ x_t,
+                                                       const float* __restrict__ c_t, const float* __restrict__ o_t) {
+  const int a = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (a >= p.n_lig) return;
+  const int K = p.num_classes, H = p.hidden;
+  const int i = p.lig_node[a];
+  const float cv = lane < K ? c_t[(size_t)a * K + lane] : -INFINITY;
+  const int v = fg_warp_argmax(cv, lane < K ? lane : 1 << 30);
+  const float* w = p.fg_emb_t + (size_t)v * H;
+  for (int f = lane; f < H; f += 32) p.h[(size_t)i * H + f] = (w[f] + p.fg_emb_b[f]) + p.lig_indicator[f];
+  if (lane < 3) {
+    p.x[3 * i + lane] = x_t[3 * a + lane];
+    p.o[3 * i + lane] = o_t[3 * a + lane];
+  }
+}
+
+struct FgOut {
+  const float* eps_pos;   // [N,3]
+  const float* o_pred;    // [N,3]
+  const float* logits;    // [N,K]
+};
+
+__global__ void __launch_bounds__(256) fg_reverse_kernel(cbg_fg_plan p, cbg_fg_coef cf, FgOut in,
+                                                         const float* __restrict__ x_t, const float* __restrict__ c_t,
+                                                         const float* __restrict__ o_t, const float* __restrict__ pos_noise,
+                                                         const float* __restrict__ rot_draws,
+                                                         const float* __restrict__ type_u, float* __restrict__ x_next,
+                                                         float* __restrict__ c_next, float* __restrict__ o_next) {
+  const int a = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (a >= p.n_lig) return;
+  const int K = p.num_classes;
+  const int i = p.lig_node[a];
+  const bool gen = p.gen_lig[a] != 0;
+
+  // positions: x' = (x + b * (-eps / sqrt(1 - abar))) / sqrt(1 - b) + [t != 0] sqrt(b) n
+  if (lane < 3) {
+    const float xt = x_t[3 * a + lane];
+    const float score = __fdiv_rn(-in.eps_pos[3 * i + lane], cf.pos_sigma);
+    float xs = __fdiv_rn(__fadd_rn(xt, __fmul_rn(cf.pos_beta, score)), cf.pos_sqrt_one_minus_beta);
+    xs = __fadd_rn(xs, __fmul_rn(cf.pos_noise_scale, pos_noise[3 * a + lane]));
+    x_next[3 * a + lane] = gen ? xs : xt;
+  }
+
+  // orientation: R' = exp(e) exp(o_pred), e = normalize(axis) * theta (zero at t <= 1)
+  if (lane == 0) {
+    const float* rd = rot_draws + (size_t)a * 6;
+    float e[3] = {0.f, 0.f, 0.f};
+    if (cf.rot_noise) {
+      float theta;
+      if (cf.rot_gaussian) {        // |2 sigma + sigma n| mod pi
+        theta = fmodf(fabsf(__fadd_rn(cf.rot_std * 2.f, __fmul_rn(rd[5], cf.rot_std))), 3.14159265358979323846f);
+      } else {                      // bin b = min{i : C_t[i] > u C_t[n_bins - 2]}, then X[b] + u' (X[b+1] - X[b])
+        const int nc = p.n_bins - 1;
+        const double* C = p.angle_cdf + (size_t)cf.t * nc;
+        const double target = (double)rd[3] * C[nc - 1];
+        int lo = 0, hi = nc - 1;
+        while (lo < hi) {
+          const int mid = (lo + hi) >> 1;
+          if (C[mid] > target) hi = mid; else lo = mid + 1;
+        }
+        const float* X = p.angle_x + (size_t)cf.t * p.n_bins;
+        theta = __fadd_rn(X[lo], __fmul_rn(rd[4], __fsub_rn(X[lo + 1], X[lo])));
+      }
+      const float nrm = fmaxf(sqrtf(rd[0] * rd[0] + rd[1] * rd[1] + rd[2] * rd[2]), 1e-12f);
+#pragma unroll
+      for (int c = 0; c < 3; ++c) e[c] = __fmul_rn(__fdiv_rn(rd[c], nrm), theta);
+    }
+    float E[9], Rp[9], Rn[9], w[3];
+    so3vec_to_rotation(e[0], e[1], e[2], E);
+    so3vec_to_rotation(in.o_pred[3 * i], in.o_pred[3 * i + 1], in.o_pred[3 * i + 2], Rp);
+    mat3_mul(E, Rp, Rn);
+    rotation_to_so3vec(Rn, w);
+#pragma unroll
+    for (int c = 0; c < 3; ++c) o_next[3 * a + c] = gen ? w[c] : o_t[3 * a + c];
+  }
+
+  // FG type: q(v_{t-1} | v_t, softmax(logits)), Gumbel-max draw; lane k = class k
+  const bool on = lane < K;
+  const float lg = on ? in.logits[(size_t)i * K + lane] : -INFINITY;
+  const float mx = fg_warp_max(lg);
+  const float se = fg_warp_sum(on ? expf(lg - mx) : 0.f);
+  const float log_c_pred = (lg - mx) - logf(se);
+  const float ctv = on ? c_t[(size_t)a * K + lane] : -INFINITY;
+  const float logK = logf((float)K);
+  const float A = fg_log_add_exp(log_c_pred + cf.log_alphas_cumprod_prev, cf.log_one_minus_alphas_cumprod_prev - logK);
+  const float B = fg_log_add_exp(logf(ctv + 1e-8f) + cf.log_alpha, cf.log_one_minus_alpha - logK);
+  const float un = on ? A + B : -INFINITY;
+  const float m2 = fg_warp_max(un);
+  const float lse2 = m2 + logf(fg_warp_sum(on ? expf(un - m2) : 0.f));
+  const float u = on ? type_u[(size_t)a * K + lane] : 0.5f;
+  const float score = on ? -logf(-logf(u + 1e-30f) + 1e-30f) + (un - lse2) : -INFINITY;
+  const int sampled = fg_warp_argmax(score, on ? lane : 1 << 30);
+  const int kept = fg_warp_argmax(ctv, on ? lane : 1 << 30);
+  const int v = gen ? sampled : kept;
+  if (on) c_next[(size_t)a * K + lane] = lane == v ? 1.f : 0.f;
+}
+
+size_t al256(size_t b) { return (b + 255) & ~(size_t)255; }
+
+}  // namespace
+
+extern "C" {
+
+int64_t cbg_fg_workspace_bytes(int64_t n_nodes, int32_t hidden, int32_t num_classes) {
+  const size_t n = (size_t)n_nodes;
+  return cbg_ipa_workspace_bytes(n_nodes, hidden) +
+         (int64_t)(2 * al256(n * 3 * 4) + al256(n * hidden * 4) + al256(n * 9 * 4) + al256(n * num_classes * 4));
+}
+
+int32_t cbg_fg_step_f32(const cbg_fg_plan* plan, cbg_fg_coef coef, const float* x_t, const float* c_t, const float* o_t,
+                        const float* pos_noise, const float* rot_draws, const float* type_u, float* x_next, float* c_next,
+                        float* o_next, void* stream) {
+  if (!plan) { cbg_set_error("cbg_fg_step_f32: plan is NULL"); return 1; }
+  const cbg_fg_plan& p = *plan;
+  if (p.hidden != 128 && p.hidden != 256) { cbg_set_error("cbg_fg_step_f32: hidden=%d (128 or 256)", p.hidden); return 1; }
+  if (p.num_classes < 1 || p.num_classes > CBG_IPA_MAXCLS) {
+    cbg_set_error("cbg_fg_step_f32: num_classes=%d outside [1,%d]", p.num_classes, CBG_IPA_MAXCLS);
+    return 1;
+  }
+  if (p.n_nodes <= 0 || p.n_nodes > 0x7fffffffLL / (5 * 256) || p.n_lig < 0 || p.n_lig > p.n_nodes) {
+    cbg_set_error("cbg_fg_step_f32: n_nodes=%lld n_lig=%d", (long long)p.n_nodes, p.n_lig);
+    return 1;
+  }
+  if (p.n_bins < 2 || coef.t < 0) { cbg_set_error("cbg_fg_step_f32: n_bins=%d t=%d", p.n_bins, coef.t); return 1; }
+  if (p.num_blocks < 1 || p.num_sublayers < 0 || p.k < 1 || p.k > CBG_KMAX) {
+    cbg_set_error("cbg_fg_step_f32: num_blocks / num_sublayers / k");
+    return 1;
+  }
+  if (!p.workspace || ((uintptr_t)p.workspace & 255) != 0 ||
+      p.workspace_bytes < cbg_fg_workspace_bytes(p.n_nodes, p.hidden, p.num_classes)) {
+    cbg_set_error("cbg_fg_step_f32: workspace missing, unaligned or too small");
+    return 1;
+  }
+  if (p.n_lig > 0 && (!x_t || !c_t || !o_t || !pos_noise || !rot_draws || !type_u || !x_next || !c_next || !o_next)) {
+    cbg_set_error("cbg_fg_step_f32: NULL state or draw pointer");
+    return 1;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  const int N = (int)p.n_nodes, H = p.hidden, K = p.num_classes;
+  char* ws = (char*)p.workspace;
+  size_t off = al256((size_t)cbg_ipa_workspace_bytes(p.n_nodes, H));
+  auto take = [&](size_t nbytes) { float* q = (float*)(ws + off); off += al256(nbytes); return q; };
+  float* eps_pos = take((size_t)N * 3 * 4);
+  float* o_pred = take((size_t)N * 3 * 4);
+  float* h_out = take((size_t)N * H * 4);
+  float* r_next = take((size_t)N * 9 * 4);
+  float* logits = take((size_t)N * K * 4);
+  const int grid = (p.n_lig + 7) / 8;
+  if (grid > 0) {
+    CBG_PROF_BEGIN(CBG_K_STEP_INIT, st);
+    fg_embed_kernel<<<grid, 256, 0, st>>>(p, x_t, c_t, o_t);
+    CBG_LAUNCHED(CBG_K_STEP_INIT, st);
+  }
+  if (int rc = cbg_ipa_launch(p.blob, H, p.num_sublayers, p.num_blocks, K, p.x, p.o, p.h, p.graph_ptr, p.n_graphs,
+                              p.max_graph_nodes, p.lig_flag, p.gen_flag, N, p.k, eps_pos, h_out, o_pred, r_next, logits, ws, st))
+    return rc;
+  if (grid > 0) {
+    CBG_PROF_BEGIN(CBG_K_REVERSE, st);
+    fg_reverse_kernel<<<grid, 256, 0, st>>>(p, coef, FgOut{eps_pos, o_pred, logits}, x_t, c_t, o_t, pos_noise, rot_draws,
+                                            type_u, x_next, c_next, o_next);
+    CBG_LAUNCHED(CBG_K_REVERSE, st);
+  }
+  return 0;
+}
+
+}  // extern "C"

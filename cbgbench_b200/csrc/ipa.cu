@@ -31,8 +31,8 @@ __host__ __device__ inline long long head_size(int H, int f) {
     case IH_ROT_B2: case IH_CRD_B2: return 4;
     case IH_CLS_W0T: return (long long)H * H;
     case IH_CLS_B0: return H;
-    case IH_CLS_W1: return CBG_MAXCLS * H;
-    case IH_CLS_B1: return CBG_MAXCLS;
+    case IH_CLS_W1: return CBG_IPA_MAXCLS * H;
+    case IH_CLS_B1: return CBG_IPA_MAXCLS;
   }
   return 0;
 }
@@ -274,13 +274,6 @@ __device__ __forceinline__ void head_mlp3(const float* s_h, float* s_t1, float* 
   __syncthreads();
 }
 
-__device__ __forceinline__ void mat3_mul(const float* A, const float* B, float* C) {
-#pragma unroll
-  for (int r = 0; r < 3; ++r)
-#pragma unroll
-    for (int c = 0; c < 3; ++c) C[3 * r + c] = A[3 * r] * B[c] + A[3 * r + 1] * B[3 + c] + A[3 * r + 2] * B[6 + c];
-}
-
 template <int H>
 __global__ void __launch_bounds__(H) ipa_heads_kernel(const float* __restrict__ h, const float* __restrict__ o_in,
                                                       const unsigned char* __restrict__ gen, const float* __restrict__ P,
@@ -322,22 +315,11 @@ __global__ void __launch_bounds__(H) ipa_heads_kernel(const float* __restrict__ 
                         2 * b * d - 2 * a * c, 2 * c * d + 2 * a * b, a * a - b * b - c * c + d * d};
     // R_o = exp_skewsym(so3vec_to_skewsym(o))               so3.py:33-57
     const float wx = o_in[3 * i], wy = o_in[3 * i + 1], wz = o_in[3 * i + 2];
-    const float S[9] = {0.f, wz, -wy, -wz, 0.f, wx, wy, -wx, 0.f};
-    const float xn = sqrtf(wx * wx + wy * wy + wz * wz);
-    const float bb = (sinf(xn) + 1e-8f) / (xn + 1e-8f);
-    const float cb = (1.f - cosf(xn) + 1e-8f) / (xn * xn + 2e-8f);
-    float S2[9], Ro[9], Rn[9];
-    mat3_mul(S, S, S2);
-#pragma unroll
-    for (int e = 0; e < 9; ++e) Ro[e] = ((e % 4 == 0) ? 1.f : 0.f) + bb * S[e] + cb * S2[e];
+    float Ro[9], Rn[9], l[3];
+    so3vec_to_rotation(wx, wy, wz, Ro);
     mat3_mul(Ro, U, Rn);                                      // R_next = R_o @ U_update   (itatransformer.py:131)
-    // o_next = rotation_to_so3vec(R_next) = skewsym_to_so3vec(log_rotation(R_next))   so3.py:10-31, 60-63 (no-grad branch)
-    const float tr = Rn[0] + Rn[4] + Rn[8];
-    const float cos_t = fmaxf((tr - 1.f) * 0.5f, -1.f);
-    const float sin_t = sqrtf(1.f - cos_t * cos_t);
-    const float theta = acosf(cos_t);
-    const float coef = (theta + 1e-8f) / (2.f * sin_t + 2e-8f);
-    const float lx = coef * (Rn[5] - Rn[7]), ly = coef * (Rn[6] - Rn[2]), lz = coef * (Rn[1] - Rn[3]);
+    rotation_to_so3vec(Rn, l);
+    const float lx = l[0], ly = l[1], lz = l[2];
     const bool g = gen[i] != 0;
     o_next[3 * i] = g ? lx : wx; o_next[3 * i + 1] = g ? ly : wy; o_next[3 * i + 2] = g ? lz : wz;
 #pragma unroll
@@ -407,6 +389,17 @@ int ipa_forward_t(const float* blob, int num_sublayers, int num_blocks, int num_
 
 }  // namespace
 
+int cbg_ipa_launch(const float* blob, int hidden, int num_sublayers, int num_blocks, int num_classes, const float* x,
+                   const float* o, const float* h_in, const int* graph_ptr, int n_graphs, int max_graph_nodes,
+                   const unsigned char* lig_flag, const unsigned char* gen_flag, int N, int k, float* eps_pos, float* h_out,
+                   float* o_next, float* R_next, float* logits, char* ws, cudaStream_t st) {
+  if (hidden == 128)
+    return ipa_forward_t<128>(blob, num_sublayers, num_blocks, num_classes, x, o, h_in, graph_ptr, n_graphs, max_graph_nodes,
+                              lig_flag, gen_flag, N, k, eps_pos, h_out, o_next, R_next, logits, ws, st);
+  return ipa_forward_t<256>(blob, num_sublayers, num_blocks, num_classes, x, o, h_in, graph_ptr, n_graphs, max_graph_nodes,
+                            lig_flag, gen_flag, N, k, eps_pos, h_out, o_next, R_next, logits, ws, st);
+}
+
 extern "C" {
 
 int64_t cbg_ipa_head_floats(int32_t hidden) {
@@ -447,17 +440,14 @@ int32_t cbg_ipa_forward_f32(const float* blob, int32_t hidden, int32_t num_subla
                             int32_t k, float* eps_pos, float* h_out, float* o_next, float* r_next, float* logits,
                             void* workspace, int64_t workspace_bytes, void* stream) {
   if (hidden != 128 && hidden != 256) { cbg_set_error("cbg_ipa_forward_f32: hidden=%d (128 or 256)", hidden); return 1; }
-  if (num_classes < 1 || num_classes > CBG_MAXCLS) { cbg_set_error("num_classes=%d outside [1,%d]", num_classes, CBG_MAXCLS); return 1; }
+  if (num_classes < 1 || num_classes > CBG_IPA_MAXCLS) { cbg_set_error("num_classes=%d outside [1,%d]", num_classes, CBG_IPA_MAXCLS); return 1; }
   if (n_nodes <= 0 || n_nodes > 0x7fffffffLL / (5 * 256)) { cbg_set_error("n_nodes=%lld out of range", (long long)n_nodes); return 1; }
   if (!workspace || workspace_bytes < cbg_ipa_workspace_bytes(n_nodes, hidden)) { cbg_set_error("workspace too small"); return 1; }
   if (((uintptr_t)workspace & 255) != 0) { cbg_set_error("workspace must be 256-byte aligned"); return 1; }
   if (num_blocks < 1 || num_sublayers < 0) { cbg_set_error("num_blocks / num_sublayers"); return 1; }
-  cudaStream_t st = (cudaStream_t)stream;
-  if (hidden == 128)
-    return ipa_forward_t<128>(blob, num_sublayers, num_blocks, num_classes, x, o, h, graph_ptr, n_graphs, max_graph_nodes,
-                              lig_flag, gen_flag, (int)n_nodes, k, eps_pos, h_out, o_next, r_next, logits, (char*)workspace, st);
-  return ipa_forward_t<256>(blob, num_sublayers, num_blocks, num_classes, x, o, h, graph_ptr, n_graphs, max_graph_nodes,
-                            lig_flag, gen_flag, (int)n_nodes, k, eps_pos, h_out, o_next, r_next, logits, (char*)workspace, st);
+  return cbg_ipa_launch(blob, hidden, num_sublayers, num_blocks, num_classes, x, o, h, graph_ptr, n_graphs, max_graph_nodes,
+                        lig_flag, gen_flag, (int)n_nodes, k, eps_pos, h_out, o_next, r_next, logits, (char*)workspace,
+                        (cudaStream_t)stream);
 }
 
 }  // extern "C"

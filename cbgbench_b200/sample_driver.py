@@ -16,6 +16,8 @@ coordinates / types (``cbgbench_b200.sharding``).
         --pockets 2 --num-samples 100 --batch-size 50      (row f3: batches built on the GPU from raw pockets,
                                                             sample.py:177-183: num_samples per pocket, batch_size per step)
     python -m cbgbench_b200.sample_driver --model diffsbdd --pockets 16      (row f2: also diffbp)
+    python -m cbgbench_b200.sample_driver --model difffg --pockets 16 --n-prot 100 --n-lig 12
+                                        (D3FG: --n-prot residues and --n-lig functional groups per pocket, one GPU)
     torchrun --nproc-per-node 8 -m cbgbench_b200.sample_driver --pockets 512 --batch-size 512
 """
 import argparse
@@ -28,10 +30,12 @@ from . import sharding, synthetic
 from .targetdiff import TargetDiffB200
 from .diffsbdd import DiffSBDDB200
 from .diffbp import DiffBPB200
+from .difffg import D3FGB200
 
 MODELS = {'targetdiff': (TargetDiffB200, synthetic.targetdiff_config),
           'diffsbdd': (DiffSBDDB200, synthetic.diffsbdd_config),
-          'diffbp': (DiffBPB200, synthetic.diffbp_config)}
+          'diffbp': (DiffBPB200, synthetic.diffbp_config),
+          'difffg': (D3FGB200, synthetic.difffg_config)}
 
 
 def split_batch_into_samples(x, v, graph_id, n_graphs):
@@ -41,6 +45,33 @@ def split_batch_into_samples(x, v, graph_id, n_graphs):
         m = graph_id == g
         out.append({'pos': x[m].cpu(), 'v': v[m].cpu()})
     return out
+
+
+def split_batch_into_samples_fg(xc, c, o, graph_id, n_graphs):
+    """Per-pocket D3FG results (sample.py:34-47, no translation: d3fg_fg.yml sets translate false): list of dicts
+    {pos_center [n,3], fg_type [n], orientation [n,3]}."""
+    out = []
+    for g in range(n_graphs):
+        m = graph_id == g
+        out.append({'pos_center': xc[m].cpu(), 'fg_type': c[m].argmax(-1).cpu(), 'orientation': o[m].cpu()})
+    return out
+
+
+def run_difffg(args, model, distributed):
+    if distributed:
+        raise SystemExit('sample_driver --model difffg runs on one GPU: D3FG pockets are not sharded over ranks')
+    results, t0 = [], time.time()
+    for b0 in range(0, args.pockets, args.batch_size):
+        nb = min(args.batch_size, args.pockets - b0)
+        batch = synthetic.make_fg_batch([args.n_prot] * nb, [args.n_lig] * nb, seed=args.seed + b0)
+        xc, c, o, gid = model.sample(batch, traj_mode='final')[0]
+        results.extend(split_batch_into_samples_fg(xc, c, o, gid, nb))
+    torch.cuda.synchronize()
+    dt = time.time() - t0
+    if args.out:
+        torch.save(results, args.out)
+    print(f'sampled {len(results)} FG sets in {dt:.2f} s ({len(results) / dt:.2f} pockets/s, {args.steps} steps)')
+    return results
 
 
 def final_state(model, sub_batch, traj_key=0):
@@ -97,6 +128,8 @@ def run(args):
         model.load_state_dict(synthetic.seeded_state_dict(model, seed=0), strict=True)
     model = model.to(dev).eval()
     torch.manual_seed(args.seed + rank)                                                    # sample.py:106,131-133
+    if args.model == 'difffg':
+        return run_difffg(args, model, distributed)
 
     if args.builder == 'device':
         batches = device_built_batches(args, dev)

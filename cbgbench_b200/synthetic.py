@@ -160,17 +160,18 @@ def make_noise(num_steps, n_lig, num_classes, seed=7):
     return pn, tu
 
 
-def seeded_state_dict(model, seed=0, skip_prefixes=('pos_scheduler.', 'type_scheduler.')):
+def seeded_state_dict(model, seed=0, skip_prefixes=('pos_scheduler.', 'type_scheduler.', 'rot_scheduler.')):
     """Deterministic weights for every learnable tensor of ``model`` (state-dict order):
     matrices ~ U(-1/sqrt(fan_in), 1/sqrt(fan_in)) (nn.Linear default scale), LayerNorm gains
     ~ N(1, 0.2^2), biases / LayerNorm shifts ~ N(0, 0.2^2) so that no affine term is trivial.
     The H2X value heads (xv_func.net.3) are scaled by 0.1 so random-weight coordinate updates stay
-    of trained-model magnitude.  Buffers (``offset``) and schedule tables are left alone."""
+    of trained-model magnitude.  Buffers (``offset``, ``freq_bands``) and schedule tables (including D3FG's angular
+    histograms under ``rot_scheduler.``) are left alone."""
     rs = np.random.RandomState(seed)
     sd = model.state_dict()
     out = {}
     for name, t in sd.items():
-        if name.startswith(tuple(skip_prefixes)) or name.endswith('.offset'):
+        if name.startswith(tuple(skip_prefixes)) or name.endswith(('.offset', '.freq_bands')):
             out[name] = t.clone()
             continue
         shape = tuple(t.shape)
@@ -228,3 +229,91 @@ def make_ipa_inputs(hidden, n_nodes, n_lig, seed, gen_mode='denovo'):
         gens.append(gen)
     cat = lambda a, dt: torch.from_numpy(np.concatenate(a, 0).astype(dt))
     return (cat(xs, np.float32), cat(os_, np.float32), cat(hs, np.float32), cat(bs, np.int64), cat(ligs, bool), cat(gens, bool))
+
+
+# ---- D3FG (difffg): functional-group pockets --------------------------------------------------------------------------
+NUM_FG_TYPES = 28          # fg_only mode (repo/utils/configuration.py:10)
+
+
+def difffg_config(num_steps=1000, num_layers=9, hidden=256, num_fgtype=NUM_FG_TYPES):
+    """configs/denovo/train/d3fg_fg.yml:1-27 (+ num_fgtype; the encoder spelled the way the reference's factory accepts)."""
+    return Cfg(dict(
+        type='difffg', num_fgtype=num_fgtype,
+        encoder=dict(type='ipatransformer', node_feat_dim=hidden, n_heads=16, num_layers=num_layers),
+        generator=dict(pos_schedule=dict(type='sigmoid', beta_start=1.e-7, beta_end=2.e-3),
+                       rot_schedule=dict(type='cosine', cosine_s=0.01), fg_schedule=dict(type='cosine', cosine_s=0.01),
+                       num_diffusion_timesteps=num_steps, time_sampler='symmetric'),
+        embedder=dict(type='fg', emb_dim=hidden, fg=dict(type='linear'), residue=dict(type='frame'))))
+
+
+def make_fg_batch(n_res, n_fg, seed=2024, num_fgtype=NUM_FG_TYPES, partial_graphs=()):
+    """Flat ragged FG batch with the reference's keys (difffg.py:174-195).  Synthetic, not taken from data: per graph a
+    C-alpha chain (3.8 A steps) split into up to three chains with residue-number gaps, N / C placed off the C-alpha at
+    non-degenerate angles, side-chain atoms around C-alpha with random atom masks (C-alpha masked in a few residues),
+    amino acids U{0..19}, protein FG types 28 + aa, FG centres ~ N(0, 2^2) around the pocket centre, FG types
+    U{0..num_fgtype-1}, orientations ~ N(0, 0.8^2) so3 vectors.  Graphs listed in ``partial_graphs`` generate only the
+    second half of their functional groups."""
+    rs = np.random.RandomState(seed)
+    keys = {k: [] for k in ('ppos', 'pmask', 'aa', 'ptype', 'res_nb', 'chain_nb', 'pb', 'nch', 'lpos', 'ltype', 'lo',
+                            'lb', 'gen')}
+    for g, (nr, nl) in enumerate(zip(n_res, n_fg)):
+        steps = rs.normal(size=(nr, 3))
+        steps = 3.8 * steps / np.linalg.norm(steps, axis=1, keepdims=True)
+        ca = np.cumsum(steps, 0)
+        ca = ca - ca.mean(0)
+        pos = ca[:, None, :] + rs.normal(0.0, 1.5, size=(nr, 15, 3))
+        u = rs.normal(size=(nr, 3))
+        u /= np.linalg.norm(u, axis=1, keepdims=True)
+        w = rs.normal(size=(nr, 3))
+        w -= (w * u).sum(1, keepdims=True) * u
+        w /= np.linalg.norm(w, axis=1, keepdims=True)
+        pos[:, 1] = ca
+        pos[:, 2] = ca + 1.52 * u                                       # C
+        pos[:, 0] = ca + 1.46 * (np.cos(1.94) * u + np.sin(1.94) * w)   # N at the tetrahedral-ish angle
+        mask = rs.random_sample(size=(nr, 15)) < 0.6
+        mask[:, :4] = True
+        mask[rs.random_sample(nr) < 0.05, 1] = False
+        n_ch = int(rs.randint(1, 4)) if nr >= 6 else 1
+        cuts = np.sort(rs.choice(np.arange(1, nr), size=n_ch - 1, replace=False)) if n_ch > 1 else np.zeros(0, int)
+        chain = np.zeros(nr, dtype=np.int64)
+        for c in cuts:
+            chain[c:] += 1
+        res = np.cumsum(1 + (rs.random_sample(nr) < 0.1).astype(np.int64) * rs.randint(1, 5, size=nr)) + 10
+        aa = rs.randint(0, 20, size=nr)
+        keys['ppos'].append(pos); keys['pmask'].append(mask); keys['aa'].append(aa); keys['ptype'].append(num_fgtype + aa)
+        keys['res_nb'].append(res); keys['chain_nb'].append(chain); keys['pb'].append(np.full(nr, g))
+        keys['nch'].append([n_ch])
+        lpos = np.zeros((nl, 15, 3))
+        lpos[:, 1] = rs.normal(0.0, 2.0, size=(nl, 3))
+        keys['lpos'].append(lpos); keys['ltype'].append(rs.randint(0, num_fgtype, size=nl))
+        keys['lo'].append(rs.normal(0.0, 0.8, size=(nl, 3))); keys['lb'].append(np.full(nl, g))
+        gen = np.ones(nl, dtype=bool)
+        if g in partial_graphs:
+            gen[: nl // 2] = False
+        keys['gen'].append(gen)
+    cat = lambda k, dt: torch.from_numpy(np.concatenate(keys[k], 0).astype(dt))
+    n_l = int(sum(n_fg))
+    batch = {
+        'protein_pos_heavyatom': cat('ppos', np.float32), 'protein_mask_heavyatom': cat('pmask', np.bool_),
+        'protein_aa': cat('aa', np.int64), 'protein_type_fg': cat('ptype', np.int64),
+        'protein_res_nb': cat('res_nb', np.int64), 'protein_chain_nb': cat('chain_nb', np.int64),
+        'protein_num_chains': cat('nch', np.int64), 'protein_type_fg_batch': cat('pb', np.int64),
+        'protein_lig_flag': torch.zeros(int(sum(n_res)), dtype=torch.bool),
+        'ligand_pos_heavyatom': cat('lpos', np.float32), 'ligand_type_fg': cat('ltype', np.int64),
+        'ligand_o_fg': cat('lo', np.float32), 'ligand_type_fg_batch': cat('lb', np.int64),
+        'ligand_lig_flag': torch.ones(n_l, dtype=torch.bool),
+    }
+    if partial_graphs:
+        batch['ligand_gen_flag'] = cat('gen', np.bool_)
+    return batch
+
+
+def make_fg_draws(num_steps, n_fg, num_fgtype=NUM_FG_TYPES, seed=7):
+    """Injected draws of one D3FG.sample call, indexed by t: positions N(0,1) [T,n,3]; rotations [T,n,6] = axis N(0,1)^3 |
+    bin uniform | in-bin uniform | Gaussian-branch N(0,1); Gumbel uniforms [T,n,K]."""
+    rs = np.random.RandomState(seed)
+    f = lambda a: torch.from_numpy(a.astype(np.float32))
+    pos = f(rs.normal(size=(num_steps, n_fg, 3)))
+    rot = np.concatenate([rs.normal(size=(num_steps, n_fg, 3)), rs.random_sample(size=(num_steps, n_fg, 2)),
+                          rs.normal(size=(num_steps, n_fg, 1))], axis=2)
+    return pos, f(rot), f(rs.random_sample(size=(num_steps, n_fg, num_fgtype)))

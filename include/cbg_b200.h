@@ -471,6 +471,51 @@ int32_t cbg_ipa_forward_f32(const float* blob, int32_t hidden, int32_t num_subla
                             int32_t k, float* eps_pos, float* h_out, float* o_next, float* r_next, float* logits,
                             void* workspace, int64_t workspace_bytes, void* stream);
 
+/* ---- D3FG sampling (`difffg` / `difffg_v2`, repo/models/diffusion/difffg.py:174-246): one reverse step per call -------
+ * Composed node arrays [protein | ligand per graph] live in the plan; the protein rows (x = C-alpha, o = backbone frame,
+ * h = FG + residue embedding) are written once per batch by the host.  A step writes the ligand rows from the state
+ * (fg_embed_kernel), runs the IPATransformer (cbg_ipa_launch) and applies the position / SO(3) / FG-type reverse updates
+ * (fg_reverse_kernel, one warp per functional group) into the next state. */
+typedef struct {
+  const float* blob;              /* IPATransformer blob (cbg_ipa_*) */
+  int32_t hidden, num_sublayers, num_blocks, num_classes, k;
+  const int32_t* graph_ptr;       /* [n_graphs+1] composed rows per graph */
+  int32_t n_graphs, max_graph_nodes;
+  int64_t n_nodes;
+  const uint8_t* lig_flag;        /* [N] composed order */
+  const uint8_t* gen_flag;        /* [N] composed order */
+  const int32_t* lig_node;        /* [n_lig] composed row of ligand row a */
+  const uint8_t* gen_lig;         /* [n_lig] */
+  int32_t n_lig;
+  float* x;                       /* [N,3] composed positions */
+  float* o;                       /* [N,3] composed so3 vectors */
+  float* h;                       /* [N,hidden] composed node features */
+  const float* fg_emb_t;          /* [num_classes,hidden] columns of ligand_fg_emb.weight */
+  const float* fg_emb_b;          /* [hidden] ligand_fg_emb.bias */
+  const float* lig_indicator;     /* [hidden] ligand_indicator(1) */
+  const float* angle_x;           /* [T,n_bins] angular_distrib_inv.X */
+  const double* angle_cdf;        /* [T,n_bins-1] inclusive float64 prefix sums of angular_distrib_inv.Y[:, :-1] */
+  int32_t n_bins;
+  void* workspace;
+  int64_t workspace_bytes;
+} cbg_fg_plan;
+
+typedef struct {
+  int32_t t;
+  float pos_beta, pos_sigma, pos_sqrt_one_minus_beta, pos_noise_scale;  /* b, sqrt(1 - abar), sqrt(1 - b), [t != 0] sqrt(b) */
+  float rot_std;                  /* angular_distrib_inv.stddevs[t] */
+  int32_t rot_gaussian;           /* angular_distrib_inv.approx_flag[t] */
+  int32_t rot_noise;              /* t > 1 */
+  float log_alphas_cumprod_prev, log_one_minus_alphas_cumprod_prev, log_alpha, log_one_minus_alpha;
+} cbg_fg_coef;
+
+int64_t cbg_fg_workspace_bytes(int64_t n_nodes, int32_t hidden, int32_t num_classes);
+/* x_t / c_t / o_t [n_lig,3|K|3] -> x_next / c_next / o_next; draws: pos_noise [n_lig,3] N(0,1), rot_draws [n_lig,6] =
+ * axis N(0,1)^3 | bin uniform | in-bin uniform | Gaussian-branch N(0,1), type_u [n_lig,K] U[0,1) */
+int32_t cbg_fg_step_f32(const cbg_fg_plan* plan, cbg_fg_coef coef, const float* x_t, const float* c_t, const float* o_t,
+                        const float* pos_noise, const float* rot_draws, const float* type_u, float* x_next, float* c_next,
+                        float* o_next, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
