@@ -146,6 +146,7 @@ SIGNATURES = {
                                    _P, _P, _P, _P, _P, _P, _I64, _P]),
     'cbg_fg_workspace_bytes': (_I64, [_I64, _I32, _I32]),
     'cbg_fg_step_f32': (_I32, [C.POINTER(FgPlan), FgCoef, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
+    'cbg_fg_reverse_f32': (_I32, [C.POINTER(FgPlan), FgCoef] + [_P] * 14),
     'cbg_reverse_step_f32': (_I32, [C.POINTER(StepCoef), _P, _P, _P, _P, _P, _P, _P, _I32, _I32, _P, _P, _P, _P]),
 }
 

@@ -350,12 +350,29 @@ __device__ __forceinline__ void so3vec_to_rotation(float wx, float wy, float wz,
 #pragma unroll
   for (int e = 0; e < 9; ++e) R[e] = ((e % 4 == 0) ? 1.f : 0.f) + bb * S[e] + cb * S2[e];
 }
-// w = skewsym_to_so3vec(log_rotation(R))   so3.py:10-31, 60-63 (no-grad branch: cos clamped at -1)
+// w = skewsym_to_so3vec(log_rotation(R))   so3.py:10-31, 60-63, reformulated so that it is finite for every angle and
+// exp(w) = R to fp32 accuracy on all of [0, pi] (DESIGN.md section 16).  The reference's acos((tr - 1) / 2) / (2 sin)
+// is NaN when rounding puts the trace above 3, and its sqrt(1 - cos^2) loses the angle quadratically near pi.
+// Here c = clamp((tr - 1) / 2, -1, 1), v = the skew vector of R = sin(theta) n, theta = atan2(|v|, c).  For c >= 0
+// w = (theta / |v|) v (ratio 1 as |v| -> 0); for c < 0 the axis comes from the symmetric part
+// (R + R^T) / 2 - c I = (1 - c) n n^T (the row of the largest diagonal entry), signed by v, and w = theta n.
 __device__ __forceinline__ void rotation_to_so3vec(const float* R, float* w) {
-  const float tr = R[0] + R[4] + R[8];
-  const float cos_t = fmaxf((tr - 1.f) * 0.5f, -1.f);
-  const float sin_t = sqrtf(1.f - cos_t * cos_t);
-  const float theta = acosf(cos_t);
-  const float coef = (theta + 1e-8f) / (2.f * sin_t + 2e-8f);
-  w[0] = coef * (R[5] - R[7]); w[1] = coef * (R[6] - R[2]); w[2] = coef * (R[1] - R[3]);
+  const float c = fminf(fmaxf((R[0] + R[4] + R[8] - 1.f) * 0.5f, -1.f), 1.f);
+  const float v[3] = {0.5f * (R[5] - R[7]), 0.5f * (R[6] - R[2]), 0.5f * (R[1] - R[3])};
+  const float s = norm3df(v[0], v[1], v[2]);
+  const float theta = atan2f(s, c);
+  if (c >= 0.f) {
+    const float k = s > 0.f ? theta / s : 1.f;
+#pragma unroll
+    for (int e = 0; e < 3; ++e) w[e] = k * v[e];
+    return;
+  }
+  const int j = (R[0] >= R[4] && R[0] >= R[8]) ? 0 : (R[4] >= R[8] ? 1 : 2);
+  float n[3];
+#pragma unroll
+  for (int e = 0; e < 3; ++e) n[e] = (e == j) ? R[4 * j] - c : 0.5f * (R[3 * j + e] + R[3 * e + j]);
+  const float rn = norm3df(n[0], n[1], n[2]);          // >= (1 - c) / sqrt(3) > 0.57
+  const float sg = (n[0] * v[0] + n[1] * v[1] + n[2] * v[2]) < 0.f ? -theta : theta;
+#pragma unroll
+  for (int e = 0; e < 3; ++e) w[e] = sg * (n[e] / rn);
 }

@@ -69,7 +69,8 @@ __global__ void __launch_bounds__(256) fg_reverse_kernel(cbg_fg_plan p, cbg_fg_c
                                                          const float* __restrict__ o_t, const float* __restrict__ pos_noise,
                                                          const float* __restrict__ rot_draws,
                                                          const float* __restrict__ type_u, float* __restrict__ x_next,
-                                                         float* __restrict__ c_next, float* __restrict__ o_next) {
+                                                         float* __restrict__ c_next, float* __restrict__ o_next,
+                                                         float* __restrict__ theta_out) {
   const int a = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
   if (a >= p.n_lig) return;
   const int K = p.num_classes;
@@ -89,8 +90,8 @@ __global__ void __launch_bounds__(256) fg_reverse_kernel(cbg_fg_plan p, cbg_fg_c
   if (lane == 0) {
     const float* rd = rot_draws + (size_t)a * 6;
     float e[3] = {0.f, 0.f, 0.f};
+    float theta = 0.f;
     if (cf.rot_noise) {
-      float theta;
       if (cf.rot_gaussian) {        // |2 sigma + sigma n| mod pi
         theta = fmodf(fabsf(__fadd_rn(cf.rot_std * 2.f, __fmul_rn(rd[5], cf.rot_std))), 3.14159265358979323846f);
       } else {                      // bin b = min{i : C_t[i] > u C_t[n_bins - 2]}, then X[b] + u' (X[b+1] - X[b])
@@ -105,7 +106,8 @@ __global__ void __launch_bounds__(256) fg_reverse_kernel(cbg_fg_plan p, cbg_fg_c
         const float* X = p.angle_x + (size_t)cf.t * p.n_bins;
         theta = __fadd_rn(X[lo], __fmul_rn(rd[4], __fsub_rn(X[lo + 1], X[lo])));
       }
-      const float nrm = fmaxf(sqrtf(rd[0] * rd[0] + rd[1] * rd[1] + rd[2] * rd[2]), 1e-12f);
+      // F.normalize: a / max(|a|, 1e-12); norm3df does not overflow for |a| up to FLT_MAX (axis draws of 1e30)
+      const float nrm = fmaxf(norm3df(rd[0], rd[1], rd[2]), 1e-12f);
 #pragma unroll
       for (int c = 0; c < 3; ++c) e[c] = __fmul_rn(__fdiv_rn(rd[c], nrm), theta);
     }
@@ -116,6 +118,7 @@ __global__ void __launch_bounds__(256) fg_reverse_kernel(cbg_fg_plan p, cbg_fg_c
     rotation_to_so3vec(Rn, w);
 #pragma unroll
     for (int c = 0; c < 3; ++c) o_next[3 * a + c] = gen ? w[c] : o_t[3 * a + c];
+    if (theta_out) theta_out[a] = theta;
   }
 
   // FG type: q(v_{t-1} | v_t, softmax(logits)), Gumbel-max draw; lane k = class k
@@ -201,9 +204,41 @@ int32_t cbg_fg_step_f32(const cbg_fg_plan* plan, cbg_fg_coef coef, const float* 
   if (grid > 0) {
     CBG_PROF_BEGIN(CBG_K_REVERSE, st);
     fg_reverse_kernel<<<grid, 256, 0, st>>>(p, coef, FgOut{eps_pos, o_pred, logits}, x_t, c_t, o_t, pos_noise, rot_draws,
-                                            type_u, x_next, c_next, o_next);
+                                            type_u, x_next, c_next, o_next, nullptr);
     CBG_LAUNCHED(CBG_K_REVERSE, st);
   }
+  return 0;
+}
+
+int32_t cbg_fg_reverse_f32(const cbg_fg_plan* plan, cbg_fg_coef coef, const float* eps_pos, const float* o_pred,
+                           const float* logits, const float* x_t, const float* c_t, const float* o_t, const float* pos_noise,
+                           const float* rot_draws, const float* type_u, float* x_next, float* c_next, float* o_next,
+                           float* theta, void* stream) {
+  if (!plan) { cbg_set_error("cbg_fg_reverse_f32: plan is NULL"); return 1; }
+  const cbg_fg_plan& p = *plan;
+  if (p.num_classes < 1 || p.num_classes > CBG_IPA_MAXCLS) {
+    cbg_set_error("cbg_fg_reverse_f32: num_classes=%d outside [1,%d]", p.num_classes, CBG_IPA_MAXCLS);
+    return 1;
+  }
+  if (p.n_lig < 0 || p.n_bins < 2 || coef.t < 0) {
+    cbg_set_error("cbg_fg_reverse_f32: n_lig=%d n_bins=%d t=%d", p.n_lig, p.n_bins, coef.t);
+    return 1;
+  }
+  if (p.n_lig == 0) return 0;
+  if (!p.lig_node || !p.gen_lig || !p.angle_x || !p.angle_cdf) {
+    cbg_set_error("cbg_fg_reverse_f32: NULL lig_node / gen_lig / angle_x / angle_cdf in the plan");
+    return 1;
+  }
+  if (!eps_pos || !o_pred || !logits || !x_t || !c_t || !o_t || !pos_noise || !rot_draws || !type_u || !x_next ||
+      !c_next || !o_next) {
+    cbg_set_error("cbg_fg_reverse_f32: NULL row, state or draw pointer");
+    return 1;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  CBG_PROF_BEGIN(CBG_K_REVERSE, st);
+  fg_reverse_kernel<<<(p.n_lig + 7) / 8, 256, 0, st>>>(p, coef, FgOut{eps_pos, o_pred, logits}, x_t, c_t, o_t, pos_noise,
+                                                      rot_draws, type_u, x_next, c_next, o_next, theta);
+  CBG_LAUNCHED(CBG_K_REVERSE, st);
   return 0;
 }
 

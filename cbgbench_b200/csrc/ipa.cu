@@ -445,6 +445,7 @@ int32_t cbg_ipa_forward_f32(const float* blob, int32_t hidden, int32_t num_subla
   if (!workspace || workspace_bytes < cbg_ipa_workspace_bytes(n_nodes, hidden)) { cbg_set_error("workspace too small"); return 1; }
   if (((uintptr_t)workspace & 255) != 0) { cbg_set_error("workspace must be 256-byte aligned"); return 1; }
   if (num_blocks < 1 || num_sublayers < 0) { cbg_set_error("num_blocks / num_sublayers"); return 1; }
+  if (k < 1 || k > CBG_KMAX) { cbg_set_error("cbg_ipa_forward_f32: k=%d outside [1,%d]", k, CBG_KMAX); return 1; }
   return cbg_ipa_launch(blob, hidden, num_sublayers, num_blocks, num_classes, x, o, h, graph_ptr, n_graphs, max_graph_nodes,
                         lig_flag, gen_flag, (int)n_nodes, k, eps_pos, h_out, o_next, r_next, logits, (char*)workspace,
                         (cudaStream_t)stream);

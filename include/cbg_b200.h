@@ -516,6 +516,15 @@ int32_t cbg_fg_step_f32(const cbg_fg_plan* plan, cbg_fg_coef coef, const float* 
                         const float* pos_noise, const float* rot_draws, const float* type_u, float* x_next, float* c_next,
                         float* o_next, void* stream);
 
+/* The reverse update alone (testing hook): fg_reverse_kernel on caller-given encoder rows.  eps_pos / o_pred / logits are
+ * composed rows [*,3|3|K], read at lig_node[a]; the state and the draws are as for cbg_fg_step_f32.  Of the plan only
+ * n_lig, num_classes, lig_node, gen_lig, angle_x, angle_cdf and n_bins are read.  theta [n_lig] (or NULL) receives the
+ * drawn rotation angle (0 when coef.rot_noise is 0). */
+int32_t cbg_fg_reverse_f32(const cbg_fg_plan* plan, cbg_fg_coef coef, const float* eps_pos, const float* o_pred,
+                           const float* logits, const float* x_t, const float* c_t, const float* o_t,
+                           const float* pos_noise, const float* rot_draws, const float* type_u, float* x_next,
+                           float* c_next, float* o_next, float* theta, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

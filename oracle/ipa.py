@@ -32,7 +32,7 @@ def x2h_attention(sd, lp, x, h, src, dst, etype, e_w):
     dist = torch.norm(rel, p=2, dim=-1, keepdim=True)
     g = gaussian_smearing(dist, sd[lp + 'distance_expansion.offset'])
     onehot = F.one_hot(etype, 4).to(x.dtype)
-    r_feat = (onehot[:, :, None] * g[:, None, :]).reshape(len(src), -1)
+    r_feat = (onehot[:, :, None] * g[:, None, :]).reshape(len(src), 4 * g.shape[-1])   # explicit width: E may be 0
     kv = torch.cat([onehot, r_feat, h[dst], h[src]], dim=-1)
     k = mlp(sd, lp + 'hk_func.', kv).view(-1, N_HEADS, H // N_HEADS)
     v = (mlp(sd, lp + 'hv_func.', kv) * e_w).view(-1, N_HEADS, H // N_HEADS)
@@ -80,14 +80,18 @@ def seq3(sd, p, x):
     return F.linear(y, sd[p + '4.weight'], sd[p + '4.bias'])
 
 
-def ipatransformer_forward(sd, x, o, h, batch_idx, lig_flag, gen_flag, prefix='', k=32, num_blocks=1):
-    """itatransformer.py:115-145 -> (eps_pos, h, o_next, R_next, c)."""
+def ipatransformer_forward(sd, x, o, h, batch_idx, lig_flag, gen_flag, prefix='', k=32, num_blocks=1, nbr=None):
+    """itatransformer.py:115-145 -> (eps_pos, h, o_next, R_next, c).
+
+    Runs in the dtype of ``x`` / ``h`` / ``sd``.  ``nbr``: a precomputed neighbour table (G.neighbor_table) instead of the
+    kNN of ``x``, so that a float64 pass sees exactly the graph of an fp32 one (no tie flips)."""
     ptr = G.graph_ptr_from_batch(batch_idx)
     n_layers = 0
     while (prefix + f'blocks.{n_layers}.x2h_layers.0.hk_func.net.0.weight') in sd:
         n_layers += 1
+    table = nbr
     for _ in range(num_blocks):
-        nbr = G.neighbor_table(x, ptr, k=k, r_max=None)
+        nbr = G.neighbor_table(x, ptr, k=k, r_max=None) if table is None else table
         src, dst = G.table_to_edge_index(nbr)
         etype = build_edge_type(src, dst, lig_flag.bool())
         e_w = edge_gate(sd, prefix, x, src, dst)

@@ -124,10 +124,6 @@ def sample(sd, batch, T, pos_noise, rot_draws, type_uniform, num_classes=28, num
     batch_ctx = torch.cat([br, bl])
     sort_idx = torch.sort(batch_ctx, stable=True).indices
     is_lig = torch.cat([rec_flag, lig_flag])[sort_idx]
-    pf = 'pos_scheduler.'
-    acp, betas = sd[pf + 'alphas_cumprod'], sd[pf + 'betas']
-    ts = 'type_scheduler.'
-    rot = 'rot_scheduler.angular_distrib_inv.'
     traj = {T - 1: (xc, c, o)}
     steps = list(reversed(range(T)))[:num_steps]
     for t_idx in steps:
@@ -141,38 +137,58 @@ def sample(sd, batch, T, pos_noise, rot_draws, type_uniform, num_classes=28, num
             sd, cat(xc_rec, xc_l), cat(o_rec, o_l.clone()), cat(h_rec, h_lig), batch_ctx[sort_idx], is_lig,
             cat(gen_rec, gen_lig), prefix='denoiser.')
         eps, o_pred, logits = eps[is_lig], o_pred[is_lig], logits[is_lig]
-        # positions: CTNVPScheduler.backward_remove_noise, type='score'
-        a = acp.index_select(0, t)[:, None][bl].expand_as(xc_l)
-        b = betas.index_select(0, t)[:, None][bl].expand_as(xc_l)
-        nonzero = (1 - (t == 0).float())[bl].unsqueeze(-1)
-        xs = (xc_l + b * (-eps / (1 - a).sqrt())) / (1 - b).sqrt()
-        xs = xs + nonzero * b.sqrt() * pos_noise[t_idx]
-        x_next = torch.where(gen_lig.unsqueeze(-1), xs, xc_l)
-        # orientation: RotVPScheduler.backward_remove_noise with ApproxAngularDistribution.sample
-        tt = t[bl]
-        rd = rot_draws[t_idx]
-        u = F.normalize(rd[:, 0:3], dim=-1)
-        X, Y, std = sd[rot + 'X'], sd[rot + 'Y'], sd[rot + 'stddevs']
-        b_idx = multinomial_bin(Y[tt][:, :-1], rd[:, 3])
+        x_next, v_next, o_next, _ = reverse_step(sd, t_idx, bl, xc_l, c_l, o_l, eps, o_pred, logits, gen_lig,
+                                                 pos_noise[t_idx], rot_draws[t_idx], type_uniform[t_idx])
+        traj[t_idx - 1] = (x_next, F.one_hot(v_next, K).float(), o_next)
+    return traj
+
+
+def reverse_step(sd, t_idx, bl, xc_l, c_l, o_l, eps, o_pred, logits, gen_lig, pos_noise, rd, type_u, theta=None):
+    """The position / SO(3) / FG-type update of one reverse step t_idx for the ligand rows, in the dtype of ``xc_l``
+    (fp32: the expressions of D3FG.sample; float64: a high-precision reference of the same step; the schedule tables
+    stay the fp32 values they hold).  ``theta``: use this rotation angle instead of drawing it (a float64 composition
+    with a given fp32 angle).  -> (x_next, v_next, o_next, (theta, bin, log_prob + gumbel))."""
+    dt = xc_l.dtype
+    K = c_l.shape[-1]
+    pf = 'pos_scheduler.'
+    ts = 'type_scheduler.'
+    rot = 'rot_scheduler.angular_distrib_inv.'
+    acp, betas = sd[pf + 'alphas_cumprod'].to(dt), sd[pf + 'betas'].to(dt)
+    eps, o_pred, logits, c_l = eps.to(dt), o_pred.to(dt), logits.to(dt), c_l.to(dt)
+    pos_noise, rd, type_u = pos_noise.to(dt), rd.to(dt), type_u.to(dt)
+    t = torch.full((int(bl.max()) + 1,), t_idx, dtype=torch.long)
+    # positions: CTNVPScheduler.backward_remove_noise, type='score'
+    a = acp.index_select(0, t)[:, None][bl].expand_as(xc_l)
+    b = betas.index_select(0, t)[:, None][bl].expand_as(xc_l)
+    nonzero = (1 - (t == 0).to(dt))[bl].unsqueeze(-1)
+    xs = (xc_l + b * (-eps / (1 - a).sqrt())) / (1 - b).sqrt()
+    xs = xs + nonzero * b.sqrt() * pos_noise
+    x_next = torch.where(gen_lig.unsqueeze(-1), xs, xc_l)
+    # orientation: RotVPScheduler.backward_remove_noise with ApproxAngularDistribution.sample
+    tt = t[bl]
+    u = F.normalize(rd[:, 0:3], dim=-1)
+    X, Y, std = sd[rot + 'X'].to(dt), sd[rot + 'Y'], sd[rot + 'stddevs'].to(dt)
+    b_idx = multinomial_bin(Y[tt][:, :-1], rd[:, 3])
+    if theta is None:
         start = X[tt, b_idx]
         s_hist = start + rd[:, 4] * (X[tt, b_idx + 1] - start)
         s_gauss = (std[tt] * 2 + rd[:, 5] * std[tt]).abs() % math.pi
         theta = torch.where(sd[rot + 'approx_flag'][tt], s_gauss, s_hist)
-        e = u * theta[:, None]
-        e = torch.where((tt > 1)[:, None].expand(-1, 3), e, torch.zeros_like(e))
-        R_next = so3vec_to_rotation(e) @ so3vec_to_rotation(o_pred)
-        o_next = torch.where(gen_lig[:, None].expand(-1, 3), rotation_to_so3vec(R_next), o_l)
-        # FG type: TypeVPScheduler.backward_remove_noise
-        tm1 = torch.clamp(t - 1, min=0)
-        lv = lambda name, tt_: sd[ts + name][tt_][bl].unsqueeze(-1)
-        lae = lambda p_, q_: torch.max(p_, q_) + torch.log(torch.exp(p_ - torch.max(p_, q_)) + torch.exp(q_ - torch.max(p_, q_)))
-        log_pred = F.log_softmax(logits, dim=-1)
-        log_ct = torch.log(c_l + 1e-8)
-        A = lae(log_pred + lv('log_alphas_cumprod_v', tm1), lv('log_one_minus_alphas_cumprod_v', tm1) - math.log(K))
-        B_ = lae(log_ct + lv('log_alphas_v', t), lv('log_one_minus_alphas_v', t) - math.log(K))
-        un = A + B_
-        log_prob = un - torch.logsumexp(un, dim=-1, keepdim=True)
-        gumbel = -torch.log(-torch.log(type_uniform[t_idx] + 1e-30) + 1e-30)
-        v_next = torch.where(gen_lig, (gumbel + log_prob).argmax(-1), c_l.argmax(-1))
-        traj[t_idx - 1] = (x_next, F.one_hot(v_next, K).float(), o_next)
-    return traj
+    e = u * theta.to(dt)[:, None]
+    e = torch.where((tt > 1)[:, None].expand(-1, 3), e, torch.zeros_like(e))
+    R_next = so3vec_to_rotation(e) @ so3vec_to_rotation(o_pred)
+    o_next = torch.where(gen_lig[:, None].expand(-1, 3), rotation_to_so3vec(R_next), o_l)
+    # FG type: TypeVPScheduler.backward_remove_noise
+    tm1 = torch.clamp(t - 1, min=0)
+    lv = lambda name, tt_: sd[ts + name].to(dt)[tt_][bl].unsqueeze(-1)
+    lae = lambda p_, q_: torch.max(p_, q_) + torch.log(torch.exp(p_ - torch.max(p_, q_)) + torch.exp(q_ - torch.max(p_, q_)))
+    log_pred = F.log_softmax(logits, dim=-1)
+    log_ct = torch.log(c_l + 1e-8)
+    A = lae(log_pred + lv('log_alphas_cumprod_v', tm1), lv('log_one_minus_alphas_cumprod_v', tm1) - math.log(K))
+    B_ = lae(log_ct + lv('log_alphas_v', t), lv('log_one_minus_alphas_v', t) - math.log(K))
+    un = A + B_
+    log_prob = un - torch.logsumexp(un, dim=-1, keepdim=True)
+    gumbel = -torch.log(-torch.log(type_u + 1e-30) + 1e-30)
+    score = gumbel + log_prob
+    v_next = torch.where(gen_lig, score.argmax(-1), c_l.argmax(-1))
+    return x_next, v_next, o_next, (theta, b_idx, score)

@@ -129,8 +129,9 @@ def _rot_agree(a, b, tol):
 
 
 def _near_pi(o, tol=1e-2):
-    """Rows whose rotation angle is within ``tol`` of pi: there the log map that stores o (so3.py:10-22) is
-    ill-conditioned, so fp32 rounding differences grow by orders of magnitude and carry into later steps."""
+    """Rows whose rotation angle is within ``tol`` of pi: there the reference's fp32 log map (so3.py:10-22), which the
+    golden trajectory and the oracle use, is ill-conditioned, so its rounding errors grow by orders of magnitude and
+    carry into later steps (the kernels' log map is exact there: tests/test_fg_kernels.py)."""
     return torch.linalg.norm(o.double(), dim=-1) > np.pi - tol
 
 
