@@ -375,6 +375,21 @@ int check_replicas(const cbg_sample_plan& p, int n_t, int copies = 1) {
   return 0;
 }
 
+// Prologue of the validation-loss entry points: open_plan, check_replicas, the batch block of the kernels' arguments and
+// h reset to h_static (the noise kernel then writes the ligand rows).  Checks an entry point makes after it leave only
+// that reset behind when they fail.
+int open_eval(const cbg_sample_plan* plan, bool args_ok, const char* null_msg, int n_t, int copies, const float* x0,
+              const int64_t* v0, Workspace* ws, EvalBatch* b, cudaStream_t st) {
+  if (int rc = open_plan(plan, args_ok, null_msg, ws)) return rc;
+  if (int rc = check_replicas(*plan, n_t, copies)) return rc;
+  b->n_lig = plan->n_lig; b->n_graphs = plan->n_graphs; b->num_classes = plan->num_classes;
+  b->lig_node = plan->lig_node; b->graph_ptr = plan->graph_ptr; b->gen = plan->gen_lig;
+  b->x0 = x0; b->v0 = (const long long*)v0; b->emb_wt = plan->emb_wt; b->h_lig_bias = plan->h_lig_bias;
+  b->x4 = ws->x4; b->h = ws->h;
+  CBG_CUDA_OK(cudaMemcpyAsync(ws->h, plan->h_static, (size_t)plan->n_nodes * CBG_H * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  return 0;
+}
+
 // cached device scratch for the *_host entry points: one per DEVICE (the buffers belong to the device that was current
 // when they were allocated); the weight blob is re-uploaded whenever the caller's (version, size, host pointer) changes -
 // the version is a process-unique id handed out by the Python side, so two models never alias
@@ -852,27 +867,20 @@ int32_t cbg_bp_eval_loss_f32(const cbg_sample_plan* plan, const float* com_blob,
                              const cbg_bp_eval_coef* coefs, int32_t n_rep, const float* x0, const int64_t* v0,
                              const float* pos_noise, const float* type_uniform, float* xt, int64_t* vt, uint8_t* mask,
                              float* vec, float* c_pred, float* rep_loss, void* stream) {
-  Workspace ws;
-  if (int rc = open_plan(plan, com_blob && coefs && x0 && v0 && pos_noise && type_uniform && xt && vt && mask && vec &&
-                         c_pred && rep_loss, "cbg_bp_eval_loss_f32: null argument", &ws)) return rc;
-  if (com_layers < 0 || com_layers > 16) { cbg_set_error("com_layers=%d outside [0,16]", com_layers); return 1; }
-  if (int rc = check_replicas(*plan, n_rep)) return rc;
   NvtxRange nvtx_eval("cbg:bp_eval_loss");
   cudaStream_t st = (cudaStream_t)stream;
-  const int K = plan->num_classes, n_lig = plan->n_lig;
+  Workspace ws;
   BpEvalArgs e{};
+  if (int rc = open_eval(plan, com_blob && coefs && x0 && v0 && pos_noise && type_uniform && xt && vt && mask && vec &&
+                         c_pred && rep_loss, "cbg_bp_eval_loss_f32: null argument", n_rep, 1, x0, v0, &ws, &e.b, st)) return rc;
+  if (com_layers < 0 || com_layers > 16) { cbg_set_error("com_layers=%d outside [0,16]", com_layers); return 1; }
   for (int r = 0; r < n_rep; ++r) e.coef.c[r] = BpEvalCoefDev{coefs[r].alphas_cumprod, coefs[r].beta, coefs[r].mask_prob};
-  e.n_rep = n_rep; e.n_lig = n_lig; e.n_graphs = plan->n_graphs; e.num_classes = K;
-  e.lig_node = plan->lig_node; e.graph_ptr = plan->graph_ptr; e.gen = plan->gen_lig;
-  e.x0 = x0; e.v0 = (const long long*)v0; e.pos_noise = pos_noise; e.type_u = type_uniform;
-  e.emb_wt = plan->emb_wt; e.h_lig_bias = plan->h_lig_bias;
-  e.x4 = ws.x4; e.h = ws.h; e.xt = xt; e.vt = (long long*)vt; e.mask = mask; e.vec = vec; e.c_pred = c_pred;
-  e.rep_loss = rep_loss;
+  e.n_rep = n_rep; e.pos_noise = pos_noise; e.type_u = type_uniform;
+  e.xt = xt; e.vt = (long long*)vt; e.mask = mask; e.vec = vec; e.c_pred = c_pred; e.rep_loss = rep_loss;
   // scratch: the X2H planes are free once the denoiser is done (the CoM head uses the H2X planes)
-  const BpScratch s = bp_scratch(ws, n_lig, K);
+  const BpScratch s = bp_scratch(ws, plan->n_lig, plan->num_classes);
   e.logits = s.logits; e.x_pred = s.x_pred;
   e.xs = (float4*)ws.plane[0]; e.thr = (int2*)ws.plane[1]; e.graph_part = ws.plane[2];
-  CBG_CUDA_OK(cudaMemcpyAsync(ws.h, plan->h_static, (size_t)plan->n_nodes * CBG_H * sizeof(float), cudaMemcpyDeviceToDevice, st));
   if (int rc = cbg_launch_bp_eval_noise(e, st)) return rc;
   if (int rc = run_bp_denoiser(*plan, com_blob, com_layers, ws, xt, s.logits, s.x_pred, st)) return rc;
   return cbg_launch_bp_eval_loss(e, st);
@@ -897,31 +905,25 @@ int32_t cbg_reverse_step_f32(const cbg_step_coef* coef, const float* x0_pred, co
 int32_t cbg_eval_loss_f32(const cbg_sample_plan* plan, const cbg_eval_coef* coefs, int32_t n_rep, const float* x0,
                           const int64_t* v0, const float* pos_noise, const float* type_uniform, float* xt, int64_t* vt,
                           float* x_pred, float* c_pred, float* graph_loss, float* rep_loss, void* stream) {
-  Workspace ws;
-  if (int rc = open_plan(plan, coefs && x0 && v0 && pos_noise && type_uniform && xt && vt && x_pred && c_pred && graph_loss &&
-                         rep_loss, "cbg_eval_loss_f32: null argument", &ws)) return rc;
-  if (int rc = check_replicas(*plan, n_rep)) return rc;
   NvtxRange nvtx_eval("cbg:eval_loss");
   cudaStream_t st = (cudaStream_t)stream;
-  const int K = plan->num_classes;
+  Workspace ws;
   EvalArgs e{};
+  if (int rc = open_eval(plan, coefs && x0 && v0 && pos_noise && type_uniform && xt && vt && x_pred && c_pred && graph_loss &&
+                         rep_loss, "cbg_eval_loss_f32: null argument", n_rep, 1, x0, v0, &ws, &e.b, st)) return rc;
   for (int r = 0; r < n_rep; ++r) {
     const cbg_eval_coef& c = coefs[r];
     e.coef.c[r] = EvalCoefDev{c.alphas_cumprod, c.log_alphas_cumprod, c.log_one_minus_alphas_cumprod, c.log_alphas_cumprod_prev,
                               c.log_one_minus_alphas_cumprod_prev, c.log_alpha, c.log_one_minus_alpha, c.t_is_zero ? 1 : 0};
   }
-  e.n_rep = n_rep; e.n_lig = plan->n_lig; e.n_graphs = plan->n_graphs; e.num_classes = K;
-  e.lig_node = plan->lig_node; e.graph_ptr = plan->graph_ptr; e.gen = plan->gen_lig;
-  e.x0 = x0; e.v0 = (const long long*)v0; e.pos_noise = pos_noise; e.type_u = type_uniform;
-  e.emb_wt = plan->emb_wt; e.h_lig_bias = plan->h_lig_bias;
-  e.x4 = ws.x4; e.h = ws.h; e.xt = xt; e.vt = (long long*)vt; e.x_pred = x_pred; e.c_pred = c_pred;
+  e.n_rep = n_rep; e.pos_noise = pos_noise; e.type_u = type_uniform;
+  e.xt = xt; e.vt = (long long*)vt; e.x_pred = x_pred; e.c_pred = c_pred;
   e.logits = ws.w;                  // classifier scratch: the attention-weight buffer is free after the layers
   e.graph_cnt = (int*)ws.ew;        // so is the edge-gate buffer (n_nodes * 32 >= n_graphs entries)
   e.graph_loss = graph_loss; e.rep_loss = rep_loss;
-  CBG_CUDA_OK(cudaMemcpyAsync(ws.h, plan->h_static, (size_t)plan->n_nodes * CBG_H * sizeof(float), cudaMemcpyDeviceToDevice, st));
   if (int rc = cbg_launch_eval_noise(e, st)) return rc;
   if (int rc = run_denoiser(*plan, ws, st)) return rc;
-  if (int rc = cbg_launch_classifier(plan->blob, ws.h, plan->lig_node, plan->n_lig, K, ws.w, st)) return rc;
+  if (int rc = cbg_launch_classifier(plan->blob, ws.h, plan->lig_node, plan->n_lig, plan->num_classes, ws.w, st)) return rc;
   return cbg_launch_eval_loss(e, st);
 }
 
@@ -929,16 +931,15 @@ int32_t cbg_sbdd_eval_loss_f32(const cbg_sample_plan* plan, const cbg_sbdd_eval_
                                const float* x0, const int64_t* v0, const float* x_rec, const float* x_t_noise,
                                const float* c_t_noise, const float* x_0_noise, const float* c_0_noise, float* vec_pos,
                                float* vec_atom, float* terms, float* t_loss, void* stream) {
-  Workspace ws;
-  if (int rc = open_plan(plan, coefs && x0 && v0 && x_t_noise && c_t_noise && x_0_noise && c_0_noise && vec_pos && vec_atom &&
-                         terms && t_loss && (x_rec || plan->n_nodes == plan->n_lig), "cbg_sbdd_eval_loss_f32: null argument", &ws)) return rc;
-  if (plan->rcache || plan->static_lists) { cbg_set_error("DiffSBDD moves the pocket with every noised copy: the plan must not carry static lists / an R-cache"); return 1; }
-  if (int rc = check_replicas(*plan, n_t, 2)) return rc;
-  if ((plan->n_nodes - plan->n_lig) % (2 * n_t)) { cbg_set_error("plan (n_nodes=%lld) is not %d replicas of one batch", (long long)plan->n_nodes, 2 * n_t); return 1; }
   NvtxRange nvtx_eval("cbg:sbdd_eval_loss");
   cudaStream_t st = (cudaStream_t)stream;
-  const int K = plan->num_classes;
+  Workspace ws;
   SbddEvalArgs e{};
+  if (int rc = open_eval(plan, coefs && x0 && v0 && x_t_noise && c_t_noise && x_0_noise && c_0_noise && vec_pos && vec_atom &&
+                         terms && t_loss && (x_rec || plan->n_nodes == plan->n_lig), "cbg_sbdd_eval_loss_f32: null argument",
+                         n_t, 2, x0, v0, &ws, &e.b, st)) return rc;
+  if (plan->rcache || plan->static_lists) { cbg_set_error("DiffSBDD moves the pocket with every noised copy: the plan must not carry static lists / an R-cache"); return 1; }
+  if ((plan->n_nodes - plan->n_lig) % (2 * n_t)) { cbg_set_error("plan (n_nodes=%lld) is not %d replicas of one batch", (long long)plan->n_nodes, 2 * n_t); return 1; }
   for (int j = 0; j < n_t; ++j) {
     const cbg_sbdd_eval_coef& c = coefs[j];
     e.coef.c[j] = SbddEvalCoefDev{c.pos_alpha_t, c.pos_sigma_t, c.type_alpha_t, c.type_sigma_t, c.pos_alpha_0, c.pos_sigma_0,
@@ -946,17 +947,13 @@ int32_t cbg_sbdd_eval_loss_f32(const cbg_sample_plan* plan, const cbg_sbdd_eval_
                                   c.type_log_const, c.pos_alpha_T, c.type_alpha_T, c.pos_log_inv_sigma_T,
                                   c.type_log_inv_sigma_T, c.pos_sigma2_T, c.type_sigma2_T};
   }
-  e.n_t = n_t; e.n_lig = plan->n_lig; e.n_graphs = plan->n_graphs; e.num_classes = K; e.n_nodes = plan->n_nodes;
-  e.lig_node = plan->lig_node; e.graph_ptr = plan->graph_ptr; e.gen = plan->gen_lig;
-  e.x0 = x0; e.v0 = (const long long*)v0; e.x_rec = x_rec;
+  e.n_t = n_t; e.n_nodes = plan->n_nodes; e.x_rec = x_rec;
   e.x_t_noise = x_t_noise; e.c_t_noise = c_t_noise; e.x_0_noise = x_0_noise; e.c_0_noise = c_0_noise;
-  e.emb_wt = plan->emb_wt; e.h_lig_bias = plan->h_lig_bias;
   e.logits = ws.w;                  // classifier scratch: the attention-weight buffer is free after the layers
-  e.x4 = ws.x4; e.h = ws.h; e.vec_pos = vec_pos; e.vec_atom = vec_atom; e.terms = terms; e.t_loss = t_loss;
-  CBG_CUDA_OK(cudaMemcpyAsync(ws.h, plan->h_static, (size_t)plan->n_nodes * CBG_H * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  e.vec_pos = vec_pos; e.vec_atom = vec_atom; e.terms = terms; e.t_loss = t_loss;
   if (int rc = cbg_launch_sbdd_eval_noise(e, st)) return rc;
   if (int rc = run_denoiser(*plan, ws, st)) return rc;
-  if (int rc = cbg_launch_classifier(plan->blob, ws.h, plan->lig_node, plan->n_lig, K, ws.w, st)) return rc;
+  if (int rc = cbg_launch_classifier(plan->blob, ws.h, plan->lig_node, plan->n_lig, plan->num_classes, ws.w, st)) return rc;
   return cbg_launch_sbdd_eval_loss(e, st);
 }
 

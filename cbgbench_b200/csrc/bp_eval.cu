@@ -16,60 +16,28 @@
 
 namespace {
 
-constexpr int kThreads = 128, kWarps = kThreads / 32;
-
-__global__ void __launch_bounds__(kThreads) bp_eval_noise_kernel(BpEvalArgs p) {
+__global__ void __launch_bounds__(128) bp_eval_noise_kernel(BpEvalArgs p) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;      // replicated ligand atom
-  if (i >= p.n_lig) return;
-  const int n1 = p.n_lig / p.n_rep;
+  if (i >= p.b.n_lig) return;
+  const int n1 = p.b.n_lig / p.n_rep;
   const int r = i / n1, a = i - r * n1;
   const BpEvalCoefDev cf = p.coef.c[r];
-  const bool gen = p.gen[i] != 0;
+  const bool gen = p.b.gen[i] != 0;
   // positions: x_t = sqrt(a) * x0 + sqrt(1 - a) * eps with the raw eps (the zero-centred one is only the target)
   const float sa = __fsqrt_rn(cf.alphas_cumprod), s1 = __fsqrt_rn(__fsub_rn(1.f, cf.alphas_cumprod));
   float xt[3];
 #pragma unroll
   for (int c = 0; c < 3; ++c) {
-    const float x0 = p.x0[3 * a + c];
+    const float x0 = p.b.x0[3 * a + c];
     xt[c] = gen ? __fadd_rn(__fmul_rn(sa, x0), __fmul_rn(s1, p.pos_noise[3 * (size_t)i + c])) : x0;
     p.xt[3 * (size_t)i + c] = xt[c];
   }
   // types: generated atoms drawn below t / T go to the absorbing state 0
   const bool mask = gen && p.type_u[i] < cf.mask_prob;
-  const int vt = mask ? 0 : (int)p.v0[a];
+  const int vt = mask ? 0 : (int)p.b.v0[a];
   p.vt[i] = vt;
   p.mask[i] = mask ? 1 : 0;
-  const int node = p.lig_node[i];
-  float4 v = p.x4[node];
-  v.x = xt[0]; v.y = xt[1]; v.z = xt[2];
-  p.x4[node] = v;
-  const float* bias = p.h_lig_bias + (size_t)i * CBG_H;
-  const float* w = p.emb_wt + (size_t)vt * CBG_H;
-  float* h = p.h + (size_t)node * CBG_H;
-  for (int k = 0; k < CBG_H; k += 4) st4(h + k, add4(ldg4(bias + k), ldg4(w + k)));
-}
-
-__device__ __forceinline__ int lower_bound(const int* __restrict__ a, int n, int key) {
-  int lo = 0, hi = n;
-  while (lo < hi) {
-    const int mid = (lo + hi) >> 1;
-    if (a[mid] < key) lo = mid + 1; else hi = mid;
-  }
-  return lo;
-}
-
-// block sum of N per-thread values into out[] (every thread gets the result); fixed order
-template <int N>
-__device__ __forceinline__ void block_sum(float (&v)[N], float (*s_red)[N], float* out) {
-#pragma unroll
-  for (int c = 0; c < N; ++c) v[c] = warp_sum(v[c]);
-  if ((threadIdx.x & 31) == 0) {
-#pragma unroll
-    for (int c = 0; c < N; ++c) s_red[threadIdx.x >> 5][c] = v[c];
-  }
-  __syncthreads();
-  if (threadIdx.x < N) out[threadIdx.x] = (s_red[0][threadIdx.x] + s_red[1][threadIdx.x]) + (s_red[2][threadIdx.x] + s_red[3][threadIdx.x]);
-  __syncthreads();
+  store_noised_ligand(p.b, i, xt, vt);
 }
 
 // the kNN distance of oracle.graph_ops.pairwise_sqdist_f32: centre (protein) minus point, individually rounded
@@ -78,28 +46,23 @@ __device__ __forceinline__ float sqdist(const float4 c, const float4 x) {
   return __fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz));
 }
 
-__global__ void __launch_bounds__(kThreads) bp_eval_loss_kernel(BpEvalArgs p) {
-  __shared__ int s_rng[2];
-  __shared__ float s_red9[kWarps][9];
-  __shared__ float s_red5[kWarps][5];
-  __shared__ float s_red1[kWarps][1];
+__global__ void __launch_bounds__(kGraphThreads) bp_eval_loss_kernel(BpEvalArgs p) {
+  __shared__ float s_red9[kGraphWarps][9];
+  __shared__ float s_red5[kGraphWarps][5];
+  __shared__ float s_red1[kGraphWarps][1];
   __shared__ float s_mean[9], s_tot[5], s_inter[1];
   const int g = blockIdx.x;                                  // replicated graph
-  const int r = g / (p.n_graphs / p.n_rep);
-  if (threadIdx.x == 0) {
-    s_rng[0] = lower_bound(p.lig_node, p.n_lig, p.graph_ptr[g]);
-    s_rng[1] = lower_bound(p.lig_node, p.n_lig, p.graph_ptr[g + 1]);
-  }
-  __syncthreads();
-  const int lo = s_rng[0], hi = s_rng[1], n_g = hi - lo;
-  const int n1 = p.n_lig / p.n_rep;
+  const int r = g / (p.b.n_graphs / p.n_rep);
+  const int2 rng = graph_ligand_range(p.b.lig_node, p.b.n_lig, p.b.graph_ptr, g);
+  const int lo = rng.x, hi = rng.y, n_g = hi - lo;
+  const int n1 = p.b.n_lig / p.n_rep;
   const BpEvalCoefDev cf = p.coef.c[r];
-  const int K = p.num_classes;
+  const int K = p.b.num_classes;
   // ---- graph means over ALL ligand atoms: raw noise, denoiser shift x_pred - x_t, CoM-head shift x_com - x_t
   {
     float s[9] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
     for (int i = lo + threadIdx.x; i < hi; i += blockDim.x) {
-      const float4 xc = p.x4[p.lig_node[i]];
+      const float4 xc = p.b.x4[p.b.lig_node[i]];
       const float com[3] = {xc.x, xc.y, xc.z};
 #pragma unroll
       for (int c = 0; c < 3; ++c) {
@@ -109,9 +72,8 @@ __global__ void __launch_bounds__(kThreads) bp_eval_loss_kernel(BpEvalArgs p) {
         s[6 + c] += __fsub_rn(com[c], xt);
       }
     }
-    float tot[9];
-    block_sum<9>(s, s_red9, tot);
-    if (threadIdx.x < 9) s_mean[threadIdx.x] = __fdiv_rn(tot[threadIdx.x], (float)(n_g > 0 ? n_g : 1));
+    block_sum<9>(s, s_red9, s_mean);
+    if (threadIdx.x < 9) s_mean[threadIdx.x] = __fdiv_rn(s_mean[threadIdx.x], (float)(n_g > 0 ? n_g : 1));
     __syncthreads();
   }
   // ---- per atom: targets / predictions, score losses, masked-type cross-entropy, xs_mean
@@ -120,7 +82,7 @@ __global__ void __launch_bounds__(kThreads) bp_eval_loss_kernel(BpEvalArgs p) {
   float acc[5] = {0.f, 0.f, 0.f, 0.f, 0.f};                 // pos, com, atom, generated count, masked count
   for (int i = lo + threadIdx.x; i < hi; i += blockDim.x) {
     const int a = i - r * n1;
-    const bool gen = p.gen[i] != 0;
+    const bool gen = p.b.gen[i] != 0;
     float* vec = p.vec + ((size_t)r * 8 * n1 + a) * 3;
     const size_t q = (size_t)n1 * 3;                         // stride between the eight vector outputs
     float dp = 0.f, dc = 0.f, xs[3];
@@ -147,7 +109,7 @@ __global__ void __launch_bounds__(kThreads) bp_eval_loss_kernel(BpEvalArgs p) {
     float se = 0.f;
     for (int c = 0; c < K; ++c) se += expf(lg[c] - mx);
     float m2 = -INFINITY, pv0 = 0.f;
-    const int v0 = (int)p.v0[a];
+    const int v0 = (int)p.b.v0[a];
     for (int c = 0; c < K; ++c) {
       const float pr = __fdiv_rn(expf(lg[c] - mx), se);
       p.c_pred[(size_t)i * K + c] = pr;
@@ -163,14 +125,14 @@ __global__ void __launch_bounds__(kThreads) bp_eval_loss_kernel(BpEvalArgs p) {
   }
   block_sum<5>(acc, s_red5, s_tot);          // its barriers also publish p.xs to the whole CTA
   // ---- interior loss: protein atoms of the graph are its first nodes (compose_context puts them before the ligand)
-  const int pb = p.graph_ptr[g], pe = p.graph_ptr[g + 1] - n_g;
+  const int pb = p.b.graph_ptr[g], pe = p.b.graph_ptr[g + 1] - n_g;
   const bool select = n_g > CBG_BP_INTER_K;
   if (select) {
     // per protein atom, one warp: the 48th smallest (d^2, ligand index) pair; the bits of a non-negative float order
     // like the float, so a bitwise radix select finds the 48th smallest d^2, then the tie at that d^2 is cut by index
     const int lane = threadIdx.x & 31;
-    for (int pn = pb + (threadIdx.x >> 5); pn < pe; pn += kWarps) {
-      const float4 xp = p.x4[pn];
+    for (int pn = pb + (threadIdx.x >> 5); pn < pe; pn += kGraphWarps) {
+      const float4 xp = p.b.x4[pn];
       unsigned prefix = 0u;
       for (int bit = 31; bit >= 0; --bit) {
         const unsigned cand = prefix | (1u << bit);
@@ -204,7 +166,7 @@ __global__ void __launch_bounds__(kThreads) bp_eval_loss_kernel(BpEvalArgs p) {
     const float4 xl = p.xs[i];
     float s = 0.f;                                           // protein terms in protein-index order
     for (int pn = pb; pn < pe; ++pn) {
-      const float d2 = sqdist(p.x4[pn], xl);
+      const float d2 = sqdist(p.b.x4[pn], xl);
       if (select) {
         const int2 t = p.thr[pn];
         const unsigned b = __float_as_uint(d2);
@@ -231,7 +193,7 @@ __global__ void __launch_bounds__(kThreads) bp_eval_loss_kernel(BpEvalArgs p) {
 __global__ void bp_eval_reduce_kernel(BpEvalArgs p) {
   const int r = blockIdx.x * blockDim.x + threadIdx.x;
   if (r >= p.n_rep) return;
-  const int B = p.n_graphs / p.n_rep;
+  const int B = p.b.n_graphs / p.n_rep;
   const float* gp = p.graph_part + 8 * (size_t)r * B;
   int last_g = -1, last_m = -1;
   for (int g = 0; g < B; ++g) {
@@ -245,23 +207,23 @@ __global__ void bp_eval_reduce_kernel(BpEvalArgs p) {
   p.rep_loss[4 * r + 0] = last_g < 0 ? NAN : __fdiv_rn(sp, (float)(last_g + 1));
   p.rep_loss[4 * r + 1] = last_m < 0 ? 0.f : __fdiv_rn(sa, (float)(last_m + 1));
   p.rep_loss[4 * r + 2] = last_g < 0 ? NAN : __fdiv_rn(sc, (float)(last_g + 1));
-  p.rep_loss[4 * r + 3] = __fdiv_rn(si, (float)(p.n_lig / p.n_rep));
+  p.rep_loss[4 * r + 3] = __fdiv_rn(si, (float)(p.b.n_lig / p.n_rep));
 }
 
 }  // namespace
 
 int cbg_launch_bp_eval_noise(const BpEvalArgs& a, cudaStream_t st) {
-  if (a.n_lig <= 0) return 0;
+  if (a.b.n_lig <= 0) return 0;
   CBG_PROF_BEGIN(CBG_K_STEP_INIT, st);
-  bp_eval_noise_kernel<<<(a.n_lig + kThreads - 1) / kThreads, kThreads, 0, st>>>(a);
+  bp_eval_noise_kernel<<<(a.b.n_lig + 127) / 128, 128, 0, st>>>(a);
   CBG_LAUNCHED(CBG_K_STEP_INIT, st);
   return 0;
 }
 
 int cbg_launch_bp_eval_loss(const BpEvalArgs& a, cudaStream_t st) {
-  if (a.n_graphs <= 0) return 0;
+  if (a.b.n_graphs <= 0) return 0;
   CBG_PROF_BEGIN(CBG_K_REVERSE, st);
-  bp_eval_loss_kernel<<<a.n_graphs, kThreads, 0, st>>>(a);
+  bp_eval_loss_kernel<<<a.b.n_graphs, kGraphThreads, 0, st>>>(a);
   CBG_LAUNCHED(CBG_K_REVERSE, st);
   CBG_PROF_BEGIN(CBG_K_REVERSE, st);
   bp_eval_reduce_kernel<<<(a.n_rep + 63) / 64, 64, 0, st>>>(a);

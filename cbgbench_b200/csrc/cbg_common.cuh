@@ -72,6 +72,49 @@ __device__ __forceinline__ float warp_sum(float v) {
   return v;
 }
 
+// ---- per-graph kernels (reverse steps, validation losses): one CTA of kGraphThreads threads per graph ----------------
+constexpr int kGraphThreads = 128, kGraphWarps = kGraphThreads / 32;
+static_assert(kGraphWarps == 4, "block_sum adds exactly four warp partials: (w0 + w1) + (w2 + w3)");
+
+// first index of the ascending a[0, n) whose value is >= key (n if none)
+__device__ __forceinline__ int lower_bound(const int* __restrict__ a, int n, int key) {
+  int lo = 0, hi = n;
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    if (a[mid] < key) lo = mid + 1; else hi = mid;
+  }
+  return lo;
+}
+
+// Graph g's ligand atoms [lo, hi), returned to every thread of the CTA: lig_node holds the ascending composed node index
+// of every ligand atom and graph g owns the nodes [graph_ptr[g], graph_ptr[g + 1]).  Thread 0 searches, a barrier
+// publishes the result.
+__device__ __forceinline__ int2 graph_ligand_range(const int* __restrict__ lig_node, int n_lig,
+                                                   const int* __restrict__ graph_ptr, int g) {
+  __shared__ int s_rng[2];
+  if (threadIdx.x == 0) {
+    s_rng[0] = lower_bound(lig_node, n_lig, graph_ptr[g]);
+    s_rng[1] = lower_bound(lig_node, n_lig, graph_ptr[g + 1]);
+  }
+  __syncthreads();
+  return make_int2(s_rng[0], s_rng[1]);
+}
+
+// Sum of N per-thread values over the kGraphThreads threads of the CTA into out[N] (shared memory, read by any thread
+// after the call), in a fixed order: warp_sum, then (w0 + w1) + (w2 + w3).  s_red is [kGraphWarps][N] shared scratch.
+template <int N>
+__device__ __forceinline__ void block_sum(float (&v)[N], float (*s_red)[N], float* out) {
+#pragma unroll
+  for (int c = 0; c < N; ++c) v[c] = warp_sum(v[c]);
+  if ((threadIdx.x & 31) == 0) {
+#pragma unroll
+    for (int c = 0; c < N; ++c) s_red[threadIdx.x >> 5][c] = v[c];
+  }
+  __syncthreads();
+  if (threadIdx.x < N) out[threadIdx.x] = (s_red[0][threadIdx.x] + s_red[1][threadIdx.x]) + (s_red[2][threadIdx.x] + s_red[3][threadIdx.x]);
+  __syncthreads();
+}
+
 // Reduce NV per-lane values across the 32 lanes of a warp with a halving butterfly.
 // On return lane l holds in v[0 .. NV/32) the full (all-lane) sums of the original
 // indices l*(NV/32) + i.  NV must be a power of two >= 32; 2*NV-64 shuffles... (NV-NV/32).

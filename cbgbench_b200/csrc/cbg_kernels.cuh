@@ -147,9 +147,36 @@ int cbg_launch_step_init_io(const StepIO* io, const int* lig_node, int n_lig, in
 // the step-invariant members of `a` are used, the per-step ones (x_t, c_t, noise, outputs, coefficients) come from *io
 int cbg_launch_reverse_io(const ReverseArgs& a, const StepIO* io, cudaStream_t st);
 
-// eval.cu: TargetDiff validation loss over R replicas of a batch (cbg_eval_loss_f32).  The plan's ligand atoms and graphs
-// are replica-major: atom i belongs to replica i / (n_lig / n_rep) and is atom i % (n_lig / n_rep) of the batch.
+// Validation losses (eval.cu, bp_eval.cu, sbdd_eval.cu).  The plan's ligand atoms and graphs are R replicas of one
+// batch, replica-major: atom i belongs to replica i / n1 and is atom i % n1 of the batch (n1 = n_lig / R).
 constexpr int CBG_EVAL_MAX_REPLICAS = 64;
+// the batch block of the three argument structs (api.cu: open_eval fills it)
+struct EvalBatch {
+  int n_lig, n_graphs, num_classes;   // n_lig / n_graphs: replicated totals
+  const int* lig_node;       // [n_lig] ascending composed node index
+  const int* graph_ptr;      // [n_graphs+1]
+  const unsigned char* gen;  // [n_lig] replicated ligand_gen_flag
+  const float* x0;           // [n1,3] the batch's ligand_pos
+  const long long* v0;       // [n1]
+  const float* emb_wt;       // [K,128]
+  const float* h_lig_bias;   // [n_lig,128]
+  float4* x4;                // node coordinates + flags
+  float* h;                  // [N,128] node features
+};
+// replicated ligand atom i noised to (xt, vt) in the denoiser's node state: its coordinates (flags kept) and
+// h = (b_atom + indicator) + W_atom one_hot(vt)
+__device__ __forceinline__ void store_noised_ligand(const EvalBatch& b, int i, const float (&xt)[3], int vt) {
+  const int node = b.lig_node[i];
+  float4 v = b.x4[node];
+  v.x = xt[0]; v.y = xt[1]; v.z = xt[2];
+  b.x4[node] = v;
+  const float* bias = b.h_lig_bias + (size_t)i * CBG_H;
+  const float* w = b.emb_wt + (size_t)vt * CBG_H;
+  float* h = b.h + (size_t)node * CBG_H;
+  for (int k = 0; k < CBG_H; k += 4) st4(h + k, add4(ldg4(bias + k), ldg4(w + k)));
+}
+
+// eval.cu: TargetDiff validation loss over R = n_rep replicas of a batch (cbg_eval_loss_f32)
 struct EvalCoefDev {       // same members as cbg_eval_coef (include/cbg_b200.h)
   float alphas_cumprod, lac, l1mac, lac_prev, l1mac_prev, la, l1ma;
   int t_is_zero;
@@ -157,19 +184,11 @@ struct EvalCoefDev {       // same members as cbg_eval_coef (include/cbg_b200.h)
 struct EvalCoefs { EvalCoefDev c[CBG_EVAL_MAX_REPLICAS]; };   // passed by value: no H2D copy per call
 struct EvalArgs {
   EvalCoefs coef;
-  int n_rep, n_lig, n_graphs, num_classes;   // n_lig / n_graphs: replicated totals
-  const int* lig_node;       // [n_lig] ascending composed node index
-  const int* graph_ptr;      // [n_graphs+1]
-  const unsigned char* gen;  // [n_lig] replicated ligand_gen_flag
-  const float* x0;           // [n_lig/n_rep,3]
-  const long long* v0;       // [n_lig/n_rep]
+  int n_rep;
+  EvalBatch b;
   const float* pos_noise;    // [n_lig,3]
   const float* type_u;       // [n_lig,K]
-  const float* emb_wt;       // [K,128]
-  const float* h_lig_bias;   // [n_lig,128]
   const float* logits;       // [n_lig,K] classifier output (loss kernel)
-  float4* x4;                // node coordinates + flags
-  float* h;                  // [N,128] node features
   float* xt;                 // [n_lig,3]
   long long* vt;             // [n_lig]
   float* x_pred;             // [n_lig,3]
@@ -237,26 +256,19 @@ struct BpArgs {
 };
 int cbg_launch_bp_reverse(const BpArgs& a, cudaStream_t st);
 
-// bp_eval.cu: DiffBP validation loss over R replicas of a batch (cbg_bp_eval_loss_f32), replica-major like EvalArgs.
+// bp_eval.cu: DiffBP validation loss over R = n_rep replicas of a batch (cbg_bp_eval_loss_f32).  After the CoM head
+// the ligand rows of x4 hold x_com.
 constexpr int CBG_BP_INTER_K = 48;       // interior loss: protein -> ligand kNN (diffbp.py:19)
 struct BpEvalCoefDev { float alphas_cumprod, beta, mask_prob; };    // same members as cbg_bp_eval_coef
 struct BpEvalCoefs { BpEvalCoefDev c[CBG_EVAL_MAX_REPLICAS]; };
 struct BpEvalArgs {
   BpEvalCoefs coef;
-  int n_rep, n_lig, n_graphs, num_classes;   // n_lig / n_graphs: replicated totals
-  const int* lig_node;       // [n_lig] ascending composed node index
-  const int* graph_ptr;      // [n_graphs+1]
-  const unsigned char* gen;  // [n_lig] replicated ligand_gen_flag
-  const float* x0;           // [n_lig/n_rep,3]
-  const long long* v0;       // [n_lig/n_rep]
+  int n_rep;
+  EvalBatch b;
   const float* pos_noise;    // [n_lig,3] raw normal draws
   const float* type_u;       // [n_lig] uniform draws of the type mask
-  const float* emb_wt;       // [K,128]
-  const float* h_lig_bias;   // [n_lig,128]
   const float* logits;       // [n_lig,K] classifier output
   const float* x_pred;       // [n_lig,3] denoiser output coordinates
-  float4* x4;                // node coordinates + flags; after the CoM head the ligand rows hold x_com
-  float* h;                  // [N,128] node features
   float* xt;                 // [n_lig,3]
   long long* vt;             // [n_lig]
   unsigned char* mask;       // [n_lig] type mask
@@ -271,8 +283,9 @@ int cbg_launch_bp_eval_noise(const BpEvalArgs& a, cudaStream_t st);
 // bp_eval_loss_kernel (one CTA per graph) followed by bp_eval_reduce_kernel (one thread per replica)
 int cbg_launch_bp_eval_loss(const BpEvalArgs& a, cudaStream_t st);
 
-// sbdd_eval.cu: DiffSBDD validation loss over n_t timesteps of a batch (cbg_sbdd_eval_loss_f32).  The plan holds 2 n_t
-// replicas, replica-major like EvalArgs: replica 2j is timestep j noised at t_j, replica 2j+1 timestep j noised at 0.
+// sbdd_eval.cu: DiffSBDD validation loss over n_t timesteps of a batch (cbg_sbdd_eval_loss_f32).  The plan holds R = 2 n_t
+// replicas: replica 2j is timestep j noised at t_j, replica 2j+1 timestep j noised at 0.  After the denoiser the ligand
+// rows of x4 hold x_pred.
 struct SbddEvalCoefDev {   // same members as cbg_sbdd_eval_coef (include/cbg_b200.h)
   float pos_alpha_t, pos_sigma_t, type_alpha_t, type_sigma_t;
   float pos_alpha_0, pos_sigma_0, type_alpha_0, type_sigma_0;
@@ -285,23 +298,15 @@ struct SbddEvalCoefDev {   // same members as cbg_sbdd_eval_coef (include/cbg_b2
 struct SbddEvalCoefs { SbddEvalCoefDev c[CBG_EVAL_MAX_REPLICAS / 2]; };
 struct SbddEvalArgs {
   SbddEvalCoefs coef;
-  int n_t, n_lig, n_graphs, num_classes;   // n_lig / n_graphs: replicated totals (2 n_t replicas)
+  int n_t;
   long long n_nodes;
-  const int* lig_node;       // [n_lig] ascending composed node index
-  const int* graph_ptr;      // [n_graphs+1]
-  const unsigned char* gen;  // [n_lig] replicated ligand_gen_flag
-  const float* x0;           // [n1,3] the batch's ligand_pos (n1 = n_lig / (2 n_t))
-  const long long* v0;       // [n1]
+  EvalBatch b;
   const float* x_rec;        // [n_rec1,3] the batch's protein_pos
   const float* x_t_noise;    // [n_t,n1,3] / [n_t,n1,K] / [n_t,n1,3] / [n_t,n1,K]: the four draws of each timestep
   const float* c_t_noise;
   const float* x_0_noise;
   const float* c_0_noise;
-  const float* emb_wt;       // [K,128]
-  const float* h_lig_bias;   // [n_lig,128]
   const float* logits;       // [n_lig,K] classifier output
-  float4* x4;                // node coordinates + flags; after the denoiser the ligand rows hold x_pred
-  float* h;                  // [N,128] node features
   float* vec_pos;            // [n_t,3,n1,3]: eps_pred, score_0, score_pred of the positions
   float* vec_atom;           // [n_t,3,n1,K]: the same of the types
   float* terms;              // [n_t,B,6]: pos_t, pos_0, pos_kl, atom_t, atom_0, atom_kl per graph of the batch

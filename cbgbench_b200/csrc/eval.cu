@@ -23,23 +23,23 @@ __device__ __forceinline__ float lae(float a, float b) {       // log_add_exp (c
 
 __global__ void __launch_bounds__(128) eval_noise_kernel(EvalArgs p) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;      // replicated ligand atom
-  if (i >= p.n_lig) return;
-  const int n1 = p.n_lig / p.n_rep;
+  if (i >= p.b.n_lig) return;
+  const int n1 = p.b.n_lig / p.n_rep;
   const int r = i / n1, a = i - r * n1;
   const EvalCoefDev cf = p.coef.c[r];
-  const int K = p.num_classes;
-  const bool gen = p.gen[i] != 0;
+  const int K = p.b.num_classes;
+  const bool gen = p.b.gen[i] != 0;
   // positions: x_t = sqrt(a) * x0 + sqrt(1 - a) * eps   (two separately rounded products and one add)
   const float sa = __fsqrt_rn(cf.alphas_cumprod), s1 = __fsqrt_rn(__fsub_rn(1.f, cf.alphas_cumprod));
   float xt[3];
 #pragma unroll
   for (int c = 0; c < 3; ++c) {
-    const float x0 = p.x0[3 * a + c];
+    const float x0 = p.b.x0[3 * a + c];
     xt[c] = gen ? __fadd_rn(__fmul_rn(sa, x0), __fmul_rn(s1, p.pos_noise[3 * (size_t)i + c])) : x0;
     p.xt[3 * (size_t)i + c] = xt[c];
   }
   // types: v_t = argmax(log q(v_t | v_0) + Gumbel(u)),  log q = log_add_exp(log_c0 + lac[t], l1mac[t] - log K)
-  const int v0 = (int)p.v0[a];
+  const int v0 = (int)p.b.v0[a];
   const float logK = (float)log((double)K);
   const float b = __fsub_rn(cf.l1mac, logK);
   int arg = 0;
@@ -52,15 +52,7 @@ __global__ void __launch_bounds__(128) eval_noise_kernel(EvalArgs p) {
   }
   const int vt = gen ? arg : v0;
   p.vt[i] = vt;
-  // node state of the denoiser: coordinates and h = (b_atom + indicator) + W_atom one_hot(v_t)
-  const int node = p.lig_node[i];
-  float4 v = p.x4[node];
-  v.x = xt[0]; v.y = xt[1]; v.z = xt[2];
-  p.x4[node] = v;
-  const float* bias = p.h_lig_bias + (size_t)i * CBG_H;
-  const float* w = p.emb_wt + (size_t)vt * CBG_H;
-  float* h = p.h + (size_t)node * CBG_H;
-  for (int k = 0; k < CBG_H; k += 4) st4(h + k, add4(ldg4(bias + k), ldg4(w + k)));
+  store_noised_ligand(p.b, i, xt, vt);
 }
 
 // q_v_posterior(log_v0, log_vt, t) (diffusion_scheduler.py:407-418) for one atom; log_vt is the clamped log one-hot of vt
@@ -79,34 +71,20 @@ __device__ __forceinline__ void q_v_posterior(const float* lv0, int vt, const Ev
   for (int c = 0; c < K; ++c) out[c] = __fsub_rn(out[c], lse);
 }
 
-__device__ __forceinline__ int lower_bound(const int* __restrict__ a, int n, int key) {
-  int lo = 0, hi = n;
-  while (lo < hi) {
-    const int mid = (lo + hi) >> 1;
-    if (a[mid] < key) lo = mid + 1; else hi = mid;
-  }
-  return lo;
-}
-
-__global__ void __launch_bounds__(128) eval_loss_kernel(EvalArgs p) {
-  __shared__ int s_rng[2];
-  __shared__ float s_red[4][3];
+__global__ void __launch_bounds__(kGraphThreads) eval_loss_kernel(EvalArgs p) {
+  __shared__ float s_red[kGraphWarps][3], s_tot[3];
   const int g = blockIdx.x;                                  // replicated graph
-  const int r = g / (p.n_graphs / p.n_rep);
-  if (threadIdx.x == 0) {
-    s_rng[0] = lower_bound(p.lig_node, p.n_lig, p.graph_ptr[g]);
-    s_rng[1] = lower_bound(p.lig_node, p.n_lig, p.graph_ptr[g + 1]);
-  }
-  __syncthreads();
-  const int lo = s_rng[0], hi = s_rng[1];
-  const int n1 = p.n_lig / p.n_rep;
+  const int r = g / (p.b.n_graphs / p.n_rep);
+  const int2 rng = graph_ligand_range(p.b.lig_node, p.b.n_lig, p.b.graph_ptr, g);
+  const int lo = rng.x, hi = rng.y;
+  const int n1 = p.b.n_lig / p.n_rep;
   const EvalCoefDev cf = p.coef.c[r];
-  const int K = p.num_classes;
+  const int K = p.b.num_classes;
   const float logK = (float)log((double)K);
   float sum_pos = 0.f, sum_atom = 0.f, cnt = 0.f;
   for (int i = lo + threadIdx.x; i < hi; i += blockDim.x) {
     const int a = i - r * n1;
-    const float4 xp = p.x4[p.lig_node[i]];
+    const float4 xp = p.b.x4[p.b.lig_node[i]];
     p.x_pred[3 * (size_t)i] = xp.x; p.x_pred[3 * (size_t)i + 1] = xp.y; p.x_pred[3 * (size_t)i + 2] = xp.z;
     // log_softmax of the classifier logits; c_pred = exp(log_softmax)
     float lcp[CBG_MAXCLS], lc0[CBG_MAXCLS], lpt[CBG_MAXCLS], lpp[CBG_MAXCLS];
@@ -119,12 +97,12 @@ __global__ void __launch_bounds__(128) eval_loss_kernel(EvalArgs p) {
       lcp[c] = __fsub_rn(__fsub_rn(lcp[c], mx), lse);
       p.c_pred[(size_t)i * K + c] = expf(lcp[c]);
     }
-    if (p.gen[i] == 0) continue;
+    if (p.b.gen[i] == 0) continue;
     // positions: ||x_pred - x0||^2
-    const float d0 = __fsub_rn(xp.x, p.x0[3 * a]), d1 = __fsub_rn(xp.y, p.x0[3 * a + 1]), d2 = __fsub_rn(xp.z, p.x0[3 * a + 2]);
+    const float d0 = __fsub_rn(xp.x, p.b.x0[3 * a]), d1 = __fsub_rn(xp.y, p.b.x0[3 * a + 1]), d2 = __fsub_rn(xp.z, p.b.x0[3 * a + 2]);
     sum_pos += __fadd_rn(__fadd_rn(__fmul_rn(d0, d0), __fmul_rn(d1, d1)), __fmul_rn(d2, d2));
     // types: KL(q(v_{t-1} | v_t, v_0) || q(v_{t-1} | v_t, c_pred)), or at t == 0 the decoder NLL -sum exp(log_c0) log p
-    const int v0 = (int)p.v0[a], vt = (int)p.vt[i];
+    const int v0 = (int)p.b.v0[a], vt = (int)p.vt[i];
     for (int c = 0; c < K; ++c) lc0[c] = c == v0 ? 0.f : log_1e30();
     q_v_posterior(lc0, vt, cf, logK, K, lpt);
     q_v_posterior(lcp, vt, cf, logK, K, lpp);
@@ -138,17 +116,13 @@ __global__ void __launch_bounds__(128) eval_loss_kernel(EvalArgs p) {
     sum_atom += __fadd_rn(__fmul_rn(mask, nll), __fmul_rn(__fsub_rn(1.f, mask), kl));
     cnt += 1.f;
   }
-  sum_pos = warp_sum(sum_pos); sum_atom = warp_sum(sum_atom); cnt = warp_sum(cnt);
-  if ((threadIdx.x & 31) == 0) { s_red[threadIdx.x >> 5][0] = sum_pos; s_red[threadIdx.x >> 5][1] = sum_atom; s_red[threadIdx.x >> 5][2] = cnt; }
-  __syncthreads();
+  float v[3] = {sum_pos, sum_atom, cnt};
+  block_sum<3>(v, s_red, s_tot);
   if (threadIdx.x == 0) {
-    float t[3];
-#pragma unroll
-    for (int c = 0; c < 3; ++c) t[c] = (s_red[0][c] + s_red[1][c]) + (s_red[2][c] + s_red[3][c]);
-    const float n = fmaxf(t[2], 1.f);                         // scatter_mean: sum / max(count, 1)
-    p.graph_loss[2 * (size_t)g] = __fdiv_rn(t[0], n);
-    p.graph_loss[2 * (size_t)g + 1] = __fdiv_rn(t[1], n);
-    p.graph_cnt[g] = (int)t[2];
+    const float n = fmaxf(s_tot[2], 1.f);                     // scatter_mean: sum / max(count, 1)
+    p.graph_loss[2 * (size_t)g] = __fdiv_rn(s_tot[0], n);
+    p.graph_loss[2 * (size_t)g + 1] = __fdiv_rn(s_tot[1], n);
+    p.graph_cnt[g] = (int)s_tot[2];
   }
 }
 
@@ -157,7 +131,7 @@ __global__ void __launch_bounds__(128) eval_loss_kernel(EvalArgs p) {
 __global__ void eval_reduce_kernel(EvalArgs p) {
   const int r = blockIdx.x * blockDim.x + threadIdx.x;
   if (r >= p.n_rep) return;
-  const int B = p.n_graphs / p.n_rep;
+  const int B = p.b.n_graphs / p.n_rep;
   int last = -1;
   for (int g = 0; g < B; ++g) if (p.graph_cnt[r * B + g] > 0) last = g;
   float s0 = 0.f, s1 = 0.f;
@@ -170,17 +144,17 @@ __global__ void eval_reduce_kernel(EvalArgs p) {
 }  // namespace
 
 int cbg_launch_eval_noise(const EvalArgs& a, cudaStream_t st) {
-  if (a.n_lig <= 0) return 0;
+  if (a.b.n_lig <= 0) return 0;
   CBG_PROF_BEGIN(CBG_K_STEP_INIT, st);
-  eval_noise_kernel<<<(a.n_lig + 127) / 128, 128, 0, st>>>(a);
+  eval_noise_kernel<<<(a.b.n_lig + 127) / 128, 128, 0, st>>>(a);
   CBG_LAUNCHED(CBG_K_STEP_INIT, st);
   return 0;
 }
 
 int cbg_launch_eval_loss(const EvalArgs& a, cudaStream_t st) {
-  if (a.n_graphs <= 0) return 0;
+  if (a.b.n_graphs <= 0) return 0;
   CBG_PROF_BEGIN(CBG_K_REVERSE, st);
-  eval_loss_kernel<<<a.n_graphs, 128, 0, st>>>(a);
+  eval_loss_kernel<<<a.b.n_graphs, kGraphThreads, 0, st>>>(a);
   CBG_LAUNCHED(CBG_K_REVERSE, st);
   CBG_PROF_BEGIN(CBG_K_REVERSE, st);
   eval_reduce_kernel<<<(a.n_rep + 63) / 64, 64, 0, st>>>(a);

@@ -194,27 +194,13 @@ __global__ void __launch_bounds__(128) reverse_io_kernel(ReverseArgs p, const St
 }
 
 // DiffSBDD reverse step + COM projection, one CTA per graph (see SbddArgs)
-__device__ __forceinline__ int lower_bound_i32(const int* __restrict__ a, int n, int key) {
-  int lo = 0, hi = n;
-  while (lo < hi) {
-    const int mid = (lo + hi) >> 1;
-    if (a[mid] < key) lo = mid + 1; else hi = mid;
-  }
-  return lo;
-}
-
-__global__ void __launch_bounds__(128) sbdd_reverse_kernel(SbddArgs p) {
-  __shared__ int s_rng[2];
-  __shared__ float s_red[4][3];
+__global__ void __launch_bounds__(kGraphThreads) sbdd_reverse_kernel(SbddArgs p) {
+  __shared__ float s_red[kGraphWarps][3];
   __shared__ float s_mean[3];
   const int g = blockIdx.x;
   const int ns = p.graph_ptr[g], ne = p.graph_ptr[g + 1];
-  if (threadIdx.x == 0) {
-    s_rng[0] = lower_bound_i32(p.lig_node, p.n_lig, ns);
-    s_rng[1] = lower_bound_i32(p.lig_node, p.n_lig, ne);
-  }
-  __syncthreads();
-  const int lo = s_rng[0], hi = s_rng[1];
+  const int2 rng = graph_ligand_range(p.lig_node, p.n_lig, p.graph_ptr, g);
+  const int lo = rng.x, hi = rng.y;
   float sum[3] = {0.f, 0.f, 0.f};
   for (int a = lo + threadIdx.x; a < hi; a += blockDim.x) {
     const float4 pr = p.x4[p.lig_node[a]];
@@ -229,18 +215,8 @@ __global__ void __launch_bounds__(128) sbdd_reverse_kernel(SbddArgs p) {
       sum[c] += zs;
     }
   }
-#pragma unroll
-  for (int c = 0; c < 3; ++c) sum[c] = warp_sum(sum[c]);
-  if ((threadIdx.x & 31) == 0) {
-#pragma unroll
-    for (int c = 0; c < 3; ++c) s_red[threadIdx.x >> 5][c] = sum[c];
-  }
-  __syncthreads();
-  if (threadIdx.x < 3) {
-    const float t = (s_red[0][threadIdx.x] + s_red[1][threadIdx.x]) + (s_red[2][threadIdx.x] + s_red[3][threadIdx.x]);
-    const int cnt = hi - lo;
-    s_mean[threadIdx.x] = __fdiv_rn(t, (float)(cnt > 0 ? cnt : 1));     // scatter_mean: sum / max(count, 1)
-  }
+  block_sum<3>(sum, s_red, s_mean);
+  if (threadIdx.x < 3) s_mean[threadIdx.x] = __fdiv_rn(s_mean[threadIdx.x], (float)(hi > lo ? hi - lo : 1));   // scatter_mean
   __syncthreads();
   const float m[3] = {s_mean[0], s_mean[1], s_mean[2]};
   for (int a = lo + threadIdx.x; a < hi; a += blockDim.x) {          // same thread wrote these entries
@@ -273,17 +249,11 @@ __global__ void scatter_x_kernel(const float* __restrict__ x, const int* __restr
 }
 
 // DiffBP reverse step, one CTA per graph (see BpArgs)
-__global__ void __launch_bounds__(128) bp_reverse_kernel(BpArgs p) {
-  __shared__ int s_rng[2];
-  __shared__ float s_red[4][6];
+__global__ void __launch_bounds__(kGraphThreads) bp_reverse_kernel(BpArgs p) {
+  __shared__ float s_red[kGraphWarps][6];
   __shared__ float s_mean[6];
-  const int g = blockIdx.x;
-  if (threadIdx.x == 0) {
-    s_rng[0] = lower_bound_i32(p.lig_node, p.n_lig, p.graph_ptr[g]);
-    s_rng[1] = lower_bound_i32(p.lig_node, p.n_lig, p.graph_ptr[g + 1]);
-  }
-  __syncthreads();
-  const int lo = s_rng[0], hi = s_rng[1];
+  const int2 rng = graph_ligand_range(p.lig_node, p.n_lig, p.graph_ptr, blockIdx.x);
+  const int lo = rng.x, hi = rng.y;
   float sum[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
   for (int a = lo + threadIdx.x; a < hi; a += blockDim.x) {
     const float4 xc = p.x4[p.lig_node[a]];
@@ -295,18 +265,8 @@ __global__ void __launch_bounds__(128) bp_reverse_kernel(BpArgs p) {
       sum[3 + c] += __fsub_rn(com[c], xt);
     }
   }
-#pragma unroll
-  for (int c = 0; c < 6; ++c) sum[c] = warp_sum(sum[c]);
-  if ((threadIdx.x & 31) == 0) {
-#pragma unroll
-    for (int c = 0; c < 6; ++c) s_red[threadIdx.x >> 5][c] = sum[c];
-  }
-  __syncthreads();
-  if (threadIdx.x < 6) {
-    const float t = (s_red[0][threadIdx.x] + s_red[1][threadIdx.x]) + (s_red[2][threadIdx.x] + s_red[3][threadIdx.x]);
-    const int cnt = hi - lo;
-    s_mean[threadIdx.x] = __fdiv_rn(t, (float)(cnt > 0 ? cnt : 1));
-  }
+  block_sum<6>(sum, s_red, s_mean);
+  if (threadIdx.x < 6) s_mean[threadIdx.x] = __fdiv_rn(s_mean[threadIdx.x], (float)(hi > lo ? hi - lo : 1));
   __syncthreads();
   const int K = p.num_classes;
   const float sigma = __fsqrt_rn(__fsub_rn(1.f, p.abar));
@@ -357,7 +317,7 @@ int cbg_launch_scatter_x(const float* x, const int* idx, int n, float4* x4, cuda
 int cbg_launch_bp_reverse(const BpArgs& a, cudaStream_t st) {
   if (a.n_graphs <= 0) return 0;
   CBG_PROF_BEGIN(CBG_K_REVERSE, st);
-  bp_reverse_kernel<<<a.n_graphs, 128, 0, st>>>(a);
+  bp_reverse_kernel<<<a.n_graphs, kGraphThreads, 0, st>>>(a);
   CBG_LAUNCHED(CBG_K_REVERSE, st);
   return 0;
 }
@@ -365,7 +325,7 @@ int cbg_launch_bp_reverse(const BpArgs& a, cudaStream_t st) {
 int cbg_launch_sbdd_reverse(const SbddArgs& a, cudaStream_t st) {
   if (a.n_graphs <= 0) return 0;
   CBG_PROF_BEGIN(CBG_K_REVERSE, st);
-  sbdd_reverse_kernel<<<a.n_graphs, 128, 0, st>>>(a);
+  sbdd_reverse_kernel<<<a.n_graphs, kGraphThreads, 0, st>>>(a);
   CBG_LAUNCHED(CBG_K_REVERSE, st);
   return 0;
 }

@@ -15,31 +15,6 @@
 
 namespace {
 
-constexpr int kThreads = 128, kWarps = kThreads / 32;
-
-__device__ __forceinline__ int lower_bound(const int* __restrict__ a, int n, int key) {
-  int lo = 0, hi = n;
-  while (lo < hi) {
-    const int mid = (lo + hi) >> 1;
-    if (a[mid] < key) lo = mid + 1; else hi = mid;
-  }
-  return lo;
-}
-
-// block sum of N per-thread values into out[] (read after the call by any thread); fixed order
-template <int N>
-__device__ __forceinline__ void block_sum(float (&v)[N], float (*s_red)[N], float* out) {
-#pragma unroll
-  for (int c = 0; c < N; ++c) v[c] = warp_sum(v[c]);
-  if ((threadIdx.x & 31) == 0) {
-#pragma unroll
-    for (int c = 0; c < N; ++c) s_red[threadIdx.x >> 5][c] = v[c];
-  }
-  __syncthreads();
-  if (threadIdx.x < N) out[threadIdx.x] = (s_red[0][threadIdx.x] + s_red[1][threadIdx.x]) + (s_red[2][threadIdx.x] + s_red[3][threadIdx.x]);
-  __syncthreads();
-}
-
 // scatter_mean of the batch's clean ligand coordinates over atoms [lo, hi) (one-batch indices) into s_mean[3]
 __device__ __forceinline__ void clean_mean(const float* __restrict__ x0, int lo, int hi, float (*s_red)[3], float* s_mean) {
   float s[3] = {0.f, 0.f, 0.f};
@@ -58,36 +33,31 @@ __device__ __forceinline__ float noised_type(bool gen, bool hot, float alpha, fl
   return gen ? __fadd_rn(__fmul_rn(alpha, c0), __fmul_rn(sigma, eps)) : c0;
 }
 
-__global__ void __launch_bounds__(kThreads) sbdd_eval_noise_kernel(SbddEvalArgs p) {
-  __shared__ int s_rng[2];
-  __shared__ float s_red[kWarps][3];
+__global__ void __launch_bounds__(kGraphThreads) sbdd_eval_noise_kernel(SbddEvalArgs p) {
+  __shared__ float s_red[kGraphWarps][3];
   __shared__ float s_mean0[3], s_m[3];
   const int g = blockIdx.x;                                  // replicated graph
-  const int n_rep = 2 * p.n_t, B1 = p.n_graphs / n_rep, n1 = p.n_lig / n_rep;
-  const int n_rec1 = (int)((p.n_nodes - p.n_lig) / n_rep);
+  const int n_rep = 2 * p.n_t, B1 = p.b.n_graphs / n_rep, n1 = p.b.n_lig / n_rep;
+  const int n_rec1 = (int)((p.n_nodes - p.b.n_lig) / n_rep);
   const int r = g / B1, j = r >> 1;
   const bool at_zero = (r & 1) != 0;
-  if (threadIdx.x == 0) {
-    s_rng[0] = lower_bound(p.lig_node, p.n_lig, p.graph_ptr[g]);
-    s_rng[1] = lower_bound(p.lig_node, p.n_lig, p.graph_ptr[g + 1]);
-  }
-  __syncthreads();
-  const int lo = s_rng[0], hi = s_rng[1], n_g = hi - lo;
+  const int2 rng = graph_ligand_range(p.b.lig_node, p.b.n_lig, p.b.graph_ptr, g);
+  const int lo = rng.x, hi = rng.y, n_g = hi - lo;
   const int lo1 = lo - r * n1, hi1 = hi - r * n1;            // the same atoms in the batch
   const SbddEvalCoefDev& cf = p.coef.c[j];
   const float ax = at_zero ? cf.pos_alpha_0 : cf.pos_alpha_t, sx = at_zero ? cf.pos_sigma_0 : cf.pos_sigma_t;
   const float ac = at_zero ? cf.type_alpha_0 : cf.type_alpha_t, sc = at_zero ? cf.type_sigma_0 : cf.type_sigma_t;
   const float* ex = (at_zero ? p.x_0_noise : p.x_t_noise) + (size_t)j * n1 * 3;
-  const int K = p.num_classes;
+  const int K = p.b.num_classes;
   const float* ec = (at_zero ? p.c_0_noise : p.c_t_noise) + (size_t)j * n1 * K;
-  clean_mean(p.x0, lo1, hi1, s_red, s_mean0);
+  clean_mean(p.b.x0, lo1, hi1, s_red, s_mean0);
   const float mean0[3] = {s_mean0[0], s_mean0[1], s_mean0[2]};
   // x_noisy = alpha * x0c + sigma * eps for every ligand atom; its graph mean m
   float s[3] = {0.f, 0.f, 0.f};
   for (int a = lo1 + threadIdx.x; a < hi1; a += blockDim.x) {
 #pragma unroll
     for (int c = 0; c < 3; ++c) {
-      const float x0c = __fsub_rn(p.x0[3 * a + c], mean0[c]);
+      const float x0c = __fsub_rn(p.b.x0[3 * a + c], mean0[c]);
       s[c] += __fadd_rn(__fmul_rn(ax, x0c), __fmul_rn(sx, ex[3 * a + c]));
     }
   }
@@ -97,37 +67,37 @@ __global__ void __launch_bounds__(kThreads) sbdd_eval_noise_kernel(SbddEvalArgs 
   const float m[3] = {s_m[0], s_m[1], s_m[2]};
   for (int a = lo1 + threadIdx.x; a < hi1; a += blockDim.x) {
     const int i = a + r * n1;
-    const bool gen = p.gen[i] != 0;
-    float4 v = p.x4[p.lig_node[i]];
+    const bool gen = p.b.gen[i] != 0;
+    float4 v = p.b.x4[p.b.lig_node[i]];
     float xv[3];
 #pragma unroll
     for (int c = 0; c < 3; ++c) {
-      const float x0c = __fsub_rn(p.x0[3 * a + c], mean0[c]);
+      const float x0c = __fsub_rn(p.b.x0[3 * a + c], mean0[c]);
       xv[c] = gen ? __fsub_rn(__fadd_rn(__fmul_rn(ax, x0c), __fmul_rn(sx, ex[3 * a + c])), m[c]) : x0c;
     }
     v.x = xv[0]; v.y = xv[1]; v.z = xv[2];
-    p.x4[p.lig_node[i]] = v;
+    p.b.x4[p.b.lig_node[i]] = v;
   }
   // pocket rows: compose_context puts a graph's protein atoms first; x_rec - mean0 - m
-  const int pb = p.graph_ptr[g], pe = p.graph_ptr[g + 1] - n_g;
+  const int pb = p.b.graph_ptr[g], pe = p.b.graph_ptr[g + 1] - n_g;
   for (int pn = pb + threadIdx.x; pn < pe; pn += blockDim.x) {
     const int q = pn - lo - r * n_rec1;                      // protein atom of the batch
-    float4 v = p.x4[pn];
+    float4 v = p.b.x4[pn];
     v.x = __fsub_rn(__fsub_rn(p.x_rec[3 * q], mean0[0]), m[0]);
     v.y = __fsub_rn(__fsub_rn(p.x_rec[3 * q + 1], mean0[1]), m[1]);
     v.z = __fsub_rn(__fsub_rn(p.x_rec[3 * q + 2], mean0[2]), m[2]);
-    p.x4[pn] = v;
+    p.b.x4[pn] = v;
   }
   // ligand rows of h: bias + sum_c W[c] * c_tau[c] (one warp per atom, four columns per lane, like step_init)
   const int lane = threadIdx.x & 31;
-  for (int i = lo + (threadIdx.x >> 5); i < hi; i += kWarps) {
+  for (int i = lo + (threadIdx.x >> 5); i < hi; i += kGraphWarps) {
     const int a = i - r * n1;
-    const bool gen = p.gen[i] != 0;
-    const int v0 = (int)p.v0[a];
-    float4 acc = ldg4(p.h_lig_bias + (size_t)i * CBG_H + 4 * lane);
+    const bool gen = p.b.gen[i] != 0;
+    const int v0 = (int)p.b.v0[a];
+    float4 acc = ldg4(p.b.h_lig_bias + (size_t)i * CBG_H + 4 * lane);
     for (int c = 0; c < K; ++c)
-      fma4(acc, ldg4(p.emb_wt + c * CBG_H + 4 * lane), noised_type(gen, c == v0, ac, sc, ec[(size_t)a * K + c]));
-    st4(p.h + (size_t)p.lig_node[i] * CBG_H + 4 * lane, acc);
+      fma4(acc, ldg4(p.b.emb_wt + c * CBG_H + 4 * lane), noised_type(gen, c == v0, ac, sc, ec[(size_t)a * K + c]));
+    st4(p.b.h + (size_t)p.b.lig_node[i] * CBG_H + 4 * lane, acc);
   }
 }
 
@@ -135,22 +105,17 @@ __device__ __forceinline__ float cdf_standard_gaussian(float x) {
   return __fmul_rn(0.5f, __fadd_rn(1.f, erff(__fdiv_rn(x, 1.41421356f))));     // x / math.sqrt(2) in fp32
 }
 
-__global__ void __launch_bounds__(kThreads) sbdd_eval_loss_kernel(SbddEvalArgs p) {
-  __shared__ int s_rng[2];
-  __shared__ float s_red3[kWarps][3];
-  __shared__ float s_red6[kWarps][6];
+__global__ void __launch_bounds__(kGraphThreads) sbdd_eval_loss_kernel(SbddEvalArgs p) {
+  __shared__ float s_red3[kGraphWarps][3];
+  __shared__ float s_red6[kGraphWarps][6];
   __shared__ float s_mean0[3], s_tot[6];
-  const int n_rep = 2 * p.n_t, B1 = p.n_graphs / n_rep, n1 = p.n_lig / n_rep;
+  const int n_rep = 2 * p.n_t, B1 = p.b.n_graphs / n_rep, n1 = p.b.n_lig / n_rep;
   const int j = blockIdx.x / B1, g = blockIdx.x - j * B1;    // timestep, graph of the batch
-  if (threadIdx.x == 0) {                                    // replica 0's atoms of graph g are the batch's
-    s_rng[0] = lower_bound(p.lig_node, p.n_lig, p.graph_ptr[g]);
-    s_rng[1] = lower_bound(p.lig_node, p.n_lig, p.graph_ptr[g + 1]);
-  }
-  __syncthreads();
-  const int lo = s_rng[0], hi = s_rng[1], n_g = hi - lo;
+  const int2 rng = graph_ligand_range(p.b.lig_node, p.b.n_lig, p.b.graph_ptr, g);     // replica 0's atoms are the batch's
+  const int lo = rng.x, hi = rng.y, n_g = hi - lo;
   const SbddEvalCoefDev& cf = p.coef.c[j];
-  const int K = p.num_classes;
-  clean_mean(p.x0, lo, hi, s_red3, s_mean0);
+  const int K = p.b.num_classes;
+  clean_mean(p.b.x0, lo, hi, s_red3, s_mean0);
   const float mean0[3] = {s_mean0[0], s_mean0[1], s_mean0[2]};
   const float* ext = p.x_t_noise + (size_t)j * n1 * 3;
   const float* ex0 = p.x_0_noise + (size_t)j * n1 * 3;
@@ -163,7 +128,7 @@ __global__ void __launch_bounds__(kThreads) sbdd_eval_loss_kernel(SbddEvalArgs p
   float acc[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
   for (int a = lo + threadIdx.x; a < hi; a += blockDim.x) {
     const int it = (2 * j) * n1 + a, i0 = (2 * j + 1) * n1 + a;
-    const float4 xt4 = p.x4[p.lig_node[it]], x04 = p.x4[p.lig_node[i0]];
+    const float4 xt4 = p.b.x4[p.b.lig_node[it]], x04 = p.b.x4[p.b.lig_node[i0]];
     const float xp_t[3] = {xt4.x, xt4.y, xt4.z}, xp_0[3] = {x04.x, x04.y, x04.z};
     float et = 0.f, e0 = 0.f, mu = 0.f;
 #pragma unroll
@@ -173,15 +138,15 @@ __global__ void __launch_bounds__(kThreads) sbdd_eval_loss_kernel(SbddEvalArgs p
       vp[(size_t)n1 * 3 + 3 * a + c] = __fmul_rn(eps, cf.pos_sigma_t);
       vp[(size_t)2 * n1 * 3 + 3 * a + c] = __fmul_rn(xp_t[c], cf.pos_sigma_t);
       const float dt = __fsub_rn(eps, xp_t[c]), d0 = __fsub_rn(ex0[3 * a + c], xp_0[c]);
-      const float xa = __fmul_rn(cf.pos_alpha_T, __fsub_rn(p.x0[3 * a + c], mean0[c]));
+      const float xa = __fmul_rn(cf.pos_alpha_T, __fsub_rn(p.b.x0[3 * a + c], mean0[c]));
       et = c == 0 ? __fmul_rn(dt, dt) : __fadd_rn(et, __fmul_rn(dt, dt));
       e0 = c == 0 ? __fmul_rn(d0, d0) : __fadd_rn(e0, __fmul_rn(d0, d0));
       mu = c == 0 ? __fmul_rn(xa, xa) : __fadd_rn(mu, __fmul_rn(xa, xa));
     }
     acc[0] += et; acc[1] += e0; acc[2] += mu;
     // types: error_t against the logits of the t copy; the discretised likelihood of the t = 0 copy's noised types
-    const bool gen = p.gen[i0] != 0;
-    const int v0 = (int)p.v0[a];
+    const bool gen = p.b.gen[i0] != 0;
+    const int v0 = (int)p.b.v0[a];
     const float* lg = p.logits + (size_t)it * K;
     float lp[CBG_MAXCLS];
     float ea = 0.f, mx = -INFINITY;
@@ -223,10 +188,10 @@ __global__ void __launch_bounds__(kThreads) sbdd_eval_loss_kernel(SbddEvalArgs p
 __global__ void sbdd_eval_reduce_kernel(SbddEvalArgs p) {
   const int j = blockIdx.x * blockDim.x + threadIdx.x;
   if (j >= p.n_t) return;
-  const int B1 = p.n_graphs / (2 * p.n_t);
+  const int B1 = p.b.n_graphs / (2 * p.n_t);
   int B = 0;
   for (int g = B1 - 1; g >= 0 && B == 0; --g)
-    if (lower_bound(p.lig_node, p.n_lig, p.graph_ptr[g]) < lower_bound(p.lig_node, p.n_lig, p.graph_ptr[g + 1])) B = g + 1;
+    if (lower_bound(p.b.lig_node, p.b.n_lig, p.b.graph_ptr[g]) < lower_bound(p.b.lig_node, p.b.n_lig, p.b.graph_ptr[g + 1])) B = g + 1;
   const float* tm = p.terms + (size_t)j * B1 * 6;
   float sp = 0.f, sa = 0.f;
   for (int g = 0; g < B; ++g) {
@@ -240,17 +205,17 @@ __global__ void sbdd_eval_reduce_kernel(SbddEvalArgs p) {
 }  // namespace
 
 int cbg_launch_sbdd_eval_noise(const SbddEvalArgs& a, cudaStream_t st) {
-  if (a.n_graphs <= 0) return 0;
+  if (a.b.n_graphs <= 0) return 0;
   CBG_PROF_BEGIN(CBG_K_STEP_INIT, st);
-  sbdd_eval_noise_kernel<<<a.n_graphs, kThreads, 0, st>>>(a);
+  sbdd_eval_noise_kernel<<<a.b.n_graphs, kGraphThreads, 0, st>>>(a);
   CBG_LAUNCHED(CBG_K_STEP_INIT, st);
   return 0;
 }
 
 int cbg_launch_sbdd_eval_loss(const SbddEvalArgs& a, cudaStream_t st) {
-  if (a.n_graphs <= 0) return 0;
+  if (a.b.n_graphs <= 0) return 0;
   CBG_PROF_BEGIN(CBG_K_REVERSE, st);
-  sbdd_eval_loss_kernel<<<a.n_graphs / 2, kThreads, 0, st>>>(a);      // n_t * B: one CTA per (timestep, graph)
+  sbdd_eval_loss_kernel<<<a.b.n_graphs / 2, kGraphThreads, 0, st>>>(a);      // n_t * B: one CTA per (timestep, graph)
   CBG_LAUNCHED(CBG_K_REVERSE, st);
   CBG_PROF_BEGIN(CBG_K_REVERSE, st);
   sbdd_eval_reduce_kernel<<<(a.n_t + 31) / 32, 32, 0, st>>>(a);

@@ -123,17 +123,10 @@ class DiffBPB200(BaseDiffB200):
                                       'interior loss unconditionally (diffbp.py:222-226) and raises UnboundLocalError')
         t_values = self._eval_t_values(t_values)
         R, K = len(t_values), self.num_classes
-        dev = next(self.parameters()).device
-        if dev.type != 'cuda':
-            raise NotImplementedError(f'{type(self).__name__}.forward needs the model on a CUDA device: the validation '
-                                      'losses have no CPU implementation')
-        b, n_graphs = self._eval_batch(batch, dev)
+        dev, b, n_graphs, x0, v0, gen = self._eval_batch(batch)
         if 'protein_gen_flag' in b and bool(b['protein_gen_flag'].any()):
             raise NotImplementedError('the interior loss reads the pocket at its input coordinates: protein_gen_flag '
                                       'must be all False')
-        x0 = b['ligand_pos'].float().contiguous()
-        v0 = b['ligand_atom_type'].long().contiguous()
-        gen = b['ligand_gen_flag'] if 'ligand_gen_flag' in b else b['ligand_lig_flag']
         n_lig = x0.shape[0]
         pos_noise, type_uniform = self._eval_noise(R, dev, pos_noise, type_uniform, (n_lig,))
 
@@ -145,20 +138,15 @@ class DiffBPB200(BaseDiffB200):
         c_pred = torch.empty(R, n_lig, K, device=dev)
         rep_loss = torch.empty(R, 4, device=dev)
         L = _lib.lib()
-        launches0 = L.cbg_launch_count()
-        for r0, r1, state in self._eval_launches(b, n_graphs, R, max_nodes):
-            n = r1 - r0
-            coefs = (_lib.BpEvalCoef * n)(*[self.eval_coef(t) for t in t_values[r0:r1]])
-            with torch.cuda.device(dev):
-                _lib.check(L.cbg_bp_eval_loss_f32(
-                    C.byref(state['plan']), com_blob.data_ptr(), self.com_head.num_layers, coefs, n, x0.data_ptr(),
-                    v0.data_ptr(), pos_noise[r0:r1].data_ptr(), type_uniform[r0:r1].data_ptr(), xt[r0:r1].data_ptr(),
-                    vt[r0:r1].data_ptr(), mask[r0:r1].data_ptr(), vec[r0:r1].data_ptr(), c_pred[r0:r1].data_ptr(),
-                    rep_loss[r0:r1].data_ptr(), _lib.stream_ptr(dev)))
-        self.last_launches = L.cbg_launch_count() - launches0
-        per_t = rep_loss.cpu()
-        # get_dict_mean (common.py:33-42): mean over t of the per-t scalars, as a CPU float32 tensor
-        loss_dict = {k: torch.mean(torch.tensor(per_t[:, i].tolist())) for i, k in enumerate(('pos', 'atom', 'com', 'inter'))}
+
+        def launch(r0, r1, state, coefs):
+            _lib.check(L.cbg_bp_eval_loss_f32(
+                C.byref(state['plan']), com_blob.data_ptr(), self.com_head.num_layers, coefs, r1 - r0, x0.data_ptr(),
+                v0.data_ptr(), pos_noise[r0:r1].data_ptr(), type_uniform[r0:r1].data_ptr(), xt[r0:r1].data_ptr(),
+                vt[r0:r1].data_ptr(), mask[r0:r1].data_ptr(), vec[r0:r1].data_ptr(), c_pred[r0:r1].data_ptr(),
+                rep_loss[r0:r1].data_ptr(), _lib.stream_ptr(dev)))
+        self._eval_loop(b, n_graphs, t_values, _lib.BpEvalCoef, max_nodes, launch)
+        loss_dict = self._eval_dict_mean(rep_loss, ('pos', 'atom', 'com', 'inter'))
         vt_onehot = F.one_hot(vt, K).float()
         # the reference's key order: pos_info, then atom_info (its mask_gen, the type mask, replaces gen), then com_info
         results = [{'eps_0': vec[r, 0], 'eps_pred': vec[r, 1], 'score_0': vec[r, 2], 'score_pred': vec[r, 3],

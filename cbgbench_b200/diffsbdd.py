@@ -27,6 +27,7 @@ import torch
 from . import _lib
 from .modules import cfg_get
 from .schedulers import DiffsbddVariationalTables
+from . import targetdiff
 from .targetdiff import BaseDiffB200, register_model
 
 TYPE_NORM = 4.0      # normalize_type / unnormalize_type (diffsbdd.py:95-96, 210-211)
@@ -34,9 +35,9 @@ EVAL_NOISE_KEYS = ('x_t', 'c_t', 'x_0', 'c_0')     # the four draws of one eval 
 
 
 def eval_t_values(num_timesteps, eval_interval=10):
-    """Timesteps of DiffSBDD's eval-mode forward (diffsbdd.py:71-77): ``np.linspace(1, T, eval_interval)``, each
-    truncated by ``torch.tensor([t] * B).long()``.  T = 1000 gives [1, 112, 223, ..., 889, 1000]: t = T is included."""
-    return [int(t) for t in np.linspace(1, num_timesteps, eval_interval).astype(np.int64)]
+    """Timesteps of DiffSBDD's eval-mode forward (diffsbdd.py:71-77): ``targetdiff.eval_t_values`` from first = 1, i.e.
+    ``np.linspace(1, T, eval_interval)`` truncated.  T = 1000 gives [1, 112, 223, ..., 889, 1000]: t = T is included."""
+    return targetdiff.eval_t_values(num_timesteps, eval_interval, first=1)
 
 
 @register_model('diffsbdd')
@@ -99,15 +100,8 @@ class DiffSBDDB200(BaseDiffB200):
         [n_lig,K])."""
         t_values = self._eval_t_values(t_values, first=1)
         R, K = len(t_values), self.num_classes
-        dev = next(self.parameters()).device
-        if dev.type != 'cuda':
-            raise NotImplementedError(f'{type(self).__name__}.forward needs the model on a CUDA device: on the CPU '
-                                      f'{type(self).__name__} is a sampling build without a validation-loss implementation')
-        b, n_graphs = self._eval_batch(batch, dev)
-        x0 = b['ligand_pos'].float().contiguous()
-        v0 = b['ligand_atom_type'].long().contiguous()
+        dev, b, n_graphs, x0, v0, gen = self._eval_batch(batch)
         x_rec = b['protein_pos'].float().contiguous()
-        gen = b['ligand_gen_flag'] if 'ligand_gen_flag' in b else b['ligand_lig_flag']
         n_lig = x0.shape[0]
         dims = {'x_t': 3, 'c_t': K, 'x_0': 3, 'c_0': K}
         if noise is None:
@@ -120,20 +114,16 @@ class DiffSBDDB200(BaseDiffB200):
         terms = torch.empty(R, n_graphs, 6, device=dev)
         t_loss = torch.empty(R, 2, device=dev)
         L = _lib.lib()
-        launches0 = L.cbg_launch_count()
-        for r0, r1, state in self._eval_launches(b, n_graphs, R, max_nodes, copies=2, protein_feature_scale=TYPE_NORM):
-            n = r1 - r0
-            coefs = (_lib.SbddEvalCoef * n)(*[self.eval_coef(t) for t in t_values[r0:r1]])
-            with torch.cuda.device(dev):
-                _lib.check(L.cbg_sbdd_eval_loss_f32(
-                    C.byref(state['plan']), coefs, n, x0.data_ptr(), v0.data_ptr(), x_rec.data_ptr() if x_rec.numel() else None,
-                    *[noise[k][r0:r1].data_ptr() for k in EVAL_NOISE_KEYS], vec_pos[r0:r1].data_ptr(),
-                    vec_atom[r0:r1].data_ptr(), terms[r0:r1].data_ptr(), t_loss[r0:r1].data_ptr(), _lib.stream_ptr(dev)))
-        self.last_launches = L.cbg_launch_count() - launches0
+
+        def launch(r0, r1, state, coefs):
+            _lib.check(L.cbg_sbdd_eval_loss_f32(
+                C.byref(state['plan']), coefs, r1 - r0, x0.data_ptr(), v0.data_ptr(), x_rec.data_ptr() if x_rec.numel() else None,
+                *[noise[k][r0:r1].data_ptr() for k in EVAL_NOISE_KEYS], vec_pos[r0:r1].data_ptr(),
+                vec_atom[r0:r1].data_ptr(), terms[r0:r1].data_ptr(), t_loss[r0:r1].data_ptr(), _lib.stream_ptr(dev)))
+        self._eval_loop(b, n_graphs, t_values, _lib.SbddEvalCoef, max_nodes, launch, copies=2,
+                        protein_feature_scale=TYPE_NORM)
         self.last_terms = terms[:, :int(b['ligand_element_batch'].max()) + 1]
-        per_t = t_loss.cpu()
-        # get_dict_mean (common.py:33-42): mean over t of the per-t scalars, as a CPU float32 tensor
-        loss_dict = {k: torch.mean(torch.tensor(per_t[:, i].tolist())) for i, k in enumerate(('pos', 'atom'))}
+        loss_dict = self._eval_dict_mean(t_loss, ('pos', 'atom'))
         # the reference's key order: pos_info, then atom_info (get_score_loss, diffusion_scheduler.py:944-961)
         results = [{'eps_0_pos': noise['x_t'][r], 'eps_pred_pos': vec_pos[r, 0], 'score_0_pos': vec_pos[r, 1],
                     'score_pred_pos': vec_pos[r, 2], 'mask_gen_pos': gen,

@@ -45,10 +45,12 @@ def get_model(config):
     return _MODEL_DICT[config.type](config)
 
 
-def eval_t_values(num_timesteps, eval_interval=10):
-    """Timesteps of the reference's eval-mode forward (targetdiff.py:67-71): ``np.linspace(0, T-1, eval_interval)``,
-    each truncated toward zero by ``torch.tensor([t] * B).long()``.  T = 50 gives [0, 5, 10, 16, 21, 27, 32, 38, 43, 49]."""
-    return [int(t) for t in np.linspace(0, num_timesteps - 1, eval_interval).astype(np.int64)]
+def eval_t_values(num_timesteps, eval_interval=10, first=0):
+    """Timesteps of the reference's eval-mode forwards: ``np.linspace(first, T - 1 + first, eval_interval)``, each
+    truncated toward zero by ``torch.tensor([t] * B).long()``.  TargetDiff and DiffBP (targetdiff.py:67-71) start at
+    first = 0: T = 50 gives [0, 5, 10, 16, 21, 27, 32, 38, 43, 49].  DiffSBDD (diffsbdd.py:71-77) starts at first = 1,
+    i.e. ``np.linspace(1, T, eval_interval)``: T = 1000 gives [1, 112, 223, ..., 889, 1000], t = T included."""
+    return [int(t) for t in np.linspace(first, num_timesteps - 1 + first, eval_interval).astype(np.int64)]
 
 
 def replicate_batch(batch, n_rep, n_graphs):
@@ -222,25 +224,49 @@ class BaseDiffB200(nn.Module):
                   'ligand_lig_flag', 'protein_lig_flag', 'ligand_element_batch', 'protein_element_batch',
                   'ligand_gen_flag', 'protein_gen_flag')
 
-    def _eval_batch(self, batch, dev):
-        """The batch's tensors on ``dev`` (dict or attribute batch) and its graph count."""
+    def _eval_batch(self, batch):
+        """(dev, b, n_graphs, x0, v0, gen): the model's CUDA device, the batch's tensors on it (dict or attribute batch),
+        its graph count, the clean ligand positions x0 [n_lig,3] float32 and types v0 [n_lig] int64, and its generation
+        flags (ligand_lig_flag when the batch has no ligand_gen_flag)."""
+        dev = next(self.parameters()).device
+        if dev.type != 'cuda':
+            raise NotImplementedError(f'{type(self).__name__}.forward needs the model on a CUDA device: on the CPU '
+                                      f'{type(self).__name__} is a sampling build without a validation-loss implementation')
         g = lambda k, d=None: batch.get(k, d) if hasattr(batch, 'get') else (batch[k] if k in batch else d)
         b = {k: g(k).to(dev) for k in self._EVAL_KEYS if g(k) is not None}
         if b['ligand_pos'].shape[0] == 0:
             raise ValueError('the batch has no ligand atoms')
         n_graphs = int(torch.cat([b['ligand_element_batch'], b['protein_element_batch']]).max()) + 1
-        return b, n_graphs
+        x0 = b['ligand_pos'].float().contiguous()
+        v0 = b['ligand_atom_type'].long().contiguous()
+        gen = b['ligand_gen_flag'] if 'ligand_gen_flag' in b else b['ligand_lig_flag']
+        return dev, b, n_graphs, x0, v0, gen
 
-    def _eval_launches(self, b, n_graphs, R, max_nodes, copies=1, **prepare_kw):
-        """Yield (r0, r1, state): timesteps r0 .. r1-1, ``copies`` noised copies each, prepared as one plan of
-        (r1 - r0) * copies * n_graphs graphs, at most 64 replicas and ``max_nodes`` composed nodes (default
-        ``eval_max_nodes``) per plan.  ``prepare_kw`` goes to ``prepare``."""
+    def _eval_loop(self, b, n_graphs, t_values, coef_type, max_nodes, launch, copies=1, **prepare_kw):
+        """Run the timesteps ``t_values`` in plans of at most 64 replicas and ``max_nodes`` composed nodes (default
+        ``eval_max_nodes``): each plan holds timesteps r0 .. r1-1, ``copies`` noised copies each, as (r1 - r0) * copies *
+        n_graphs graphs (``prepare_kw`` goes to ``prepare``).  ``launch(r0, r1, state, coefs)`` makes the plan's C call,
+        with ``coefs`` the ctypes array of ``eval_coef`` over t_values[r0:r1], on the plan's device.  ``last_launches``
+        counts the kernels of all plans."""
         n_nodes = b['ligand_pos'].shape[0] + b['protein_pos'].shape[0]
         budget = self.eval_max_nodes if max_nodes is None else int(max_nodes)
         per_launch = max(1, min(_lib.EVAL_MAX_REPLICAS // copies, budget // (copies * n_nodes)))
-        for r0 in range(0, R, per_launch):
-            r1 = min(R, r0 + per_launch)
-            yield r0, r1, self.prepare(replicate_batch(b, (r1 - r0) * copies, n_graphs), **prepare_kw)
+        L = _lib.lib()
+        launches0 = L.cbg_launch_count()
+        for r0 in range(0, len(t_values), per_launch):
+            r1 = min(len(t_values), r0 + per_launch)
+            state = self.prepare(replicate_batch(b, (r1 - r0) * copies, n_graphs), **prepare_kw)
+            coefs = (coef_type * (r1 - r0))(*[self.eval_coef(t) for t in t_values[r0:r1]])
+            with torch.cuda.device(state['device']):
+                launch(r0, r1, state, coefs)
+        self.last_launches = L.cbg_launch_count() - launches0
+
+    @staticmethod
+    def _eval_dict_mean(per_t, keys):
+        """get_dict_mean (common.py:33-42) of the per-t losses [R, len(keys)]: for each key the mean over t of its column,
+        as a CPU float32 0-d tensor."""
+        per_t = per_t.cpu()
+        return {k: torch.mean(torch.tensor(per_t[:, i].tolist())) for i, k in enumerate(keys)}
 
     # ---- setup of the step-invariant state ------------------------------------------------
     @torch.no_grad()
@@ -390,13 +416,8 @@ class TargetDiffB200(BaseDiffB200):
         the model device in the reference's order (for each t: randn [n_lig,3], then rand [n_lig,K])."""
         t_values = self._eval_t_values(t_values)
         R, K = len(t_values), self.num_classes
-        dev = next(self.parameters()).device
-        if dev.type != 'cuda':
-            raise RuntimeError(f'{type(self).__name__}.forward needs the model on a CUDA device (no CPU fallback)')
-        b, n_graphs = self._eval_batch(batch, dev)
-        x0 = b['ligand_pos'].float().contiguous()
-        v0 = b['ligand_atom_type'].long().contiguous()
-        mask_gen = b['ligand_gen_flag'].bool() if 'ligand_gen_flag' in b else b['ligand_lig_flag'].bool()
+        dev, b, n_graphs, x0, v0, gen = self._eval_batch(batch)
+        mask_gen = gen.bool()
         n_lig = x0.shape[0]
         pos_noise, type_uniform = self._eval_noise(R, dev, pos_noise, type_uniform, (n_lig, K))
 
@@ -406,21 +427,15 @@ class TargetDiffB200(BaseDiffB200):
         c_pred = torch.empty(R, n_lig, K, device=dev)
         rep_loss = torch.empty(R, 2, device=dev)
         L = _lib.lib()
-        launches0 = L.cbg_launch_count()
-        for r0, r1, state in self._eval_launches(b, n_graphs, R, max_nodes):
-            n = r1 - r0
-            coefs = (_lib.EvalCoef * n)(*[self.eval_coef(t) for t in t_values[r0:r1]])
-            graph_loss = torch.empty(n * n_graphs, 2, device=dev)
-            with torch.cuda.device(dev):
-                _lib.check(L.cbg_eval_loss_f32(
-                    C.byref(state['plan']), coefs, n, x0.data_ptr(), v0.data_ptr(), pos_noise[r0:r1].data_ptr(),
-                    type_uniform[r0:r1].data_ptr(), xt[r0:r1].data_ptr(), vt[r0:r1].data_ptr(), x_pred[r0:r1].data_ptr(),
-                    c_pred[r0:r1].data_ptr(), graph_loss.data_ptr(), rep_loss[r0:r1].data_ptr(), _lib.stream_ptr(dev)))
-        self.last_launches = L.cbg_launch_count() - launches0
-        per_t = rep_loss.cpu()
-        # get_dict_mean (common.py:33-42): mean over t of the per-t scalars, as a CPU float32 tensor
-        loss_dict = {'pos': torch.mean(torch.tensor(per_t[:, 0].tolist())),
-                     'atom': torch.mean(torch.tensor(per_t[:, 1].tolist()))}
+
+        def launch(r0, r1, state, coefs):
+            graph_loss = torch.empty((r1 - r0) * n_graphs, 2, device=dev)
+            _lib.check(L.cbg_eval_loss_f32(
+                C.byref(state['plan']), coefs, r1 - r0, x0.data_ptr(), v0.data_ptr(), pos_noise[r0:r1].data_ptr(),
+                type_uniform[r0:r1].data_ptr(), xt[r0:r1].data_ptr(), vt[r0:r1].data_ptr(), x_pred[r0:r1].data_ptr(),
+                c_pred[r0:r1].data_ptr(), graph_loss.data_ptr(), rep_loss[r0:r1].data_ptr(), _lib.stream_ptr(dev)))
+        self._eval_loop(b, n_graphs, t_values, _lib.EvalCoef, max_nodes, launch)
+        loss_dict = self._eval_dict_mean(rep_loss, ('pos', 'atom'))
         results = [{'x0': x0, 'xt': xt[r], 'x_pred': x_pred[r], 'mask_gen': mask_gen,
                     'v0': v0, 'vt': vt[r], 'c_pred': c_pred[r]} for r in range(R)]
         return loss_dict, results

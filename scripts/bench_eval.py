@@ -1,14 +1,15 @@
 #!/usr/bin/env python
-"""Measurement of the validation loss: eval-mode ``TargetDiffB200.forward(batch)`` (R = eval_interval = 10 timesteps,
-T = 1000 schedule) on one GPU, device-resident inputs, seeded synthetic weights.
+"""Measurement of the validation loss: eval-mode ``forward(batch)`` of TargetDiff, DiffBP or DiffSBDD (R =
+eval_interval = 10 timesteps, DiffSBDD's each noised at t and at 0, T = 1000 schedule) on one GPU, device-resident
+inputs, seeded synthetic weights.
 
 Shapes: c2 (64 pockets x (300 + 24) atoms) and a 4-graph validation batch (the train configs' batch_size: 4).  For
 each: ms per forward (CUDA events around each call, mean over --steps calls after --warmup), kernel launches per call,
-the same R timesteps as R sequential single-timestep calls (what the reference's loop does, on this path), and, when
-the reference has been staged into oracle/_ref/, the reference's eager GPU forward on the same batch.  Prints one
-JSON line.  The GPU name and power limit go with the numbers.
+the same R timesteps as R sequential single-timestep calls (what the reference's loop does, on this path), and, for
+TargetDiff when the reference has been staged into oracle/_ref/, the reference's eager GPU forward on the same batch.
+Prints one JSON line.  The GPU name and power limit go with the numbers.
 
-    python scripts/bench_eval.py [--steps 5] [--warmup 2] [--no-ref]
+    python scripts/bench_eval.py [--model targetdiff|diffbp|diffsbdd] [--steps 5] [--warmup 2] [--no-ref]
 """
 import argparse
 import json
@@ -49,45 +50,61 @@ def time_calls(fn, steps, warmup):
     return sum(s.elapsed_time(e) for s, e in zip(starts, ends)) / steps
 
 
+def noise_kwargs(model_name, R, n, K, dev):
+    """Seeded draws of R timesteps as the keyword arguments of the model's forward / eval_losses, and a slicer that
+    picks timesteps r0 .. r1-1 of them."""
+    from cbgbench_b200 import synthetic
+    if model_name == 'diffsbdd':
+        noise = {k: v.to(dev) for k, v in synthetic.make_sbdd_eval_noise(R, n, K, seed=7).items()}
+        return {'noise': noise}, lambda r0, r1: {'noise': {k: v[r0:r1] for k, v in noise.items()}}
+    pn, tu = synthetic.make_bp_noise(R, n, seed=7) if model_name == 'diffbp' else synthetic.make_noise(R, n, K, seed=7)
+    pn, tu = pn.to(dev), tu.to(dev)
+    return {'pos_noise': pn, 'type_uniform': tu}, lambda r0, r1: {'pos_noise': pn[r0:r1], 'type_uniform': tu[r0:r1]}
+
+
 def main():
     ap = argparse.ArgumentParser()
+    ap.add_argument('--model', choices=('targetdiff', 'diffbp', 'diffsbdd'), default='targetdiff')
     ap.add_argument('--steps', type=int, default=5)
     ap.add_argument('--warmup', type=int, default=2)
-    ap.add_argument('--no-ref', action='store_true')
+    ap.add_argument('--no-ref', action='store_true', help='skip the reference arm (TargetDiff only)')
     args = ap.parse_args()
     import torch
     from cbgbench_b200 import synthetic
-    from cbgbench_b200.targetdiff import TargetDiffB200, eval_t_values
+    from cbgbench_b200.targetdiff import eval_t_values, get_model
     if not torch.cuda.is_available():
         raise SystemExit('bench_eval.py measures the GPU path: no CUDA device')
     torch.set_grad_enabled(False)
     dev = torch.device('cuda', 0)
     torch.cuda.set_device(dev)
-    model = TargetDiffB200(synthetic.targetdiff_config(num_steps=T))
+    cfg = getattr(synthetic, f'{args.model}_config')(num_steps=T)
+    model = get_model(cfg)
     model.load_state_dict(synthetic.seeded_state_dict(model, seed=0), strict=True)
     model = model.to(dev).eval()
-    t_values = eval_t_values(T, 10)
+    t_values = eval_t_values(T, 10, first=1 if args.model == 'diffsbdd' else 0)
     ref = None
-    if not args.no_ref:
+    if args.model == 'targetdiff' and not args.no_ref:
         from baseline import ref_runner
         if ref_runner.ref_root() is not None:
             ref = ref_runner.build_reference_model(T, {}, dev)
-    out = {'workload': f'eval-mode TargetDiff.forward, R={len(t_values)} timesteps, T={T}', 'gpu': gpu_info(),
+    label = {'targetdiff': 'TargetDiff', 'diffbp': 'DiffBP', 'diffsbdd': 'DiffSBDD'}[args.model]
+    copies = ' x 2 noised copies' if args.model == 'diffsbdd' else ''
+    out = {'workload': f'eval-mode {label}.forward, R={len(t_values)} timesteps{copies}, T={T}', 'gpu': gpu_info(),
            'n_gpus': 1, 'steps': args.steps, 'warmup': args.warmup, 'dtype': 'f32', 'data': 'synthetic'}
-    for name, (n_prot, n_lig) in SHAPES.items():
+    for shape, (n_prot, n_lig) in SHAPES.items():
         batch = {k: v.to(dev) for k, v in synthetic.make_batch(n_prot, n_lig, seed=2024).items()}
         n = batch['ligand_pos'].shape[0]
-        pn, tu = synthetic.make_noise(len(t_values), n, 13, seed=7)
-        pn, tu = pn.to(dev), tu.to(dev)
+        kw, part = noise_kwargs(args.model, len(t_values), n, model.num_classes, dev)
         row = {'shape': f'{len(n_prot)} pockets x ({n_prot[0]}+{n_lig[0]}) atoms'}
-        row['ms_per_forward'] = round(time_calls(lambda: model(batch, pos_noise=pn, type_uniform=tu),
-                                                 args.steps, args.warmup), 3)
+        row['ms_per_forward'] = round(time_calls(lambda: model(batch, **kw), args.steps, args.warmup), 3)
         row['launches_per_forward'] = model.last_launches
 
         def sequential():
             for r, t in enumerate(t_values):
-                model.eval_losses(batch, [t], pos_noise=pn[r:r + 1], type_uniform=tu[r:r + 1])
+                model.eval_losses(batch, [t], **part(r, r + 1))
         row['ms_sequential_R_calls'] = round(time_calls(sequential, args.steps, args.warmup), 3)
+        if args.model == 'targetdiff':
+            row['reference_gpu_ms_per_forward'] = None
         if ref is not None:
             # the reference draws its own noise (randn_like / rand_like on the device): same work, other numbers
             torch.cuda.synchronize()
@@ -97,9 +114,7 @@ def main():
             ref(batch)
             torch.cuda.synchronize()
             row['reference_gpu_ms_per_forward'] = round((time.perf_counter() - t0) * 1e3, 3)
-        else:
-            row['reference_gpu_ms_per_forward'] = None
-        out[name] = row
+        out[shape] = row
     print(json.dumps(out), flush=True)
 
 

@@ -24,6 +24,26 @@ def golden(name):
     return np.load(os.path.join(GOLDEN, name))
 
 
+def case_batch(n_prot, n_lig, seed, gen_mode='denovo', empty_graphs=()):
+    """synthetic.make_batch, with the ligand atoms of the graphs ``empty_graphs`` not generated (validation-loss cases)."""
+    batch = synthetic.make_batch(n_prot, n_lig, seed=seed, gen_mode=gen_mode)
+    if empty_graphs:
+        gen = batch.get('ligand_gen_flag', batch['ligand_lig_flag']).clone()
+        for g in empty_graphs:
+            gen[batch['ligand_element_batch'] == g] = False
+        batch['ligand_gen_flag'] = gen
+    return batch
+
+
+def to_dev(batch):
+    return {k: v.cuda() for k, v in batch.items()}
+
+
+def stack(res, key):
+    """The per-t result dicts' ``key`` stacked into one CPU tensor."""
+    return torch.stack([r[key] for r in res]).cpu()
+
+
 def make_model(num_steps=10, device=None, **enc):
     model = TargetDiffB200(synthetic.targetdiff_config(num_steps=num_steps, **enc))
     sd = synthetic.seeded_state_dict(model, seed=WEIGHT_SEED)

@@ -6,7 +6,7 @@ import pytest
 import torch
 
 import bp_eval_loss_oracle as BO
-from helpers import assert_close, golden
+from helpers import assert_close, case_batch, golden, stack, to_dev
 from cbgbench_b200 import synthetic
 from cbgbench_b200.diffbp import DiffBPB200
 from cbgbench_b200.targetdiff import eval_t_values
@@ -31,16 +31,6 @@ def loss_close(got, want):
     if math.isnan(want):
         return math.isnan(got)
     return abs(got - want) <= LOSS_RTOL * abs(want)
-
-
-def case_batch(n_prot, n_lig, seed, gen_mode='denovo', empty_graphs=()):
-    batch = synthetic.make_batch(n_prot, n_lig, seed=seed, gen_mode=gen_mode)
-    if empty_graphs:
-        gen = batch.get('ligand_gen_flag', batch['ligand_lig_flag']).clone()
-        for g in empty_graphs:
-            gen[batch['ligand_element_batch'] == g] = False
-        batch['ligand_gen_flag'] = gen
-    return batch
 
 
 def bp_model(T, device=None, interval=None, **kw):
@@ -137,14 +127,6 @@ def test_forward_raises_without_a_gpu_path():
 
 
 # ---- GPU --------------------------------------------------------------------------------------------------------------
-def to_dev(batch):
-    return {k: v.cuda() for k, v in batch.items()}
-
-
-def stack(res, key):
-    return torch.stack([r[key] for r in res]).cpu()
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize('case', BP_EVAL_CASES, ids=[c[0] for c in BP_EVAL_CASES])
 def test_gpu_forward_matches_reference_fixtures(case):

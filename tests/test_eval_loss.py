@@ -7,7 +7,7 @@ import pytest
 import torch
 
 import eval_loss_oracle as EO
-from helpers import assert_close, golden, make_model
+from helpers import assert_close, case_batch, golden, stack, to_dev, make_model
 from cbgbench_b200 import synthetic
 from cbgbench_b200.targetdiff import eval_t_values
 
@@ -18,16 +18,6 @@ EVAL_CASES = [
     ('t50_interval7', 50, 7, [90, 70], [14, 9], 43, 'denovo', [], 53),
     ('interval1', 1000, 1, [100, 50], [16, 8], 44, 'denovo', [], 54),
 ]
-
-
-def case_batch(n_prot, n_lig, seed, gen_mode='denovo', empty_graphs=()):
-    batch = synthetic.make_batch(n_prot, n_lig, seed=seed, gen_mode=gen_mode)
-    if empty_graphs:
-        gen = batch.get('ligand_gen_flag', batch['ligand_lig_flag']).clone()
-        for g in empty_graphs:
-            gen[batch['ligand_element_batch'] == g] = False
-        batch['ligand_gen_flag'] = gen
-    return batch
 
 
 # Losses agree to 1e-4 relative, plus an absolute 5e-7 (four fp32 ulps of 1): at t == 0 the type loss is the decoder
@@ -121,14 +111,6 @@ def gpu_model(T, interval=None):
     if interval is not None:
         model.cfg['eval_interval'] = interval
     return model, sd
-
-
-def to_dev(batch):
-    return {k: v.cuda() for k, v in batch.items()}
-
-
-def stack(res, key):
-    return torch.stack([r[key] for r in res]).cpu()
 
 
 @pytest.mark.gpu

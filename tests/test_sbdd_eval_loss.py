@@ -7,7 +7,7 @@ import pytest
 import torch
 
 import sbdd_eval_loss_oracle as SO
-from helpers import assert_close, golden
+from helpers import assert_close, case_batch, golden, stack, to_dev
 from cbgbench_b200 import synthetic
 from cbgbench_b200.diffsbdd import DiffSBDDB200, eval_t_values
 
@@ -34,16 +34,6 @@ LOSS_RTOL, TERM_ATOL = 1e-4, 5e-5
 
 def loss_close(got, want):
     return abs(got - want) <= LOSS_RTOL * abs(want)
-
-
-def case_batch(n_prot, n_lig, seed, gen_mode='denovo', empty_graphs=()):
-    batch = synthetic.make_batch(n_prot, n_lig, seed=seed, gen_mode=gen_mode)
-    if empty_graphs:
-        gen = batch.get('ligand_gen_flag', batch['ligand_lig_flag']).clone()
-        for g in empty_graphs:
-            gen[batch['ligand_element_batch'] == g] = False
-        batch['ligand_gen_flag'] = gen
-    return batch
 
 
 def sbdd_model(T, device=None, interval=None, **kw):
@@ -114,14 +104,6 @@ def test_forward_raises_without_a_gpu_path():
 
 
 # ---- GPU --------------------------------------------------------------------------------------------------------------
-def to_dev(batch):
-    return {k: v.cuda() for k, v in batch.items()}
-
-
-def stack(res, key):
-    return torch.stack([r[key] for r in res]).cpu()
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize('case', SBDD_EVAL_CASES, ids=[c[0] for c in SBDD_EVAL_CASES])
 def test_gpu_forward_matches_reference_fixtures(case):
