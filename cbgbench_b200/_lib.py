@@ -148,6 +148,8 @@ SIGNATURES = {
     'cbg_fg_step_f32': (_I32, [C.POINTER(FgPlan), FgCoef, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     'cbg_fg_reverse_f32': (_I32, [C.POINTER(FgPlan), FgCoef] + [_P] * 14),
     'cbg_reverse_step_f32': (_I32, [C.POINTER(StepCoef), _P, _P, _P, _P, _P, _P, _P, _I32, _I32, _P, _P, _P, _P]),
+    'cbg_sbdd_reverse_f32': (_I32, [_P, _P, _I32, _P, _I32, _I32, C.POINTER(SbddCoef)] + [_P] * 8),
+    'cbg_bp_reverse_f32': (_I32, [_P, _P, _I32, _P, _I32, _I32, C.POINTER(BpCoef)] + [_P] * 12),
 }
 
 

@@ -816,6 +816,42 @@ int64_t cbg_sample_step_graph_nodes(const cbg_sample_plan* plan, void* stream) {
   return 0;
 }
 
+namespace {
+// the launch arguments of the DiffSBDD / DiffBP reverse kernels, shared by the steps and the test hooks
+SbddArgs sbdd_args(float4* x4, const int* graph_ptr, int n_graphs, const int* lig_node, int n_lig, int K,
+                   const cbg_sbdd_coef& coef, const float* logits, const float* x_t, const float* c_t,
+                   const float* x_noise, const float* c_noise, float* x_next, float* c_next) {
+  SbddArgs r{};
+  r.x4 = x4; r.graph_ptr = graph_ptr; r.lig_node = lig_node; r.n_lig = n_lig;
+  r.num_classes = K; r.n_graphs = n_graphs; r.logits = logits; r.x_t = x_t; r.c_t = c_t;
+  r.x_noise = x_noise; r.c_noise = c_noise; r.a = coef.a; r.b = coef.b; r.s = coef.s; r.mode = coef.mode;
+  r.x_next = x_next; r.c_next = c_next;
+  return r;
+}
+BpArgs bp_args(const float4* x4, const int* graph_ptr, int n_graphs, const int* lig_node, int n_lig, int K,
+               const cbg_bp_coef& coef, const float* x_pred, const float* logits, const float* x_t, const float* c_t,
+               const unsigned char* gen, const float* pos_noise, const float* type_u, float* x_next, float* c_next,
+               int64_t* v_next, float* eps_out) {
+  BpArgs r{};
+  r.x4 = x4; r.graph_ptr = graph_ptr; r.lig_node = lig_node; r.n_lig = n_lig; r.num_classes = K;
+  r.n_graphs = n_graphs; r.x_pred = x_pred; r.logits = logits; r.x_t = x_t; r.c_t = c_t; r.gen = gen;
+  r.pos_noise = pos_noise; r.type_u = type_u; r.abar = coef.alpha_cumprod; r.beta = coef.beta;
+  r.nonzero = coef.nonzero; r.prob = coef.change_prob; r.x_next = x_next; r.c_next = c_next;
+  r.v_next = (long long*)v_next; r.eps_out = eps_out;
+  return r;
+}
+// argument checks of the per-graph reverse hooks (before any device work)
+int check_graph_hook(const char* fn, bool ptrs_ok, int n_graphs, int n_lig, int num_classes) {
+  if (!ptrs_ok) { cbg_set_error("%s: null argument", fn); return 1; }
+  if (n_graphs < 0 || n_lig < 0) { cbg_set_error("%s: n_graphs=%d n_lig=%d", fn, n_graphs, n_lig); return 1; }
+  if (num_classes < 1 || num_classes > CBG_MAXCLS) {
+    cbg_set_error("%s: num_classes=%d outside [1,%d]", fn, num_classes, CBG_MAXCLS);
+    return 1;
+  }
+  return 0;
+}
+}  // namespace
+
 int32_t cbg_sbdd_step_f32(const cbg_sample_plan* plan, const cbg_sbdd_coef* coef, const float* x_t, const float* c_t,
                           const float* x_noise, const float* c_noise, float* x_next, float* c_next,
                           float* x_pred, float* logits, void* stream) {
@@ -833,12 +869,19 @@ int32_t cbg_sbdd_step_f32(const cbg_sample_plan* plan, const cbg_sbdd_coef* coef
   if (x_pred) {
     if (int rc = cbg_launch_gather_x(ws.x4, plan->lig_node, plan->n_lig, x_pred, st)) return rc;
   }
-  SbddArgs r{};
-  r.x4 = ws.x4; r.graph_ptr = plan->graph_ptr; r.lig_node = plan->lig_node; r.n_lig = plan->n_lig;
-  r.num_classes = K; r.n_graphs = plan->n_graphs; r.logits = lg; r.x_t = x_t; r.c_t = c_t;
-  r.x_noise = x_noise; r.c_noise = c_noise; r.a = coef->a; r.b = coef->b; r.s = coef->s; r.mode = coef->mode;
-  r.x_next = x_next; r.c_next = c_next;
-  return cbg_launch_sbdd_reverse(r, st);
+  return cbg_launch_sbdd_reverse(sbdd_args(ws.x4, plan->graph_ptr, plan->n_graphs, plan->lig_node, plan->n_lig, K, *coef,
+                                           lg, x_t, c_t, x_noise, c_noise, x_next, c_next), st);
+}
+
+int32_t cbg_sbdd_reverse_f32(float* x4, const int32_t* graph_ptr, int32_t n_graphs, const int32_t* lig_node, int32_t n_lig,
+                             int32_t num_classes, const cbg_sbdd_coef* coef, const float* logits, const float* x_t,
+                             const float* c_t, const float* x_noise, const float* c_noise, float* x_next, float* c_next,
+                             void* stream) {
+  if (int rc = check_graph_hook("cbg_sbdd_reverse_f32", x4 && graph_ptr && lig_node && coef && logits && x_t && c_t &&
+                                x_noise && c_noise && x_next && c_next, n_graphs, n_lig, num_classes)) return rc;
+  if (coef->mode != 0 && coef->mode != 1) { cbg_set_error("cbg_sbdd_reverse_f32: mode=%d is not 0 or 1", coef->mode); return 1; }
+  return cbg_launch_sbdd_reverse(sbdd_args((float4*)x4, graph_ptr, n_graphs, lig_node, n_lig, num_classes, *coef, logits,
+                                           x_t, c_t, x_noise, c_noise, x_next, c_next), (cudaStream_t)stream);
 }
 
 int32_t cbg_bp_step_f32(const cbg_sample_plan* plan, const float* com_blob, int32_t com_layers, const cbg_bp_coef* coef,
@@ -854,13 +897,22 @@ int32_t cbg_bp_step_f32(const cbg_sample_plan* plan, const float* com_blob, int3
   const BpScratch s = bp_scratch(ws, n_lig, K);
   float* lg = logits ? logits : s.logits;
   if (int rc = run_bp_denoiser(*plan, com_blob, com_layers, ws, x_t, lg, s.x_pred, st)) return rc;
-  BpArgs r{};
-  r.x4 = ws.x4; r.graph_ptr = plan->graph_ptr; r.lig_node = plan->lig_node; r.n_lig = n_lig; r.num_classes = K;
-  r.n_graphs = plan->n_graphs; r.x_pred = s.x_pred; r.logits = lg; r.x_t = x_t; r.c_t = c_t; r.gen = plan->gen_lig;
-  r.pos_noise = pos_noise; r.type_u = type_uniform; r.abar = coef->alpha_cumprod; r.beta = coef->beta;
-  r.nonzero = coef->nonzero; r.prob = coef->change_prob; r.x_next = x_next; r.c_next = c_next;
-  r.v_next = (long long*)v_next; r.eps_out = eps_out;
-  return cbg_launch_bp_reverse(r, st);
+  return cbg_launch_bp_reverse(bp_args(ws.x4, plan->graph_ptr, plan->n_graphs, plan->lig_node, n_lig, K, *coef, s.x_pred,
+                                       lg, x_t, c_t, plan->gen_lig, pos_noise, type_uniform, x_next, c_next, v_next,
+                                       eps_out), st);
+}
+
+int32_t cbg_bp_reverse_f32(const float* x4, const int32_t* graph_ptr, int32_t n_graphs, const int32_t* lig_node,
+                           int32_t n_lig, int32_t num_classes, const cbg_bp_coef* coef, const float* x_pred,
+                           const float* logits, const float* x_t, const float* c_t, const uint8_t* gen,
+                           const float* pos_noise, const float* type_uniform, float* x_next, float* c_next,
+                           int64_t* v_next, float* eps_out, void* stream) {
+  if (int rc = check_graph_hook("cbg_bp_reverse_f32", x4 && graph_ptr && lig_node && coef && x_pred && logits && x_t &&
+                                c_t && gen && pos_noise && type_uniform && x_next && c_next && v_next,
+                                n_graphs, n_lig, num_classes)) return rc;
+  return cbg_launch_bp_reverse(bp_args((const float4*)x4, graph_ptr, n_graphs, lig_node, n_lig, num_classes, *coef, x_pred,
+                                       logits, x_t, c_t, gen, pos_noise, type_uniform, x_next, c_next, v_next, eps_out),
+                               (cudaStream_t)stream);
 }
 
 int32_t cbg_bp_eval_loss_f32(const cbg_sample_plan* plan, const float* com_blob, int32_t com_layers,
@@ -890,7 +942,11 @@ int32_t cbg_reverse_step_f32(const cbg_step_coef* coef, const float* x0_pred, co
                              const float* c_t, const uint8_t* gen, const float* pos_noise, const float* type_uniform,
                              int32_t n, int32_t num_classes, float* x_next, float* c_next, int64_t* v_next,
                              void* stream) {
-  if (!coef) { cbg_set_error("null coef"); return 1; }
+  if (!(coef && x0_pred && logits && x_t && c_t && gen && pos_noise && type_uniform && x_next && c_next && v_next)) {
+    cbg_set_error("cbg_reverse_step_f32: null argument");
+    return 1;
+  }
+  if (n < 0) { cbg_set_error("cbg_reverse_step_f32: n=%d", n); return 1; }
   if (num_classes < 1 || num_classes > CBG_MAXCLS) { cbg_set_error("num_classes=%d outside [1,%d]", num_classes, CBG_MAXCLS); return 1; }
   ReverseArgs r{};
   r.x0 = x0_pred; r.x0_stride = 3; r.x0_idx = nullptr;

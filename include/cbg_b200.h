@@ -254,7 +254,7 @@ int32_t cbg_eval_loss_f32(const cbg_sample_plan* plan, const cbg_eval_coef* coef
                           float* xt, int64_t* vt, float* x_pred, float* c_pred, float* graph_loss, float* rep_loss,
                           void* stream);
 
-/* the reverse step alone (testing / integration hook) */
+/* the reverse step alone (testing / integration hook); refuses NULL pointers and n < 0 before touching the device */
 int32_t cbg_reverse_step_f32(const cbg_step_coef* coef, const float* x0_pred /*[n,3]*/, const float* logits /*[n,K]*/,
                              const float* x_t, const float* c_t, const uint8_t* gen /*[n]*/,
                              const float* pos_noise, const float* type_uniform,
@@ -281,6 +281,20 @@ int32_t cbg_sbdd_step_f32(const cbg_sample_plan* plan, const cbg_sbdd_coef* coef
                           float* x_next /*[n_lig,3]*/, float* c_next /*[n_lig,K]*/,
                           float* x_pred /*[n_lig,3] or NULL*/, float* logits /*[n_lig,K] or NULL*/, void* stream);
 
+/* The DiffSBDD reverse step alone (testing hook): the kernel of cbg_sbdd_step_f32 on caller-given rows.  x4 [N,4] holds
+ * the node coordinates and the flag float (bit 0 = ligand): its ligand rows are the denoiser's output coordinates
+ * eps_pred, its pocket rows (bit 0 clear) are shifted in place by their graph's ligand mean.  Graph g owns the nodes
+ * [graph_ptr[g], graph_ptr[g + 1]); lig_node [n_lig] must be ascending and every entry must lie inside the node range
+ * of the graph it belongs to.  The pocket of a graph without ligand atoms is not moved (its mean is taken as 0).
+ * Refuses NULL pointers, num_classes outside [1, 16], n_graphs < 0, n_lig < 0 and a mode other than 0 / 1 before
+ * touching the device. */
+int32_t cbg_sbdd_reverse_f32(float* x4 /*[N,4]*/, const int32_t* graph_ptr /*[n_graphs+1]*/, int32_t n_graphs,
+                             const int32_t* lig_node /*[n_lig]*/, int32_t n_lig, int32_t num_classes,
+                             const cbg_sbdd_coef* coef, const float* logits /*[n_lig,K]*/,
+                             const float* x_t /*[n_lig,3]*/, const float* c_t /*[n_lig,K]*/,
+                             const float* x_noise /*[n_lig,3]*/, const float* c_noise /*[n_lig,K]*/,
+                             float* x_next /*[n_lig,3]*/, float* c_next /*[n_lig,K]*/, void* stream);
+
 /* DiffBP (diffbp.py:240-299): embed -> denoiser -> CoM head (CoMPredictor, diffbp.py:30-101: the step's kNN graph,
  * its own edge gate, com_layers x H2X on the denoiser's final h starting from the step's input coordinates) ->
  * CTNVPScheduler.backward_remove_noise(type='score') (diffusion_scheduler.py:144-165) on eps + eps_com and
@@ -299,6 +313,19 @@ int32_t cbg_bp_step_f32(const cbg_sample_plan* plan, const float* com_blob, int3
                         float* x_next /*[n_lig,3]*/, float* c_next /*[n_lig,K]*/, int64_t* v_next /*[n_lig]*/,
                         float* eps_out /*[n_lig,3] or NULL: eps + eps_com*/, float* logits /*[n_lig,K] or NULL*/,
                         void* stream);
+
+/* The DiffBP reverse step alone (testing hook): the kernel of cbg_bp_step_f32 on caller-given rows.  x4 [N,4] as in
+ * cbg_sbdd_reverse_f32, its ligand rows holding x_com (the CoM head's output coordinates); it is only read.  graph_ptr /
+ * lig_node as in cbg_sbdd_reverse_f32 (ascending, inside the graphs' node ranges).  x_pred: the denoiser's output
+ * coordinates [n_lig,3]; type_uniform [n_lig]; eps_out may be NULL.  Refuses NULL pointers (other than eps_out),
+ * num_classes outside [1, 16], n_graphs < 0 and n_lig < 0 before touching the device. */
+int32_t cbg_bp_reverse_f32(const float* x4 /*[N,4]*/, const int32_t* graph_ptr /*[n_graphs+1]*/, int32_t n_graphs,
+                           const int32_t* lig_node /*[n_lig]*/, int32_t n_lig, int32_t num_classes,
+                           const cbg_bp_coef* coef, const float* x_pred /*[n_lig,3]*/, const float* logits /*[n_lig,K]*/,
+                           const float* x_t /*[n_lig,3]*/, const float* c_t /*[n_lig,K]*/, const uint8_t* gen /*[n_lig]*/,
+                           const float* pos_noise /*[n_lig,3]*/, const float* type_uniform /*[n_lig]*/,
+                           float* x_next /*[n_lig,3]*/, float* c_next /*[n_lig,K]*/, int64_t* v_next /*[n_lig]*/,
+                           float* eps_out /*[n_lig,3] or NULL*/, void* stream);
 
 /* ---- validation loss: DiffBP.forward in eval mode (diffbp.py:133-230) ------------------------------------------------
  *

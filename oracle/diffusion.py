@@ -82,35 +82,55 @@ def log_add_exp(a, b):
     return m + torch.log(torch.exp(a - m) + torch.exp(b - m))
 
 
-def pos_reverse_step(sd, x0_pred, x_t, t_idx, gen_flag, noise, prefix='pos_scheduler.'):
-    """CTNVPScheduler.backward_remove_noise(type='denoise'), all graphs at the same t."""
-    c0 = sd[prefix + 'posterior_mean_c0_coef'][t_idx]
-    ct = sd[prefix + 'posterior_mean_ct_coef'][t_idx]
-    logvar = sd[prefix + 'posterior_logvar'][t_idx]
-    nonzero = 0.0 if t_idx == 0 else 1.0
-    mean = c0 * x0_pred + ct * x_t
-    xs = mean + nonzero * (0.5 * logvar).exp() * noise
+def _scalar(v, dtype):
+    return torch.as_tensor(v, dtype=dtype)
+
+
+def pos_reverse_update(x0_pred, x_t, c0, ct, logvar, nonzero, gen_flag, noise):
+    """The position update of CTNVPScheduler.backward_remove_noise(type='denoise') for the step's scalars
+    (posterior_mean_c0_coef[t], posterior_mean_ct_coef[t], posterior_logvar[t], 0 at t == 0 else 1), in the dtype of
+    ``x_t``: fp32 is the reference's expression, float64 a high-precision reference of it on the same inputs."""
+    dt = x_t.dtype
+    c0, ct, logvar, nonzero = (_scalar(v, dt) for v in (c0, ct, logvar, nonzero))
+    mean = c0 * x0_pred.to(dt) + ct * x_t
+    xs = mean + nonzero * (0.5 * logvar).exp() * noise.to(dt)
     return torch.where(gen_flag.unsqueeze(-1), xs, x_t)
 
 
-def type_reverse_step(sd, logits, c_t, t_idx, gen_flag, uniform, num_classes, prefix='type_scheduler.'):
-    """TypeVPScheduler.backward_remove_noise(pred_logit=True)."""
+def pos_reverse_step(sd, x0_pred, x_t, t_idx, gen_flag, noise, prefix='pos_scheduler.'):
+    """CTNVPScheduler.backward_remove_noise(type='denoise'), all graphs at the same t."""
+    return pos_reverse_update(x0_pred, x_t, sd[prefix + 'posterior_mean_c0_coef'][t_idx],
+                              sd[prefix + 'posterior_mean_ct_coef'][t_idx], sd[prefix + 'posterior_logvar'][t_idx],
+                              0.0 if t_idx == 0 else 1.0, gen_flag, noise)
+
+
+def type_reverse_update(logits, c_t, lac, l1mac, la, l1ma, gen_flag, uniform, num_classes):
+    """The type update of TypeVPScheduler.backward_remove_noise(pred_logit=True) for the step's scalars
+    (log_alphas_cumprod_v / log_one_minus_alphas_cumprod_v at max(t - 1, 0), log_alphas_v / log_one_minus_alphas_v at
+    t), in the dtype of ``logits``.  -> (one-hot c_next, v_next, Gumbel score gumbel + log posterior)."""
     K = num_classes
+    dt = logits.dtype
+    lac, l1mac, la, l1ma = (_scalar(v, dt) for v in (lac, l1mac, la, l1ma))
+    c_t, uniform = c_t.to(dt), uniform.to(dt)
     log_c_pred = F.log_softmax(logits, dim=-1)
     log_ct = torch.log(c_t + 1e-8)
-    tm1 = max(t_idx - 1, 0)
-    lac = sd[prefix + 'log_alphas_cumprod_v'][tm1]
-    l1mac = sd[prefix + 'log_one_minus_alphas_cumprod_v'][tm1]
-    la = sd[prefix + 'log_alphas_v'][t_idx]
-    l1ma = sd[prefix + 'log_one_minus_alphas_v'][t_idx]
     log_qvt1_v0 = log_add_exp(log_c_pred + lac, l1mac - np.log(K))
     log_qvs1_vt = log_add_exp(log_ct + la, l1ma - np.log(K))
     un = log_qvt1_v0 + log_qvs1_vt
     log_post = un - torch.logsumexp(un, dim=-1, keepdim=True)
     gumbel = -torch.log(-torch.log(uniform + 1e-30) + 1e-30)
-    v_next = (gumbel + log_post).argmax(dim=-1)
-    v_next = torch.where(gen_flag, v_next, c_t.argmax(-1))
-    return F.one_hot(v_next, num_classes=K).float(), v_next
+    score = gumbel + log_post
+    v_next = torch.where(gen_flag, score.argmax(dim=-1), c_t.argmax(-1))
+    return F.one_hot(v_next, num_classes=K).float(), v_next, score
+
+
+def type_reverse_step(sd, logits, c_t, t_idx, gen_flag, uniform, num_classes, prefix='type_scheduler.'):
+    """TypeVPScheduler.backward_remove_noise(pred_logit=True)."""
+    tm1 = max(t_idx - 1, 0)
+    c_next, v_next, _ = type_reverse_update(
+        logits, c_t, sd[prefix + 'log_alphas_cumprod_v'][tm1], sd[prefix + 'log_one_minus_alphas_cumprod_v'][tm1],
+        sd[prefix + 'log_alphas_v'][t_idx], sd[prefix + 'log_one_minus_alphas_v'][t_idx], gen_flag, uniform, num_classes)
+    return c_next, v_next
 
 
 def context_embed(sd, c_lig, v_rec, aa_rec, lig_flag, rec_flag, prefix='context_embedder.'):

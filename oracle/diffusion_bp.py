@@ -37,8 +37,6 @@ def num_com_layers(sd, prefix='com_head.'):
 
 def com_head(sd, x_lig_pred, bl, x, h, gen, lig, batch_idx, k=32, prefix='com_head.'):
     """CoMPredictor.forward (diffbp.py:80-101) on composed tensors."""
-    noise = x_lig_pred - x[lig]
-    noise = noise - G.scatter_mean(noise, bl, dim=0)[bl]
     ptr = G.graph_ptr_from_batch(batch_idx)
     nbr = G.neighbor_table(x, ptr, k=k)
     src, dst = G.table_to_edge_index(nbr)
@@ -48,15 +46,25 @@ def com_head(sd, x_lig_pred, bl, x, h, gen, lig, batch_idx, k=32, prefix='com_he
     for l in range(num_com_layers(sd, prefix)):
         dx = h2x_attention(sd, prefix + f'h2xattentions.{l}.', x_out, h, src, dst, etype, e_w)
         x_out = x_out + dx * gen.unsqueeze(-1).to(x.dtype)
-    delta = (x_out - x)[lig]
-    return noise, G.scatter_mean(delta, bl, dim=0)[bl]
+    return com_eps(x_lig_pred, x[lig], x_out[lig], bl)
 
 
-def pos_reverse_step_score(sd, eps, x_t, t_idx, gen_flag, noise, prefix='pos_scheduler.'):
-    """CTNVPScheduler.backward_remove_noise(type='score'), all graphs at the same t."""
-    a = sd[prefix + 'alphas_cumprod'][t_idx]
-    b = sd[prefix + 'betas'][t_idx]
-    nonzero = 0.0 if t_idx == 0 else 1.0
+def com_eps(x_pred, x_t, x_com, bl, num_graphs=None):
+    """The two outputs of CoMPredictor.forward (diffbp.py:80-101) on the ligand rows, in the dtype of the inputs:
+    the zero-mean noise prediction (x_pred - x_t) - mean_g(x_pred - x_t) and the per-graph shift mean_g(x_com - x_t),
+    where x_com are the CoM head's output coordinates.  ``num_graphs`` sizes the per-graph tables."""
+    noise = x_pred - x_t
+    noise = noise - G.scatter_mean(noise, bl, dim=0, dim_size=num_graphs)[bl]
+    delta = x_com - x_t
+    return noise, G.scatter_mean(delta, bl, dim=0, dim_size=num_graphs)[bl]
+
+
+def pos_score_update(eps, x_t, abar, beta, nonzero, gen_flag, noise):
+    """The position update of CTNVPScheduler.backward_remove_noise(type='score') for the step's scalars
+    (alphas_cumprod[t], betas[t], 0 at t == 0 else 1), in the dtype of ``x_t``."""
+    dt = x_t.dtype
+    a, b, nonzero = (torch.as_tensor(v, dtype=dt) for v in (abar, beta, nonzero))
+    eps, noise = eps.to(dt), noise.to(dt)
     sigma = (1 - a).sqrt()
     score = -eps / sigma
     xs = (x_t + b * score) / (1 - b).sqrt()
@@ -64,15 +72,29 @@ def pos_reverse_step_score(sd, eps, x_t, t_idx, gen_flag, noise, prefix='pos_sch
     return torch.where(gen_flag.unsqueeze(-1), xs, x_t)
 
 
-def mask_type_reverse_step(logits, c_t, t_idx, num_steps, gen_flag, uniform, num_classes):
-    """MaskTypeSchedule.backward_remove_noise(pred_logit=True, fix_pred=True)."""
+def pos_reverse_step_score(sd, eps, x_t, t_idx, gen_flag, noise, prefix='pos_scheduler.'):
+    """CTNVPScheduler.backward_remove_noise(type='score'), all graphs at the same t."""
+    return pos_score_update(eps, x_t, sd[prefix + 'alphas_cumprod'][t_idx], sd[prefix + 'betas'][t_idx],
+                            0.0 if t_idx == 0 else 1.0, gen_flag, noise)
+
+
+def mask_type_update(logits, c_t, prob, gen_flag, uniform, num_classes):
+    """MaskTypeSchedule.backward_remove_noise(pred_logit=True, fix_pred=True) for the change probability ``prob`` of
+    the step, in the dtype of ``logits``.  -> (one-hot c_next, v_next, softmax(logits))."""
+    dt = logits.dtype
     c_pred = F.softmax(logits, dim=-1)
     vt = c_t.argmax(-1)
+    change = (uniform.to(dt) < torch.as_tensor(prob, dtype=dt)) & gen_flag & (vt == ABSORBING_STATE)
+    v_next = torch.where(change, c_pred.argmax(-1), vt)
+    return F.one_hot(v_next, num_classes=num_classes).float(), v_next, c_pred
+
+
+def mask_type_reverse_step(logits, c_t, t_idx, num_steps, gen_flag, uniform, num_classes):
+    """MaskTypeSchedule.backward_remove_noise(pred_logit=True, fix_pred=True)."""
     t = torch.full((c_t.shape[0],), t_idx, dtype=torch.long)
     prob = ((num_steps - t) / num_steps).clamp(max=1., min=0.)
-    change = (uniform < prob) & gen_flag & (vt == ABSORBING_STATE)
-    v_next = torch.where(change, c_pred.argmax(-1), vt)
-    return F.one_hot(v_next, num_classes=num_classes).float(), v_next
+    c_next, v_next, _ = mask_type_update(logits, c_t, prob, gen_flag, uniform, num_classes)
+    return c_next, v_next
 
 
 def denoise(sd, batch, x_lig, c_lig, k=32):

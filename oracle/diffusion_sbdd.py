@@ -73,9 +73,24 @@ def final_scalars(gamma, timesteps):
     return torch.sqrt(torch.sigmoid(-g0))[0], torch.sqrt(torch.sigmoid(g0))[0], torch.exp(0.5 * g0)[0]
 
 
-def remove_mean_batch(x_lig, x_rec, bl, br):
-    mean = G.scatter_mean(x_lig, bl, dim=0)
+def remove_mean_batch(x_lig, x_rec, bl, br, num_graphs=None):
+    """diffusion_scheduler.py:706-710.  ``num_graphs`` sizes the mean table: without it a trailing graph without ligand
+    atoms indexes past the table when its pocket is moved (the reference's own behaviour); with it such a graph's
+    mean is 0 and its pocket does not move."""
+    mean = G.scatter_mean(x_lig, bl, dim=0, dim_size=num_graphs)
     return x_lig - mean[bl], x_rec - mean[br]
+
+
+def reverse_update(z_t, eps, a, b, s, noise, mode=0):
+    """z_s before the COM projection, for the step's scalars, in the dtype of ``z_t``:
+    mode 0  sample_p_zs_given_zt (a = alpha_t|s, b = sigma2_t|s / alpha_t|s / sigma_t, s = sigma_t|s sigma_s / sigma_t):
+            z_t / a - b eps + s noise
+    mode 1  sample_p_xh_given_z0 (a = 1 / alpha_0, b = sigma_0, s = exp(0.5 gamma_0)): a (z_t - b eps) + s noise."""
+    dt = z_t.dtype
+    a, b, s = (torch.as_tensor(v, dtype=dt) for v in (a, b, s))
+    eps, noise = eps.to(dt), noise.to(dt)
+    mu = z_t / a - b * eps if mode == 0 else a * (z_t - b * eps)
+    return mu + s * noise
 
 
 def denoise(sd, batch, x_lig, c_lig, x_rec, v_rec, k, cutoff_mode, r_max):
@@ -112,9 +127,9 @@ def sample(sd, batch, num_steps, noise, num_classes=13, k=32, cutoff_mode='knn',
         x_lig, c_lig = traj[t_idx]
         x_pred, c_out = denoise(sd, batch, x_lig, c_lig, x_rec, v_rec, k, cutoff_mode, r_max)
         a_ts, k_eps, sig = step_scalars(gamma, t_idx, T)
-        zs = x_lig / a_ts - k_eps * x_pred + sig * noise['step_x'][t_idx]
+        zs = reverse_update(x_lig, x_pred, a_ts, k_eps, sig, noise['step_x'][t_idx])
         x_next, x_rec = remove_mean_batch(zs, x_rec, bl, br)
-        c_next = c_lig / a_ts - k_eps * c_out + sig * noise['step_c'][t_idx]
+        c_next = reverse_update(c_lig, c_out, a_ts, k_eps, sig, noise['step_c'][t_idx])
         traj[t_idx - 1] = (x_next, c_next)
         done += 1
         if stop_after is not None and done >= stop_after:
@@ -124,7 +139,7 @@ def sample(sd, batch, num_steps, noise, num_classes=13, k=32, cutoff_mode='knn',
         x_lig, c_lig = traj[-1]
         x_pred, _ = denoise(sd, batch, x_lig, c_lig, x_rec, v_rec, k, cutoff_mode, r_max)
         alpha0, sigma0, sigma_x = final_scalars(gamma, T)
-        mu_x = 1.0 / alpha0 * (x_lig - sigma0 * x_pred)
-        x_fin, _ = remove_mean_batch(mu_x + sigma_x * noise['final_x'], x_rec, bl, br)
+        zs = reverse_update(x_lig, x_pred, 1.0 / alpha0, sigma0, sigma_x, noise['final_x'], mode=1)
+        x_fin, _ = remove_mean_batch(zs, x_rec, bl, br)
         traj[0] = (x_fin, c_lig * TYPE_NORM)
     return traj, x_rec
