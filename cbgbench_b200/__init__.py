@@ -19,7 +19,7 @@ from .modules import UniTransformerB200, get_e3_gnn  # noqa: F401
 from .targetdiff import TargetDiffB200, get_model, register_model  # noqa: F401
 from .diffsbdd import DiffSBDDB200  # noqa: F401
 from .diffbp import DiffBPB200  # noqa: F401
-from .difffg import D3FGB200  # noqa: F401
+from .difffg import D3FGB200, D3FGV2B200  # noqa: F401
 from .batch_builder import DeviceBatchBuilder, SizePrior  # noqa: F401
 
 __version__ = '0.1.0'

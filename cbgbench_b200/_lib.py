@@ -85,6 +85,17 @@ class FgCoef(C.Structure):
                 ('log_alpha', C.c_float), ('log_one_minus_alpha', C.c_float)]
 
 
+class FgEvalCoef(C.Structure):
+    _fields_ = [('t', C.c_int32), ('pos_sqrt_alphas_cumprod', C.c_float), ('pos_sqrt_one_minus_alphas_cumprod', C.c_float),
+                ('rot_sqrt_alphas_cumprod', C.c_float), ('rot_std', C.c_float), ('rot_gaussian', C.c_int32),
+                ('log_alphas_cumprod', C.c_float), ('log_one_minus_alphas_cumprod', C.c_float),
+                ('log_alphas_cumprod_prev', C.c_float), ('log_one_minus_alphas_cumprod_prev', C.c_float),
+                ('log_alpha', C.c_float), ('log_one_minus_alpha', C.c_float), ('t_is_zero', C.c_int32)]
+
+
+FG_LOSS_SCORE, FG_LOSS_DENOISE = 0, 1     # cbg_fg_eval_loss_f32 loss_form (include/cbg_b200.h: CBG_FG_LOSS_*)
+
+
 _P, _I32, _I64, _F, _SZ = C.c_void_p, C.c_int32, C.c_int64, C.c_float, C.c_size_t
 
 # name -> (restype, argtypes); must list every symbol of include/cbg_b200.h
@@ -147,6 +158,7 @@ SIGNATURES = {
     'cbg_fg_workspace_bytes': (_I64, [_I64, _I32, _I32]),
     'cbg_fg_step_f32': (_I32, [C.POINTER(FgPlan), FgCoef, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     'cbg_fg_reverse_f32': (_I32, [C.POINTER(FgPlan), FgCoef] + [_P] * 14),
+    'cbg_fg_eval_loss_f32': (_I32, [C.POINTER(FgPlan), C.POINTER(FgEvalCoef), _I32, _I32] + [_P] * 17),
     'cbg_reverse_step_f32': (_I32, [C.POINTER(StepCoef), _P, _P, _P, _P, _P, _P, _P, _I32, _I32, _P, _P, _P, _P]),
     'cbg_sbdd_reverse_f32': (_I32, [_P, _P, _I32, _P, _I32, _I32, C.POINTER(SbddCoef)] + [_P] * 8),
     'cbg_bp_reverse_f32': (_I32, [_P, _P, _I32, _P, _I32, _I32, C.POINTER(BpCoef)] + [_P] * 12),

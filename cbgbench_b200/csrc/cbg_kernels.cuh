@@ -381,3 +381,63 @@ __device__ __forceinline__ void rotation_to_so3vec(const float* R, float* w) {
 #pragma unroll
   for (int e = 0; e < 3; ++e) w[e] = sg * (n[e] / rn);
 }
+
+// ---- D3FG per-FG helpers shared by fg.cu (reverse step) and fg_eval.cu (validation loss): one warp per functional
+// group, lane k holding class k ------------------------------------------------------------------------------------------
+__device__ __forceinline__ float fg_log_add_exp(float a, float b) {      // categorical.py: log_add_exp
+  const float m = fmaxf(a, b);
+  return m + logf(expf(a - m) + expf(b - m));
+}
+
+__device__ __forceinline__ float fg_warp_max(float v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(CBG_FULL, v, o));
+  return v;
+}
+
+__device__ __forceinline__ float fg_warp_sum(float v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(CBG_FULL, v, o);
+  return v;
+}
+
+// torch.argmax over the lanes: the largest value, the lowest index among equal values
+__device__ __forceinline__ int fg_warp_argmax(float v, int idx) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const float ov = __shfl_xor_sync(CBG_FULL, v, o);
+    const int oi = __shfl_xor_sync(CBG_FULL, idx, o);
+    if (ov > v || (ov == v && oi < idx)) { v = ov; idx = oi; }
+  }
+  return idx;
+}
+
+// The rotation noise e = normalize(axis) * theta of random_normal_so3 (so3.py:140-146) for one FG, with theta drawn
+// by ApproxAngularDistribution.sample (:111-138) from the distribution whose tables are angle_x [T,n_bins] /
+// angle_cdf [T,n_bins-1]: |2 std + std n| mod pi when `gaussian`, else the histogram bin
+// b = min{i : C_t[i] > u C_t[n_bins - 2]} (the definition of the multinomial draw) and X[b] + u' (X[b+1] - X[b]).
+// rd = axis N(0,1)^3 | bin uniform u | in-bin uniform u' | Gaussian-branch N(0,1) n.  Returns theta.
+__device__ __forceinline__ float fg_draw_rotation(const float* rd, int t, float std, bool gaussian,
+                                                  const float* angle_x, const double* angle_cdf, int n_bins,
+                                                  float (&e)[3]) {
+  float theta;
+  if (gaussian) {
+    theta = fmodf(fabsf(__fadd_rn(std * 2.f, __fmul_rn(rd[5], std))), 3.14159265358979323846f);
+  } else {
+    const int nc = n_bins - 1;
+    const double* C = angle_cdf + (size_t)t * nc;
+    const double target = (double)rd[3] * C[nc - 1];
+    int lo = 0, hi = nc - 1;
+    while (lo < hi) {
+      const int mid = (lo + hi) >> 1;
+      if (C[mid] > target) hi = mid; else lo = mid + 1;
+    }
+    const float* X = angle_x + (size_t)t * n_bins;
+    theta = __fadd_rn(X[lo], __fmul_rn(rd[4], __fsub_rn(X[lo + 1], X[lo])));
+  }
+  // F.normalize: a / max(|a|, 1e-12); norm3df does not overflow for |a| up to FLT_MAX (axis draws of 1e30)
+  const float nrm = fmaxf(norm3df(rd[0], rd[1], rd[2]), 1e-12f);
+#pragma unroll
+  for (int c = 0; c < 3; ++c) e[c] = __fmul_rn(__fdiv_rn(rd[c], nrm), theta);
+  return theta;
+}

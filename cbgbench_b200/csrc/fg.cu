@@ -14,34 +14,6 @@
 
 namespace {
 
-__device__ __forceinline__ float fg_log_add_exp(float a, float b) {      // categorical.py: log_add_exp
-  const float m = fmaxf(a, b);
-  return m + logf(expf(a - m) + expf(b - m));
-}
-
-__device__ __forceinline__ float fg_warp_max(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(CBG_FULL, v, o));
-  return v;
-}
-
-__device__ __forceinline__ float fg_warp_sum(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(CBG_FULL, v, o);
-  return v;
-}
-
-// torch.argmax over the lanes: the largest value, the lowest index among equal values
-__device__ __forceinline__ int fg_warp_argmax(float v, int idx) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    const float ov = __shfl_xor_sync(CBG_FULL, v, o);
-    const int oi = __shfl_xor_sync(CBG_FULL, idx, o);
-    if (ov > v || (ov == v && oi < idx)) { v = ov; idx = oi; }
-  }
-  return idx;
-}
-
 __global__ void __launch_bounds__(256) fg_embed_kernel(cbg_fg_plan p, const float* __restrict__ x_t,
                                                        const float* __restrict__ c_t, const float* __restrict__ o_t) {
   const int a = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
@@ -91,26 +63,8 @@ __global__ void __launch_bounds__(256) fg_reverse_kernel(cbg_fg_plan p, cbg_fg_c
     const float* rd = rot_draws + (size_t)a * 6;
     float e[3] = {0.f, 0.f, 0.f};
     float theta = 0.f;
-    if (cf.rot_noise) {
-      if (cf.rot_gaussian) {        // |2 sigma + sigma n| mod pi
-        theta = fmodf(fabsf(__fadd_rn(cf.rot_std * 2.f, __fmul_rn(rd[5], cf.rot_std))), 3.14159265358979323846f);
-      } else {                      // bin b = min{i : C_t[i] > u C_t[n_bins - 2]}, then X[b] + u' (X[b+1] - X[b])
-        const int nc = p.n_bins - 1;
-        const double* C = p.angle_cdf + (size_t)cf.t * nc;
-        const double target = (double)rd[3] * C[nc - 1];
-        int lo = 0, hi = nc - 1;
-        while (lo < hi) {
-          const int mid = (lo + hi) >> 1;
-          if (C[mid] > target) hi = mid; else lo = mid + 1;
-        }
-        const float* X = p.angle_x + (size_t)cf.t * p.n_bins;
-        theta = __fadd_rn(X[lo], __fmul_rn(rd[4], __fsub_rn(X[lo + 1], X[lo])));
-      }
-      // F.normalize: a / max(|a|, 1e-12); norm3df does not overflow for |a| up to FLT_MAX (axis draws of 1e30)
-      const float nrm = fmaxf(norm3df(rd[0], rd[1], rd[2]), 1e-12f);
-#pragma unroll
-      for (int c = 0; c < 3; ++c) e[c] = __fmul_rn(__fdiv_rn(rd[c], nrm), theta);
-    }
+    if (cf.rot_noise)
+      theta = fg_draw_rotation(rd, cf.t, cf.rot_std, cf.rot_gaussian != 0, p.angle_x, p.angle_cdf, p.n_bins, e);
     float E[9], Rp[9], Rn[9], w[3];
     so3vec_to_rotation(e[0], e[1], e[2], E);
     so3vec_to_rotation(in.o_pred[3 * i], in.o_pred[3 * i + 1], in.o_pred[3 * i + 2], Rp);

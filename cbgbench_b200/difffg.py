@@ -1,8 +1,9 @@
-"""CUDA (H100) drop-in for the reference's ``D3FG`` model (``difffg`` / ``difffg_v2``), sampling path. DESIGN.md section 16.
+"""CUDA (H100) drop-in for the reference's ``D3FG`` model (``difffg`` / ``difffg_v2``): sampling (DESIGN.md section 16)
+and the eval-mode validation losses (section 17).
 
 Mirrors repo/models/diffusion/difffg.py:32-63 (constructor, sub-module names => state-dict keys, including the angular
 histograms of the rotation schedule) and :174-246 (``sample(batch) -> traj``).  ``difffg_v2`` differs from ``difffg``
-only in its training loss, so both names build this class.
+only in its position loss: ``D3FGV2B200`` is the same module with the denoise-form loss.
 
 Once per batch, with torch ops on the device: the protein rows of the composed graph (C-alpha positions, backbone frames
 as so3 vectors, FG-type + PerResidueEncoder embeddings), the compose_context permutation and the plan.  Once per model:
@@ -12,6 +13,9 @@ the float64 prefix sums of the inverse angular histograms.  Per reverse step: ON
 Random numbers: per step, in the reference's order, ``randn [n,3]`` (positions), ``randn [n,3]`` (rotation axes),
 ``rand [n]`` (the histogram bin, see ``multinomial_bin``), ``rand [n]`` (offset in the bin), ``randn [n]`` (Gaussian
 branch), ``rand [n,K]`` (Gumbel), from torch's generator of the model device; or injected for parity tests.
+
+Validation losses (difffg.py:65-171): the R eval timesteps noise R copies of the batch, which run as R * B graphs through
+ONE C-ABI call, ``cbg_fg_eval_loss_f32`` (csrc/fg_eval.cu): forward noising, one encoder pass, per-graph losses.
 """
 import ctypes as C
 import math
@@ -23,7 +27,7 @@ import torch.nn.functional as F
 from . import _lib
 from .modules import cfg_get, get_e3_gnn, graph_ptr_from_batch, _Workspace
 from .schedulers import CTNVPTables, TypeVPTables, VPTables
-from .targetdiff import register_model
+from .targetdiff import BaseDiffB200, eval_t_values, register_model
 
 NUM_AA_TYPES = 21          # repo/utils/protein/constants.py:75: len(AA), the width added to num_fgtype by FGContextEmbedder
 NUM_AA_ONEHOT = 20         # len(aa_name_number): the reference one-hots protein_aa with 20 classes (context_emb.py:119)
@@ -81,12 +85,19 @@ class RotVPTables(VPTables):
     def bin_cdf(self, device):
         """Inclusive float64 prefix sums C_t of ``angular_distrib_inv.Y[t, :-1]`` on ``device`` (cached per table
         version).  Summed on the CPU row by row, the same sums the definition of the bin draw uses."""
-        Y = self.angular_distrib_inv.Y
+        return self._prefix_sums('inv', self.angular_distrib_inv.Y, device)
+
+    def fwd_cdf(self, device):
+        """The same prefix sums of ``angular_distrib_fwd.Y``: the forward noising of the validation loss draws its angles
+        from the forward distribution.  Cached separately from ``bin_cdf``."""
+        return self._prefix_sums('fwd', self.angular_distrib_fwd.Y, device)
+
+    def _prefix_sums(self, name, Y, device):
         key = (Y.data_ptr(), Y._version, str(device))
-        if self.__dict__.get('_cdf_key') != key:
-            self.__dict__['_cdf'] = Y.detach().cpu()[:, :-1].double().cumsum(-1).to(device).contiguous()
-            self.__dict__['_cdf_key'] = key
-        return self.__dict__['_cdf']
+        if self.__dict__.get('_cdf_key_' + name) != key:
+            self.__dict__['_cdf_' + name] = Y.detach().cpu()[:, :-1].double().cumsum(-1).to(device).contiguous()
+            self.__dict__['_cdf_key_' + name] = key
+        return self.__dict__['_cdf_' + name]
 
 
 def multinomial_bin(prob, u):
@@ -217,10 +228,12 @@ def backbone_dihedrals(pos, chain_nb, res_nb, mask):
 
 # ---- the model ---------------------------------------------------------------------------------------------------------
 
-@register_model('difffg_v2')
 @register_model('difffg')
 class D3FGB200(nn.Module):
-    """D3FG (difffg.py:32-63, 250-280) with a CUDA sampling path."""
+    """D3FG (difffg.py:32-63, 250-280) with CUDA sampling and validation-loss paths."""
+
+    pos_loss_form = _lib.FG_LOSS_SCORE    # difffg: get_score_loss(score_in=False) (difffg.py:145-148)
+    eval_max_nodes = 1 << 20              # composed nodes per validation-loss launch (about 8 GB at ~7.6 KB/node, H = 256)
 
     def __init__(self, cfg):
         super().__init__()
@@ -245,10 +258,7 @@ class D3FGB200(nn.Module):
         if self.context_embedder.emb_dim != self.denoiser.hidden_dim:
             raise NotImplementedError('D3FGB200: embedder.emb_dim must equal encoder.node_feat_dim')
         self._ws = _Workspace()
-
-    def forward(self, batch):
-        raise NotImplementedError('D3FGB200 builds the sampling path only: the training loss and the eval-mode validation '
-                                  'losses of difffg.py:65-171 are not implemented')
+        self.last_launches = 0
 
     def _device(self):
         dev = next(self.parameters()).device
@@ -258,10 +268,12 @@ class D3FGB200(nn.Module):
 
     # ---- once per batch ------------------------------------------------------------------------------------------------
     @torch.no_grad()
-    def begin(self, batch):
-        """Protein features, composed arrays and the step plan for ``batch`` (the reference's FG batch keys)."""
+    def _context(self, batch):
+        """The batch's tensors on the model's device, checked, and the protein rows of the composed graph.  Computed once
+        per batch: the PerResidueEncoder MLP runs through cuBLAS, whose kernel choice depends on the row count, so the
+        replicas of the validation loss tile these rows instead of recomputing them on a larger batch."""
         dev = self._device()
-        K, H = self.num_classes, self.denoiser.hidden_dim
+        K = self.num_classes
         g = lambda k: batch[k].to(dev)
         xc_lig = g('ligand_pos_heavyatom')[:, BB_CA].float().contiguous()
         v_lig = g('ligand_type_fg').long()
@@ -285,31 +297,49 @@ class D3FGB200(nn.Module):
         xc_rec, o_rec, h_rec = self.context_embedder.protein_features(
             g('protein_pos_heavyatom').float(), g('protein_type_fg').long(), aa, g('protein_res_nb').long(), chain_nb,
             g('protein_mask_heavyatom').bool())
+        return {'device': dev, 'n_lig': n_lig, 'n_rec': n_rec, 'bl': bl, 'br': br, 'xc_lig': xc_lig, 'v_lig': v_lig,
+                'o_lig': o_lig, 'lig_flag': lig_flag, 'rec_flag': rec_flag, 'gen_lig': gen_lig, 'gen_rec': gen_rec,
+                'xc_rec': xc_rec, 'o_rec': o_rec, 'h_rec': h_rec}
+
+    @torch.no_grad()
+    def _compose(self, ctx, n_rep, angular, cdf):
+        """Composed arrays and the plan of ``n_rep`` replicas of the batch of ``ctx``, replica-major: replica r's graph g is
+        graph r * B + g.  The protein rows are written here; the ligand rows of x / o / h are the kernels'.  ``angular``
+        (an ApproxAngularTables) and ``cdf`` (its prefix sums) are the angle tables the plan points at."""
+        dev = ctx['device']
+        K, H = self.num_classes, self.denoiser.hidden_dim
+        bl, br = ctx['bl'], ctx['br']
+        if n_rep == 1:
+            tile = off = lambda v: v
+        else:
+            B = int(torch.cat([br, bl]).max()) + 1
+            steps = torch.arange(n_rep, device=dev).unsqueeze(1) * B
+            tile = lambda v: v.repeat(n_rep, *([1] * (v.dim() - 1)))
+            off = lambda b: (b.unsqueeze(0) + steps).reshape(-1)
+        n_lig, n_rec = ctx['n_lig'] * n_rep, ctx['n_rec'] * n_rep
         # compose_context (common.py:189-214): [protein | ligand] stably sorted by graph id
-        batch_ctx = torch.cat([br, bl])
+        batch_ctx = torch.cat([off(br), off(bl)])
         sort_idx = torch.sort(batch_ctx, stable=True).indices
         inv = torch.empty_like(sort_idx)
         inv[sort_idx] = torch.arange(sort_idx.numel(), device=dev)
         N = n_rec + n_lig
         cat = lambda a, b: torch.cat([a, b])[sort_idx].contiguous()
-        x = cat(xc_rec.float(), xc_lig)
-        o = cat(o_rec.float(), o_lig)
-        h = cat(h_rec.float(), torch.zeros(n_lig, H, device=dev))
-        lig8 = cat(rec_flag, lig_flag).to(torch.uint8)
-        gen8 = cat(gen_rec, gen_lig).to(torch.uint8)
+        x = cat(tile(ctx['xc_rec']).float(), tile(ctx['xc_lig']))
+        o = cat(tile(ctx['o_rec']).float(), tile(ctx['o_lig']))
+        h = cat(tile(ctx['h_rec']).float(), torch.zeros(n_lig, H, device=dev))
+        lig8 = cat(tile(ctx['rec_flag']), tile(ctx['lig_flag'])).to(torch.uint8)
+        gen8 = cat(tile(ctx['gen_rec']), tile(ctx['gen_lig'])).to(torch.uint8)
         gptr, n_graphs, max_n = graph_ptr_from_batch(batch_ctx[sort_idx])
         lig_node = inv[n_rec:].to(torch.int32).contiguous()
         ce = self.context_embedder
         fg_emb_t = ce.ligand_fg_emb.weight.detach()[:, :K].t().float().contiguous()
         fg_emb_b = ce.ligand_fg_emb.bias.detach().float().contiguous()
         lig_ind = ce.ligand_indicator(torch.ones(1, 1, device=dev))[0].float().contiguous()
-        rot = self.rot_scheduler.angular_distrib_inv
-        angle_x = rot.X.detach().float().contiguous()
-        cdf = self.rot_scheduler.bin_cdf(dev)
+        angle_x = angular.X.detach().float().contiguous()
         blob = self.denoiser.packed_blob(dev)
         L = _lib.lib()
         ws_ptr, ws_have = self._ws.get(L.cbg_fg_workspace_bytes(N, H, K), dev)
-        gen_lig8 = gen_lig.to(torch.uint8).contiguous()
+        gen_lig8 = tile(ctx['gen_lig']).to(torch.uint8).contiguous()
         d = self.denoiser
         plan = _lib.FgPlan(blob=blob.data_ptr(), hidden=H, num_sublayers=d.num_layers * d.num_x2h, num_blocks=d.num_blocks,
                       num_classes=K, k=d.cut_off, graph_ptr=gptr.data_ptr(), n_graphs=n_graphs, max_graph_nodes=max_n,
@@ -318,11 +348,19 @@ class D3FGB200(nn.Module):
                       x=x.data_ptr(), o=o.data_ptr(), h=h.data_ptr(), fg_emb_t=fg_emb_t.data_ptr(),
                       fg_emb_b=fg_emb_b.data_ptr(), lig_indicator=lig_ind.data_ptr(), angle_x=angle_x.data_ptr(),
                       angle_cdf=cdf.data_ptr(), n_bins=angle_x.shape[1], workspace=ws_ptr, workspace_bytes=ws_have)
-        c0 = F.one_hot(v_lig, num_classes=K).float()
         # tensors the plan points into stay alive with the state
         keep = (blob, gptr, lig8, gen8, lig_node, gen_lig8, x, o, h, fg_emb_t, fg_emb_b, lig_ind, angle_x, cdf)
-        return {'plan': plan, 'keep': keep, 'device': dev, 'n_lig': n_lig, 'batch_idx_lig': bl,
-                'x0': xc_lig, 'c0': c0, 'o0': o_lig}
+        return {'plan': plan, 'keep': keep, 'device': dev, 'n_lig': n_lig, 'n_graphs': n_graphs, 'n_nodes': N}
+
+    @torch.no_grad()
+    def begin(self, batch):
+        """Protein features, composed arrays and the step plan for ``batch`` (the reference's FG batch keys)."""
+        ctx = self._context(batch)
+        rot = self.rot_scheduler
+        state = self._compose(ctx, 1, rot.angular_distrib_inv, rot.bin_cdf(ctx['device']))
+        state.update(batch_idx_lig=ctx['bl'], x0=ctx['xc_lig'], c0=F.one_hot(ctx['v_lig'], num_classes=self.num_classes).float(),
+                     o0=ctx['o_lig'])
+        return state
 
     # ---- per step ------------------------------------------------------------------------------------------------------
     def step_coef(self, t, rot_std, rot_flag):
@@ -392,3 +430,139 @@ class D3FGB200(nn.Module):
             traj[t] = (Xh[t - t_last], Ch[t - t_last], Oh[t - t_last], bl_cpu)
         traj[t_last - 1] = (X[t_last].clone(), Cc[t_last].clone(), O[t_last].clone(), bl)
         return traj
+
+    # ---- validation losses (D3FG.forward with self.training == False, difffg.py:65-171 / :283-389) -----------------------
+    def forward(self, batch, pos_noise=None, rot_draws=None, type_uniform=None):
+        """The reference's forward in eval mode: ``(loss_dict, results)`` of ``eval_losses`` for the ``eval_interval``
+        (default 10) timesteps ``np.linspace(0, T-1, eval_interval)`` truncated to integers.  Training mode needs autograd
+        through the encoder and raises, as does a model on the CPU."""
+        self._eval_device()
+        t_values = eval_t_values(self.num_diffusion_timesteps, cfg_get(self.cfg, 'eval_interval', 10))
+        return self.eval_losses(batch, t_values, pos_noise=pos_noise, rot_draws=rot_draws, type_uniform=type_uniform)
+
+    def _eval_device(self):
+        name = type(self).__name__
+        if self.training:
+            raise NotImplementedError(f'{name}.forward in training mode needs autograd through the encoder, which the CUDA '
+                                      'path does not provide: training is out of scope (call model.eval() for the '
+                                      'validation losses)')
+        dev = next(self.parameters()).device
+        if dev.type != 'cuda':
+            raise NotImplementedError(f'{name}.forward needs the model on a CUDA device: there is no CPU implementation '
+                                      'of the validation losses')
+        return dev
+
+    def eval_coef(self, t):
+        """Host scalars of the validation loss at timestep t, with the reference's fp32 torch expressions."""
+        ps, rs, ts = self.pos_scheduler, self.rot_scheduler, self.type_scheduler
+        a = torch.tensor(ps.host_table('alphas_cumprod')[t])
+        ar = torch.tensor(rs.host_table('alphas_cumprod')[t])
+        fwd = rs.angular_distrib_fwd
+        tm1 = max(t - 1, 0)
+        tab = ts.host_table
+        return _lib.FgEvalCoef(
+            t=t, pos_sqrt_alphas_cumprod=float(a.sqrt()), pos_sqrt_one_minus_alphas_cumprod=float((1. - a).sqrt()),
+            rot_sqrt_alphas_cumprod=float(torch.sqrt(ar)), rot_std=float(fwd.stddevs[t]),
+            rot_gaussian=int(bool(fwd.approx_flag[t])),
+            log_alphas_cumprod=float(tab('log_alphas_cumprod_v')[t]),
+            log_one_minus_alphas_cumprod=float(tab('log_one_minus_alphas_cumprod_v')[t]),
+            log_alphas_cumprod_prev=float(tab('log_alphas_cumprod_v')[tm1]),
+            log_one_minus_alphas_cumprod_prev=float(tab('log_one_minus_alphas_cumprod_v')[tm1]),
+            log_alpha=float(tab('log_alphas_v')[t]), log_one_minus_alpha=float(tab('log_one_minus_alphas_v')[t]),
+            t_is_zero=1 if t == 0 else 0)
+
+    @torch.no_grad()
+    def eval_losses(self, batch, t_values, pos_noise=None, rot_draws=None, type_uniform=None, max_nodes=None):
+        """Validation losses of ``batch`` at the timesteps ``t_values`` (D3FG.get_loss once per t).  Returns
+        ``(loss_dict, results)`` like the reference's eval-mode forward: ``loss_dict`` = {'pos', 'rot', 'fg'} as CPU 0-d
+        float32 tensors (mean over t of the per-t losses), ``results`` one dict per t of device tensors, keys in the
+        reference's order: eps_0, eps_pred, score_0, score_pred (``difffg``) or x0, xt, x_pred (``difffg_v2``), then
+        mask_gen, v0, vt, c_pred, R0, R_pred.  A t whose batch has no generated FG gets NaN losses.
+
+        The encoder does not see t, so the R = len(t_values) noised copies of the batch run as R * B graphs through ONE
+        encoder pass; above ``max_nodes`` composed nodes (default ``eval_max_nodes``) or 64 copies they are split over
+        several launches, which changes no bit.  ``last_ot`` [R,n,3] keeps the noised orientations and
+        ``last_graph_loss`` [R*B,4] the per-graph pos / rot / fg means and generated-FG counts.
+
+        Draws, all three or none: ``pos_noise`` [R,n,3] N(0,1), ``rot_draws`` [R,n,6] (axis N(0,1)^3, bin uniform,
+        in-bin uniform, Gaussian-branch N(0,1)), ``type_uniform`` [R,n,K] U[0,1).  By default they are drawn with torch on
+        the model device in the reference's order (for each t: randn [n,3], randn [n,3], rand [n], rand [n], randn [n],
+        rand [n,K]; the bin draw stands for ``torch.multinomial``, see ``multinomial_bin``)."""
+        T, K = self.num_diffusion_timesteps, self.num_classes
+        t_values = [int(t) for t in t_values]
+        if not t_values:
+            raise ValueError('t_values is empty')
+        if any(t < 0 or t > T - 1 for t in t_values):
+            raise ValueError(f't_values must lie in [0, {T - 1}]')
+        if (pos_noise is None) != (rot_draws is None) or (pos_noise is None) != (type_uniform is None):
+            raise ValueError('inject pos_noise, rot_draws and type_uniform together, or none of them')
+        bl, br = batch['ligand_type_fg_batch'], batch['protein_type_fg_batch']
+        if bl.numel() and br.numel() and int(br.max()) > int(bl.max()):
+            # the reference sizes t by the last graph with FGs and indexes it with the residues' graph ids (IndexError)
+            raise ValueError('D3FGB200.forward: the last graph of the batch has residues but no functional group')
+        dev = self._eval_device()
+        ctx = self._context(batch)
+        R, n = len(t_values), ctx['n_lig']
+        if pos_noise is None:
+            pos_noise, rot_draws, type_uniform = (torch.empty(R, n, w, device=dev) for w in (3, ROT_DRAWS, K))
+            for r in range(R):
+                pos_noise[r] = torch.randn(n, 3, device=dev)
+                rot_draws[r, :, 0:3] = torch.randn(n, 3, device=dev)
+                rot_draws[r, :, 3] = torch.rand(n, device=dev)
+                rot_draws[r, :, 4] = torch.rand(n, device=dev)
+                rot_draws[r, :, 5] = torch.randn(n, device=dev)
+                type_uniform[r] = torch.rand(n, K, device=dev)
+        to = lambda a, w: a.to(dev, torch.float32).reshape(R, n, w).contiguous()
+        pn, rd, tu = to(pos_noise, 3), to(rot_draws, ROT_DRAWS), to(type_uniform, K)
+        score_form = self.pos_loss_form == _lib.FG_LOSS_SCORE
+        xt, ot, pred = (torch.empty(R, n, 3, device=dev) for _ in range(3))
+        vt = torch.empty(R, n, dtype=torch.int64, device=dev)
+        score = torch.empty(R, 2, n, 3, device=dev) if score_form else None
+        c_pred = torch.empty(R, n, K, device=dev)
+        R_pred = torch.empty(R, n, 3, 3, device=dev)
+        R0 = torch.empty(n, 3, 3, device=dev)
+        rep_loss = torch.empty(R, 3, device=dev)
+        x0, v0, o0 = ctx['xc_lig'], ctx['v_lig'].contiguous(), ctx['o_lig']
+        n_nodes = n + ctx['n_rec']
+        budget = self.eval_max_nodes if max_nodes is None else int(max_nodes)
+        per_launch = max(1, min(_lib.EVAL_MAX_REPLICAS, budget // n_nodes))
+        fwd, cdf = self.rot_scheduler.angular_distrib_fwd, self.rot_scheduler.fwd_cdf(dev)
+        L = _lib.lib()
+        st = _lib.stream_ptr(dev)
+        launches0 = L.cbg_launch_count()
+        graph_loss = []
+        with torch.cuda.device(dev):
+            for r0 in range(0, R, per_launch):
+                r1 = min(R, r0 + per_launch)
+                state = self._compose(ctx, r1 - r0, fwd, cdf)
+                gl = torch.empty(state['n_graphs'], 4, device=dev)
+                coefs = (_lib.FgEvalCoef * (r1 - r0))(*[self.eval_coef(t) for t in t_values[r0:r1]])
+                _lib.check(L.cbg_fg_eval_loss_f32(
+                    C.byref(state['plan']), coefs, r1 - r0, self.pos_loss_form, x0.data_ptr(), v0.data_ptr(),
+                    o0.data_ptr(), pn[r0:r1].data_ptr(), rd[r0:r1].data_ptr(), tu[r0:r1].data_ptr(), xt[r0:r1].data_ptr(),
+                    ot[r0:r1].data_ptr(), vt[r0:r1].data_ptr(), pred[r0:r1].data_ptr(),
+                    score[r0:r1].data_ptr() if score_form else None, c_pred[r0:r1].data_ptr(), R_pred[r0:r1].data_ptr(),
+                    R0.data_ptr(), gl.data_ptr(), rep_loss[r0:r1].data_ptr(), st))
+                graph_loss.append(gl)
+        self.last_launches = L.cbg_launch_count() - launches0
+        self.last_ot = ot
+        self.last_graph_loss = torch.cat(graph_loss)
+        loss_dict = BaseDiffB200._eval_dict_mean(rep_loss, ('pos', 'rot', 'fg'))
+        mask_gen = ctx['gen_lig']
+        results = []
+        for r in range(R):
+            if score_form:
+                res = {'eps_0': pn[r], 'eps_pred': pred[r], 'score_0': score[r, 0], 'score_pred': score[r, 1]}
+            else:
+                res = {'x0': x0, 'xt': xt[r], 'x_pred': pred[r]}
+            res.update({'mask_gen': mask_gen, 'v0': v0, 'vt': vt[r], 'c_pred': c_pred[r], 'R0': R0, 'R_pred': R_pred[r]})
+            results.append(res)
+        return loss_dict, results
+
+
+@register_model('difffg_v2')
+class D3FGV2B200(D3FGB200):
+    """``difffg_v2`` (difffg.py:250-389): the module of ``difffg``; its position loss is get_loss(type='denoise'),
+    ||x_pred - x0||^2 on the encoder's position output (difffg.py:363-365)."""
+
+    pos_loss_form = _lib.FG_LOSS_DENOISE

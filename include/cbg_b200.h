@@ -552,6 +552,56 @@ int32_t cbg_fg_reverse_f32(const cbg_fg_plan* plan, cbg_fg_coef coef, const floa
                            const float* pos_noise, const float* rot_draws, const float* type_u, float* x_next,
                            float* c_next, float* o_next, float* theta, void* stream);
 
+/* ---- validation loss: D3FG.forward in eval mode (`difffg` / `difffg_v2`, difffg.py:65-171 / :283-389) ------------------
+ *
+ * The plan holds n_rep replicas of one batch of B graphs and n1 = n_lig / n_rep functional groups, replica-major: graph
+ * r*B + g and ligand row r*n1 + a are graph g and FG a of the batch, noised at replica r's timestep.  Its protein rows of
+ * x / o / h are written by the host (once per batch, tiled n_rep times); angle_x / angle_cdf point at the FORWARD angular
+ * tables (rot_scheduler.angular_distrib_fwd).  The encoder does not see t, so the replicas share one pass.  One call
+ * enqueues:
+ *   fg_eval_noise_kernel   one warp per (replica, FG): CTNVPScheduler.forward_add_noise (diffusion_scheduler.py:117-134),
+ *                          RotVPScheduler.forward_add_noise (:531-556; o_t = log(exp(e) exp(sqrt(abar_rot) o_0)), e drawn
+ *                          from angular_distrib_fwd, no zeroing at small t) and TypeVPScheduler.forward_add_noise (:339-346,
+ *                          Gumbel-max over q(v_t | v_0)), each only where gen_lig is set, then the ligand rows of x / o / h
+ *   cbg_ipa_launch         the IPATransformer over all n_rep * B graphs
+ *   fg_eval_loss_kernel    one CTA per (replica, graph), over its generated FGs in a fixed order: the position loss
+ *                          (score form: ||eps_pred - eps||^2, get_score_loss; denoise form: ||x_pred - x_0||^2, get_loss),
+ *                          rotation_matrix_cosine_loss (difffg.py:16-31) and the type KL / decoder NLL at t == 0
+ *                          (TypeVPScheduler.get_loss, :348-418)
+ *   fg_eval_reduce_kernel  per replica: scatter_mean(...).mean() over graphs 0 .. (last graph with a generated FG)
+ * No atomics: repeated calls are bit-identical. */
+#define CBG_FG_LOSS_SCORE 0     /* difffg: get_score_loss(score_in=False) on the encoder's eps_pos */
+#define CBG_FG_LOSS_DENOISE 1   /* difffg_v2: get_loss(type='denoise') on the encoder's eps_pos as x_pred */
+
+typedef struct {                 /* one replica's timestep t: the reference's fp32 torch expressions, evaluated on the host */
+  int32_t t;
+  float pos_sqrt_alphas_cumprod;            /* pos_scheduler.alphas_cumprod[t].sqrt() */
+  float pos_sqrt_one_minus_alphas_cumprod;  /* (1 - pos_scheduler.alphas_cumprod[t]).sqrt() */
+  float rot_sqrt_alphas_cumprod;            /* rot_scheduler.alphas_cumprod[t].sqrt() */
+  float rot_std;                            /* angular_distrib_fwd.stddevs[t] = sqrt(1 - rot abar[t]) */
+  int32_t rot_gaussian;                     /* angular_distrib_fwd.approx_flag[t] */
+  float log_alphas_cumprod, log_one_minus_alphas_cumprod;            /* type_scheduler tables at t */
+  float log_alphas_cumprod_prev, log_one_minus_alphas_cumprod_prev;  /* ... at max(t - 1, 0) */
+  float log_alpha, log_one_minus_alpha;                              /* log_alphas_v / log_one_minus_alphas_v at t */
+  int32_t t_is_zero;                        /* 1: the type loss is the decoder NLL instead of the KL */
+} cbg_fg_eval_coef;
+
+/* coefs: host array [n_rep], 1 <= n_rep <= 64; every t must index the plan's angle tables.  loss_form: CBG_FG_LOSS_*.
+ * The batch: x0 [n1,3] (C-alpha of ligand_pos_heavyatom), v0 [n1] (ligand_type_fg), o0 [n1,3] (ligand_o_fg).  Draws from
+ * the caller: pos_noise [n_rep,n1,3] N(0,1), rot_draws [n_rep,n1,6] as for cbg_fg_step_f32, type_u [n_rep,n1,K] U[0,1).
+ * Outputs: xt [n_rep,n1,3]; ot [n_rep,n1,3] or NULL; vt [n_rep,n1]; pred [n_rep,n1,3] (eps_pred or x_pred);
+ * score [n_rep,2,n1,3] = score_0, score_pred (score = eps * sqrt(1 - abar)), required for CBG_FG_LOSS_SCORE, ignored
+ * otherwise; c_pred = softmax(logits) [n_rep,n1,K]; R_pred [n_rep,n1,3,3] (the encoder's R_next); R0 = exp(o0) [n1,3,3];
+ * graph_loss [n_rep*B,4] = per-graph pos, rot, fg means over generated FGs (0 without any) and their count;
+ * rep_loss [n_rep,3] = pos, rot, fg (NaN when no FG is generated).  The plan's workspace is sized by
+ * cbg_fg_workspace_bytes.  Refuses NULL pointers, n_rep, K, a plan that is not n_rep replicas, t < 0 and a missing,
+ * unaligned or small workspace before touching the device. */
+int32_t cbg_fg_eval_loss_f32(const cbg_fg_plan* plan, const cbg_fg_eval_coef* coefs, int32_t n_rep, int32_t loss_form,
+                             const float* x0, const int64_t* v0, const float* o0, const float* pos_noise,
+                             const float* rot_draws, const float* type_u, float* xt, float* ot, int64_t* vt, float* pred,
+                             float* score, float* c_pred, float* R_pred, float* R0, float* graph_loss, float* rep_loss,
+                             void* stream);
+
 #ifdef __cplusplus
 }
 #endif
