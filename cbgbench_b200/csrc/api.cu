@@ -56,8 +56,6 @@ const FieldInfo kLayerFields[] = {
 #undef X
 };
 
-inline size_t align256(size_t v) { return (v + 255) & ~(size_t)255; }
-
 // workspace carve-up
 struct Workspace {
   float4* x4;
@@ -926,7 +924,7 @@ int32_t cbg_bp_eval_loss_f32(const cbg_sample_plan* plan, const float* com_blob,
   if (int rc = open_eval(plan, com_blob && coefs && x0 && v0 && pos_noise && type_uniform && xt && vt && mask && vec &&
                          c_pred && rep_loss, "cbg_bp_eval_loss_f32: null argument", n_rep, 1, x0, v0, &ws, &e.b, st)) return rc;
   if (com_layers < 0 || com_layers > 16) { cbg_set_error("com_layers=%d outside [0,16]", com_layers); return 1; }
-  for (int r = 0; r < n_rep; ++r) e.coef.c[r] = BpEvalCoefDev{coefs[r].alphas_cumprod, coefs[r].beta, coefs[r].mask_prob};
+  for (int r = 0; r < n_rep; ++r) e.coef.c[r] = coefs[r];
   e.n_rep = n_rep; e.pos_noise = pos_noise; e.type_u = type_uniform;
   e.xt = xt; e.vt = (long long*)vt; e.mask = mask; e.vec = vec; e.c_pred = c_pred; e.rep_loss = rep_loss;
   // scratch: the X2H planes are free once the denoiser is done (the CoM head uses the H2X planes)
@@ -967,11 +965,7 @@ int32_t cbg_eval_loss_f32(const cbg_sample_plan* plan, const cbg_eval_coef* coef
   EvalArgs e{};
   if (int rc = open_eval(plan, coefs && x0 && v0 && pos_noise && type_uniform && xt && vt && x_pred && c_pred && graph_loss &&
                          rep_loss, "cbg_eval_loss_f32: null argument", n_rep, 1, x0, v0, &ws, &e.b, st)) return rc;
-  for (int r = 0; r < n_rep; ++r) {
-    const cbg_eval_coef& c = coefs[r];
-    e.coef.c[r] = EvalCoefDev{c.alphas_cumprod, c.log_alphas_cumprod, c.log_one_minus_alphas_cumprod, c.log_alphas_cumprod_prev,
-                              c.log_one_minus_alphas_cumprod_prev, c.log_alpha, c.log_one_minus_alpha, c.t_is_zero ? 1 : 0};
-  }
+  for (int r = 0; r < n_rep; ++r) e.coef.c[r] = coefs[r];
   e.n_rep = n_rep; e.pos_noise = pos_noise; e.type_u = type_uniform;
   e.xt = xt; e.vt = (long long*)vt; e.x_pred = x_pred; e.c_pred = c_pred;
   e.logits = ws.w;                  // classifier scratch: the attention-weight buffer is free after the layers
@@ -996,13 +990,7 @@ int32_t cbg_sbdd_eval_loss_f32(const cbg_sample_plan* plan, const cbg_sbdd_eval_
                          n_t, 2, x0, v0, &ws, &e.b, st)) return rc;
   if (plan->rcache || plan->static_lists) { cbg_set_error("DiffSBDD moves the pocket with every noised copy: the plan must not carry static lists / an R-cache"); return 1; }
   if ((plan->n_nodes - plan->n_lig) % (2 * n_t)) { cbg_set_error("plan (n_nodes=%lld) is not %d replicas of one batch", (long long)plan->n_nodes, 2 * n_t); return 1; }
-  for (int j = 0; j < n_t; ++j) {
-    const cbg_sbdd_eval_coef& c = coefs[j];
-    e.coef.c[j] = SbddEvalCoefDev{c.pos_alpha_t, c.pos_sigma_t, c.type_alpha_t, c.type_sigma_t, c.pos_alpha_0, c.pos_sigma_0,
-                                  c.type_alpha_0, c.type_sigma_0, c.pos_t_weight, c.type_t_weight, c.pos_log_const,
-                                  c.type_log_const, c.pos_alpha_T, c.type_alpha_T, c.pos_log_inv_sigma_T,
-                                  c.type_log_inv_sigma_T, c.pos_sigma2_T, c.type_sigma2_T};
-  }
+  for (int j = 0; j < n_t; ++j) e.coef.c[j] = coefs[j];
   e.n_t = n_t; e.n_nodes = plan->n_nodes; e.x_rec = x_rec;
   e.x_t_noise = x_t_noise; e.c_t_noise = c_t_noise; e.x_0_noise = x_0_noise; e.c_0_noise = c_0_noise;
   e.logits = ws.w;                  // classifier scratch: the attention-weight buffer is free after the layers

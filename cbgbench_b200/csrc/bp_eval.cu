@@ -21,7 +21,7 @@ __global__ void __launch_bounds__(128) bp_eval_noise_kernel(BpEvalArgs p) {
   if (i >= p.b.n_lig) return;
   const int n1 = p.b.n_lig / p.n_rep;
   const int r = i / n1, a = i - r * n1;
-  const BpEvalCoefDev cf = p.coef.c[r];
+  const cbg_bp_eval_coef cf = p.coef.c[r];
   const bool gen = p.b.gen[i] != 0;
   // positions: x_t = sqrt(a) * x0 + sqrt(1 - a) * eps with the raw eps (the zero-centred one is only the target)
   const float sa = __fsqrt_rn(cf.alphas_cumprod), s1 = __fsqrt_rn(__fsub_rn(1.f, cf.alphas_cumprod));
@@ -56,7 +56,7 @@ __global__ void __launch_bounds__(kGraphThreads) bp_eval_loss_kernel(BpEvalArgs 
   const int2 rng = graph_ligand_range(p.b.lig_node, p.b.n_lig, p.b.graph_ptr, g);
   const int lo = rng.x, hi = rng.y, n_g = hi - lo;
   const int n1 = p.b.n_lig / p.n_rep;
-  const BpEvalCoefDev cf = p.coef.c[r];
+  const cbg_bp_eval_coef cf = p.coef.c[r];
   const int K = p.b.num_classes;
   // ---- graph means over ALL ligand atoms: raw noise, denoiser shift x_pred - x_t, CoM-head shift x_com - x_t
   {

@@ -66,6 +66,9 @@ inline cudaError_t cbg_launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 bloc
   return cudaLaunchKernelEx(&cfg, kernel, KArgs(args)...);
 }
 
+// workspace carves: every region starts on a 256-byte boundary
+inline size_t align256(size_t v) { return (v + 255) & ~(size_t)255; }
+
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int m = 16; m >= 1; m >>= 1) v += __shfl_xor_sync(CBG_FULL, v, m);

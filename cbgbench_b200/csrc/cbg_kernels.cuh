@@ -1,5 +1,6 @@
 // Internal launcher declarations (one per kernel family).  Not part of the C-ABI.
 #pragma once
+#include "../../include/cbg_b200.h"
 #include "cbg_common.cuh"
 
 #define CBG_MODE_KNN 0
@@ -147,9 +148,12 @@ int cbg_launch_step_init_io(const StepIO* io, const int* lig_node, int n_lig, in
 // the step-invariant members of `a` are used, the per-step ones (x_t, c_t, noise, outputs, coefficients) come from *io
 int cbg_launch_reverse_io(const ReverseArgs& a, const StepIO* io, cudaStream_t st);
 
-// Validation losses (eval.cu, bp_eval.cu, sbdd_eval.cu).  The plan's ligand atoms and graphs are R replicas of one
-// batch, replica-major: atom i belongs to replica i / n1 and is atom i % n1 of the batch (n1 = n_lig / R).
+// Validation losses (eval.cu, bp_eval.cu, sbdd_eval.cu, fg_eval.cu).  The plan's ligand atoms and graphs are R replicas
+// of one batch, replica-major: atom i belongs to replica i / n1 and is atom i % n1 of the batch (n1 = n_lig / R).
 constexpr int CBG_EVAL_MAX_REPLICAS = 64;
+// the per-replica coefficients (the public cbg_*_eval_coef structs), passed by value in the kernel arguments: no H2D
+// copy per call
+template <class C, int N> struct CoefArray { C c[N]; };
 // the batch block of the three argument structs (api.cu: open_eval fills it)
 struct EvalBatch {
   int n_lig, n_graphs, num_classes;   // n_lig / n_graphs: replicated totals
@@ -177,13 +181,8 @@ __device__ __forceinline__ void store_noised_ligand(const EvalBatch& b, int i, c
 }
 
 // eval.cu: TargetDiff validation loss over R = n_rep replicas of a batch (cbg_eval_loss_f32)
-struct EvalCoefDev {       // same members as cbg_eval_coef (include/cbg_b200.h)
-  float alphas_cumprod, lac, l1mac, lac_prev, l1mac_prev, la, l1ma;
-  int t_is_zero;
-};
-struct EvalCoefs { EvalCoefDev c[CBG_EVAL_MAX_REPLICAS]; };   // passed by value: no H2D copy per call
 struct EvalArgs {
-  EvalCoefs coef;
+  CoefArray<cbg_eval_coef, CBG_EVAL_MAX_REPLICAS> coef;
   int n_rep;
   EvalBatch b;
   const float* pos_noise;    // [n_lig,3]
@@ -259,10 +258,8 @@ int cbg_launch_bp_reverse(const BpArgs& a, cudaStream_t st);
 // bp_eval.cu: DiffBP validation loss over R = n_rep replicas of a batch (cbg_bp_eval_loss_f32).  After the CoM head
 // the ligand rows of x4 hold x_com.
 constexpr int CBG_BP_INTER_K = 48;       // interior loss: protein -> ligand kNN (diffbp.py:19)
-struct BpEvalCoefDev { float alphas_cumprod, beta, mask_prob; };    // same members as cbg_bp_eval_coef
-struct BpEvalCoefs { BpEvalCoefDev c[CBG_EVAL_MAX_REPLICAS]; };
 struct BpEvalArgs {
-  BpEvalCoefs coef;
+  CoefArray<cbg_bp_eval_coef, CBG_EVAL_MAX_REPLICAS> coef;
   int n_rep;
   EvalBatch b;
   const float* pos_noise;    // [n_lig,3] raw normal draws
@@ -286,18 +283,8 @@ int cbg_launch_bp_eval_loss(const BpEvalArgs& a, cudaStream_t st);
 // sbdd_eval.cu: DiffSBDD validation loss over n_t timesteps of a batch (cbg_sbdd_eval_loss_f32).  The plan holds R = 2 n_t
 // replicas: replica 2j is timestep j noised at t_j, replica 2j+1 timestep j noised at 0.  After the denoiser the ligand
 // rows of x4 hold x_pred.
-struct SbddEvalCoefDev {   // same members as cbg_sbdd_eval_coef (include/cbg_b200.h)
-  float pos_alpha_t, pos_sigma_t, type_alpha_t, type_sigma_t;
-  float pos_alpha_0, pos_sigma_0, type_alpha_0, type_sigma_0;
-  float pos_t_weight, type_t_weight;
-  float pos_log_const, type_log_const;
-  float pos_alpha_T, type_alpha_T;
-  float pos_log_inv_sigma_T, type_log_inv_sigma_T;
-  float pos_sigma2_T, type_sigma2_T;
-};
-struct SbddEvalCoefs { SbddEvalCoefDev c[CBG_EVAL_MAX_REPLICAS / 2]; };
 struct SbddEvalArgs {
-  SbddEvalCoefs coef;
+  CoefArray<cbg_sbdd_eval_coef, CBG_EVAL_MAX_REPLICAS / 2> coef;
   int n_t;
   long long n_nodes;
   EvalBatch b;
@@ -336,6 +323,24 @@ int cbg_ipa_launch(const float* blob, int hidden, int num_sublayers, int num_blo
                    const float* o, const float* h_in, const int* graph_ptr, int n_graphs, int max_graph_nodes,
                    const unsigned char* lig_flag, const unsigned char* gen_flag, int N, int k, float* eps_pos, float* h_out,
                    float* o_next, float* R_next, float* logits, char* ws, cudaStream_t st);
+// The IPATransformer shape checks shared by cbg_ipa_forward_f32, cbg_fg_step_f32 and cbg_fg_eval_loss_f32: hidden 128 /
+// 256, num_classes in [1, CBG_IPA_MAXCLS], n_nodes in [1, 2^31 / (5 * 256)), num_blocks >= 1, num_sublayers >= 0,
+// k in [1, CBG_KMAX] and a non-NULL, 256-byte aligned workspace of at least need_bytes.  Returns 0, or 1 with the error
+// set (message prefixed by fn).
+int check_ipa_shape(const char* fn, int hidden, int num_classes, long long n_nodes, int num_blocks, int num_sublayers,
+                    int k, const void* workspace, long long workspace_bytes, long long need_bytes);
+
+// fg.cu: the D3FG encoder workspace = cbg_ipa_workspace_bytes(n_nodes, hidden) bytes of IPATransformer scratch, then
+// the encoder's five output row arrays.  ws == NULL returns the sizes only (null pointers).
+struct FgRows {
+  float* eps_pos;   // [N,3]
+  float* o_pred;    // [N,3]
+  float* h_out;     // [N,hidden]
+  float* r_next;    // [N,9]
+  float* logits;    // [N,K]
+  size_t bytes;     // the whole workspace
+};
+FgRows fg_rows(void* ws, long long n_nodes, int hidden, int K);
 
 // ---- SO(3) maps of repo/models/utils/so3.py in fp32, used by ipa.cu (heads) and fg.cu (D3FG orientation step) ----------
 __device__ __forceinline__ void mat3_mul(const float* A, const float* B, float* C) {
@@ -382,22 +387,19 @@ __device__ __forceinline__ void rotation_to_so3vec(const float* R, float* w) {
   for (int e = 0; e < 3; ++e) w[e] = sg * (n[e] / rn);
 }
 
-// ---- D3FG per-FG helpers shared by fg.cu (reverse step) and fg_eval.cu (validation loss): one warp per functional
-// group, lane k holding class k ------------------------------------------------------------------------------------------
-__device__ __forceinline__ float fg_log_add_exp(float a, float b) {      // categorical.py: log_add_exp
+// ---- categorical helpers of the type schedules (misc.cu, eval.cu, fg.cu, fg_eval.cu) --------------------------------------
+__device__ __forceinline__ float log_add_exp(float a, float b) {         // categorical.py:35-37
   const float m = fmaxf(a, b);
   return m + logf(expf(a - m) + expf(b - m));
 }
+// log(clamp(0, 1e-30)) in fp32 (index_to_log_onehot, categorical.py:5-11): the off-class entry of a log one-hot
+__device__ __forceinline__ float log_1e30() { return __int_as_float(-1031133259); }   // -69.07755f
 
+// ---- D3FG per-FG helpers shared by fg.cu (reverse step) and fg_eval.cu (validation loss): one warp per functional
+// group, lane k holding class k ------------------------------------------------------------------------------------------
 __device__ __forceinline__ float fg_warp_max(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(CBG_FULL, v, o));
-  return v;
-}
-
-__device__ __forceinline__ float fg_warp_sum(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(CBG_FULL, v, o);
   return v;
 }
 

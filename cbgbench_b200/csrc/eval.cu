@@ -13,20 +13,12 @@
 
 namespace {
 
-// log(clamp(0, 1e-30)) in fp32 (index_to_log_onehot, categorical.py:5-11): the off-class entry of a log one-hot
-__device__ __forceinline__ float log_1e30() { return __int_as_float(-1031133259); }   // -69.07755f
-
-__device__ __forceinline__ float lae(float a, float b) {       // log_add_exp (categorical.py:35-37)
-  const float m = fmaxf(a, b);
-  return m + logf(expf(a - m) + expf(b - m));
-}
-
 __global__ void __launch_bounds__(128) eval_noise_kernel(EvalArgs p) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;      // replicated ligand atom
   if (i >= p.b.n_lig) return;
   const int n1 = p.b.n_lig / p.n_rep;
   const int r = i / n1, a = i - r * n1;
-  const EvalCoefDev cf = p.coef.c[r];
+  const cbg_eval_coef cf = p.coef.c[r];
   const int K = p.b.num_classes;
   const bool gen = p.b.gen[i] != 0;
   // positions: x_t = sqrt(a) * x0 + sqrt(1 - a) * eps   (two separately rounded products and one add)
@@ -41,11 +33,11 @@ __global__ void __launch_bounds__(128) eval_noise_kernel(EvalArgs p) {
   // types: v_t = argmax(log q(v_t | v_0) + Gumbel(u)),  log q = log_add_exp(log_c0 + lac[t], l1mac[t] - log K)
   const int v0 = (int)p.b.v0[a];
   const float logK = (float)log((double)K);
-  const float b = __fsub_rn(cf.l1mac, logK);
+  const float b = __fsub_rn(cf.log_one_minus_alphas_cumprod, logK);
   int arg = 0;
   float best = -INFINITY;
   for (int c = 0; c < K; ++c) {
-    const float lq = lae(__fadd_rn(c == v0 ? 0.f : log_1e30(), cf.lac), b);
+    const float lq = log_add_exp(__fadd_rn(c == v0 ? 0.f : log_1e30(), cf.log_alphas_cumprod), b);
     const float u = p.type_u[(size_t)i * K + c];
     const float score = -logf(-logf(u + 1e-30f) + 1e-30f) + lq;
     if (score > best) { best = score; arg = c; }
@@ -56,12 +48,12 @@ __global__ void __launch_bounds__(128) eval_noise_kernel(EvalArgs p) {
 }
 
 // q_v_posterior(log_v0, log_vt, t) (diffusion_scheduler.py:407-418) for one atom; log_vt is the clamped log one-hot of vt
-__device__ __forceinline__ void q_v_posterior(const float* lv0, int vt, const EvalCoefDev& cf, float logK, int K, float* out) {
-  const float ba = __fsub_rn(cf.l1mac_prev, logK), bb = __fsub_rn(cf.l1ma, logK);
+__device__ __forceinline__ void q_v_posterior(const float* lv0, int vt, const cbg_eval_coef& cf, float logK, int K, float* out) {
+  const float ba = __fsub_rn(cf.log_one_minus_alphas_cumprod_prev, logK), bb = __fsub_rn(cf.log_one_minus_alpha, logK);
   float m = -INFINITY;
   for (int c = 0; c < K; ++c) {
-    const float A = lae(__fadd_rn(lv0[c], cf.lac_prev), ba);
-    const float B = lae(__fadd_rn(c == vt ? 0.f : log_1e30(), cf.la), bb);
+    const float A = log_add_exp(__fadd_rn(lv0[c], cf.log_alphas_cumprod_prev), ba);
+    const float B = log_add_exp(__fadd_rn(c == vt ? 0.f : log_1e30(), cf.log_alpha), bb);
     out[c] = __fadd_rn(A, B);
     m = fmaxf(m, out[c]);
   }
@@ -78,7 +70,7 @@ __global__ void __launch_bounds__(kGraphThreads) eval_loss_kernel(EvalArgs p) {
   const int2 rng = graph_ligand_range(p.b.lig_node, p.b.n_lig, p.b.graph_ptr, g);
   const int lo = rng.x, hi = rng.y;
   const int n1 = p.b.n_lig / p.n_rep;
-  const EvalCoefDev cf = p.coef.c[r];
+  const cbg_eval_coef cf = p.coef.c[r];
   const int K = p.b.num_classes;
   const float logK = (float)log((double)K);
   float sum_pos = 0.f, sum_atom = 0.f, cnt = 0.f;

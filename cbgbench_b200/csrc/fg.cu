@@ -79,15 +79,15 @@ __global__ void __launch_bounds__(256) fg_reverse_kernel(cbg_fg_plan p, cbg_fg_c
   const bool on = lane < K;
   const float lg = on ? in.logits[(size_t)i * K + lane] : -INFINITY;
   const float mx = fg_warp_max(lg);
-  const float se = fg_warp_sum(on ? expf(lg - mx) : 0.f);
+  const float se = warp_sum(on ? expf(lg - mx) : 0.f);
   const float log_c_pred = (lg - mx) - logf(se);
   const float ctv = on ? c_t[(size_t)a * K + lane] : -INFINITY;
   const float logK = logf((float)K);
-  const float A = fg_log_add_exp(log_c_pred + cf.log_alphas_cumprod_prev, cf.log_one_minus_alphas_cumprod_prev - logK);
-  const float B = fg_log_add_exp(logf(ctv + 1e-8f) + cf.log_alpha, cf.log_one_minus_alpha - logK);
+  const float A = log_add_exp(log_c_pred + cf.log_alphas_cumprod_prev, cf.log_one_minus_alphas_cumprod_prev - logK);
+  const float B = log_add_exp(logf(ctv + 1e-8f) + cf.log_alpha, cf.log_one_minus_alpha - logK);
   const float un = on ? A + B : -INFINITY;
   const float m2 = fg_warp_max(un);
-  const float lse2 = m2 + logf(fg_warp_sum(on ? expf(un - m2) : 0.f));
+  const float lse2 = m2 + logf(warp_sum(on ? expf(un - m2) : 0.f));
   const float u = on ? type_u[(size_t)a * K + lane] : 0.5f;
   const float score = on ? -logf(-logf(u + 1e-30f) + 1e-30f) + (un - lse2) : -INFINITY;
   const int sampled = fg_warp_argmax(score, on ? lane : 1 << 30);
@@ -96,16 +96,27 @@ __global__ void __launch_bounds__(256) fg_reverse_kernel(cbg_fg_plan p, cbg_fg_c
   if (on) c_next[(size_t)a * K + lane] = lane == v ? 1.f : 0.f;
 }
 
-size_t al256(size_t b) { return (b + 255) & ~(size_t)255; }
-
 }  // namespace
+
+FgRows fg_rows(void* ws, long long n_nodes, int hidden, int K) {
+  const size_t n = (size_t)n_nodes;
+  char* b = (char*)ws;
+  size_t off = align256((size_t)cbg_ipa_workspace_bytes(n_nodes, hidden));
+  auto take = [&](size_t nbytes) { float* p = b ? (float*)(b + off) : nullptr; off += align256(nbytes); return p; };
+  FgRows r;
+  r.eps_pos = take(n * 3 * 4);
+  r.o_pred = take(n * 3 * 4);
+  r.h_out = take(n * hidden * 4);
+  r.r_next = take(n * 9 * 4);
+  r.logits = take(n * K * 4);
+  r.bytes = off;
+  return r;
+}
 
 extern "C" {
 
 int64_t cbg_fg_workspace_bytes(int64_t n_nodes, int32_t hidden, int32_t num_classes) {
-  const size_t n = (size_t)n_nodes;
-  return cbg_ipa_workspace_bytes(n_nodes, hidden) +
-         (int64_t)(2 * al256(n * 3 * 4) + al256(n * hidden * 4) + al256(n * 9 * 4) + al256(n * num_classes * 4));
+  return (int64_t)fg_rows(nullptr, n_nodes, hidden, num_classes).bytes;
 }
 
 int32_t cbg_fg_step_f32(const cbg_fg_plan* plan, cbg_fg_coef coef, const float* x_t, const float* c_t, const float* o_t,
@@ -113,39 +124,22 @@ int32_t cbg_fg_step_f32(const cbg_fg_plan* plan, cbg_fg_coef coef, const float* 
                         float* o_next, void* stream) {
   if (!plan) { cbg_set_error("cbg_fg_step_f32: plan is NULL"); return 1; }
   const cbg_fg_plan& p = *plan;
-  if (p.hidden != 128 && p.hidden != 256) { cbg_set_error("cbg_fg_step_f32: hidden=%d (128 or 256)", p.hidden); return 1; }
-  if (p.num_classes < 1 || p.num_classes > CBG_IPA_MAXCLS) {
-    cbg_set_error("cbg_fg_step_f32: num_classes=%d outside [1,%d]", p.num_classes, CBG_IPA_MAXCLS);
-    return 1;
-  }
-  if (p.n_nodes <= 0 || p.n_nodes > 0x7fffffffLL / (5 * 256) || p.n_lig < 0 || p.n_lig > p.n_nodes) {
+  if (int rc = check_ipa_shape("cbg_fg_step_f32", p.hidden, p.num_classes, p.n_nodes, p.num_blocks, p.num_sublayers, p.k,
+                               p.workspace, p.workspace_bytes,
+                               cbg_fg_workspace_bytes(p.n_nodes, p.hidden, p.num_classes)))
+    return rc;
+  if (p.n_lig < 0 || p.n_lig > p.n_nodes) {
     cbg_set_error("cbg_fg_step_f32: n_nodes=%lld n_lig=%d", (long long)p.n_nodes, p.n_lig);
     return 1;
   }
   if (p.n_bins < 2 || coef.t < 0) { cbg_set_error("cbg_fg_step_f32: n_bins=%d t=%d", p.n_bins, coef.t); return 1; }
-  if (p.num_blocks < 1 || p.num_sublayers < 0 || p.k < 1 || p.k > CBG_KMAX) {
-    cbg_set_error("cbg_fg_step_f32: num_blocks / num_sublayers / k");
-    return 1;
-  }
-  if (!p.workspace || ((uintptr_t)p.workspace & 255) != 0 ||
-      p.workspace_bytes < cbg_fg_workspace_bytes(p.n_nodes, p.hidden, p.num_classes)) {
-    cbg_set_error("cbg_fg_step_f32: workspace missing, unaligned or too small");
-    return 1;
-  }
   if (p.n_lig > 0 && (!x_t || !c_t || !o_t || !pos_noise || !rot_draws || !type_u || !x_next || !c_next || !o_next)) {
     cbg_set_error("cbg_fg_step_f32: NULL state or draw pointer");
     return 1;
   }
   cudaStream_t st = (cudaStream_t)stream;
   const int N = (int)p.n_nodes, H = p.hidden, K = p.num_classes;
-  char* ws = (char*)p.workspace;
-  size_t off = al256((size_t)cbg_ipa_workspace_bytes(p.n_nodes, H));
-  auto take = [&](size_t nbytes) { float* q = (float*)(ws + off); off += al256(nbytes); return q; };
-  float* eps_pos = take((size_t)N * 3 * 4);
-  float* o_pred = take((size_t)N * 3 * 4);
-  float* h_out = take((size_t)N * H * 4);
-  float* r_next = take((size_t)N * 9 * 4);
-  float* logits = take((size_t)N * K * 4);
+  const FgRows rows = fg_rows(p.workspace, p.n_nodes, H, K);
   const int grid = (p.n_lig + 7) / 8;
   if (grid > 0) {
     CBG_PROF_BEGIN(CBG_K_STEP_INIT, st);
@@ -153,12 +147,13 @@ int32_t cbg_fg_step_f32(const cbg_fg_plan* plan, cbg_fg_coef coef, const float* 
     CBG_LAUNCHED(CBG_K_STEP_INIT, st);
   }
   if (int rc = cbg_ipa_launch(p.blob, H, p.num_sublayers, p.num_blocks, K, p.x, p.o, p.h, p.graph_ptr, p.n_graphs,
-                              p.max_graph_nodes, p.lig_flag, p.gen_flag, N, p.k, eps_pos, h_out, o_pred, r_next, logits, ws, st))
+                              p.max_graph_nodes, p.lig_flag, p.gen_flag, N, p.k, rows.eps_pos, rows.h_out, rows.o_pred,
+                              rows.r_next, rows.logits, (char*)p.workspace, st))
     return rc;
   if (grid > 0) {
     CBG_PROF_BEGIN(CBG_K_REVERSE, st);
-    fg_reverse_kernel<<<grid, 256, 0, st>>>(p, coef, FgOut{eps_pos, o_pred, logits}, x_t, c_t, o_t, pos_noise, rot_draws,
-                                            type_u, x_next, c_next, o_next, nullptr);
+    fg_reverse_kernel<<<grid, 256, 0, st>>>(p, coef, FgOut{rows.eps_pos, rows.o_pred, rows.logits}, x_t, c_t, o_t,
+                                            pos_noise, rot_draws, type_u, x_next, c_next, o_next, nullptr);
     CBG_LAUNCHED(CBG_K_REVERSE, st);
   }
   return 0;

@@ -13,14 +13,9 @@
 
 namespace {
 
-// log(clamp(0, 1e-30)) in fp32 (index_to_log_onehot, categorical.py:5-11): the off-class entry of a log one-hot
-__device__ __forceinline__ float log_1e30() { return __int_as_float(-1031133259); }   // -69.07755f
-
-struct FgEvalCoefs { cbg_fg_eval_coef c[CBG_EVAL_MAX_REPLICAS]; };   // passed by value: no H2D copy per call
-
 struct FgEvalArgs {
   cbg_fg_plan p;
-  FgEvalCoefs coef;
+  CoefArray<cbg_fg_eval_coef, CBG_EVAL_MAX_REPLICAS> coef;
   int n_rep, loss_form;
   const float* x0;           // [n1,3]
   const long long* v0;       // [n1]
@@ -87,7 +82,7 @@ __global__ void __launch_bounds__(256) fg_eval_noise_kernel(FgEvalArgs A) {
   const bool on = lane < K;
   const int v0 = (int)A.v0[a];
   const float logK = (float)log((double)K);
-  const float lq = fg_log_add_exp(__fadd_rn(lane == v0 ? 0.f : log_1e30(), cf.log_alphas_cumprod),
+  const float lq = log_add_exp(__fadd_rn(lane == v0 ? 0.f : log_1e30(), cf.log_alphas_cumprod),
                                   __fsub_rn(cf.log_one_minus_alphas_cumprod, logK));
   const float u = on ? A.type_u[(size_t)i * K + lane] : 0.5f;
   const float sc = on ? -logf(-logf(u + 1e-30f) + 1e-30f) + lq : -INFINITY;
@@ -103,13 +98,13 @@ __global__ void __launch_bounds__(256) fg_eval_noise_kernel(FgEvalArgs A) {
 // lv0 is log v_0 (log one-hot or log-probabilities), vt the noised class.  Lanes >= K return -inf.
 __device__ __forceinline__ float fg_q_v_posterior(float lv0, int vt, const cbg_fg_eval_coef& cf, float logK, bool on,
                                                   int lane) {
-  const float A = fg_log_add_exp(__fadd_rn(lv0, cf.log_alphas_cumprod_prev),
+  const float A = log_add_exp(__fadd_rn(lv0, cf.log_alphas_cumprod_prev),
                                  __fsub_rn(cf.log_one_minus_alphas_cumprod_prev, logK));
-  const float B = fg_log_add_exp(__fadd_rn(lane == vt ? 0.f : log_1e30(), cf.log_alpha),
+  const float B = log_add_exp(__fadd_rn(lane == vt ? 0.f : log_1e30(), cf.log_alpha),
                                  __fsub_rn(cf.log_one_minus_alpha, logK));
   const float un = on ? __fadd_rn(A, B) : -INFINITY;
   const float m = fg_warp_max(un);
-  const float lse = m + logf(fg_warp_sum(on ? expf(un - m) : 0.f));
+  const float lse = m + logf(warp_sum(on ? expf(un - m) : 0.f));
   return on ? __fsub_rn(un, lse) : -INFINITY;
 }
 
@@ -183,15 +178,15 @@ __global__ void __launch_bounds__(kGraphThreads) fg_eval_loss_kernel(FgEvalArgs 
     // at t == 0 the decoder NLL -sum exp(log_c0) log p
     const float lg = on ? A.logits[(size_t)node * K + lane] : -INFINITY;
     const float mx = fg_warp_max(lg);
-    const float se = fg_warp_sum(on ? expf(lg - mx) : 0.f);
+    const float se = warp_sum(on ? expf(lg - mx) : 0.f);
     const float lcp = __fsub_rn(__fsub_rn(lg, mx), logf(se));
     if (on) A.c_pred[(size_t)i * K + lane] = expf(lcp);
     const int v0 = (int)A.v0[a], vt = (int)A.vt[i];
     const float lc0 = lane == v0 ? 0.f : log_1e30();
     const float lpt = fg_q_v_posterior(lc0, vt, cf, logK, on, lane);
     const float lpp = fg_q_v_posterior(lcp, vt, cf, logK, on, lane);
-    const float kl = fg_warp_sum(on ? __fmul_rn(expf(lpt), __fsub_rn(lpt, lpp)) : 0.f);
-    const float nll = -fg_warp_sum(on ? __fmul_rn(expf(lc0), lpp) : 0.f);
+    const float kl = warp_sum(on ? __fmul_rn(expf(lpt), __fsub_rn(lpt, lpp)) : 0.f);
+    const float nll = -warp_sum(on ? __fmul_rn(expf(lc0), lpp) : 0.f);
     if (lane == 0 && gen) {
       sum_pos += __fadd_rn(__fadd_rn(d2, d2_1), d2_2);
       sum_rot += rot;
@@ -226,8 +221,6 @@ __global__ void fg_eval_reduce_kernel(FgEvalArgs A) {
   for (int c = 0; c < 3; ++c) A.rep_loss[3 * r + c] = last < 0 ? NAN : __fdiv_rn(s[c], n);
 }
 
-size_t al256(size_t b) { return (b + 255) & ~(size_t)255; }
-
 }  // namespace
 
 extern "C" int32_t cbg_fg_eval_loss_f32(const cbg_fg_plan* plan, const cbg_fg_eval_coef* coefs, int32_t n_rep,
@@ -245,21 +238,16 @@ extern "C" int32_t cbg_fg_eval_loss_f32(const cbg_fg_plan* plan, const cbg_fg_ev
     cbg_set_error("cbg_fg_eval_loss_f32: loss_form=%d (0 score, 1 denoise)", loss_form);
     return 1;
   }
-  if (p.hidden != 128 && p.hidden != 256) { cbg_set_error("cbg_fg_eval_loss_f32: hidden=%d (128 or 256)", p.hidden); return 1; }
-  if (p.num_classes < 1 || p.num_classes > CBG_IPA_MAXCLS) {
-    cbg_set_error("cbg_fg_eval_loss_f32: num_classes=%d outside [1,%d]", p.num_classes, CBG_IPA_MAXCLS);
-    return 1;
-  }
-  if (p.n_nodes <= 0 || p.n_nodes > 0x7fffffffLL / (5 * 256) || p.n_lig < n_rep || p.n_lig > p.n_nodes ||
-      p.n_lig % n_rep || p.n_graphs < n_rep || p.n_graphs % n_rep) {
+  if (int rc = check_ipa_shape("cbg_fg_eval_loss_f32", p.hidden, p.num_classes, p.n_nodes, p.num_blocks, p.num_sublayers,
+                               p.k, p.workspace, p.workspace_bytes,
+                               cbg_fg_workspace_bytes(p.n_nodes, p.hidden, p.num_classes)))
+    return rc;
+  if (p.n_lig < n_rep || p.n_lig > p.n_nodes || p.n_lig % n_rep || p.n_graphs < n_rep || p.n_graphs % n_rep) {
     cbg_set_error("cbg_fg_eval_loss_f32: plan (n_nodes=%lld, n_lig=%d, n_graphs=%d) is not %d replicas of one batch",
                   (long long)p.n_nodes, p.n_lig, p.n_graphs, n_rep);
     return 1;
   }
-  if (p.n_bins < 2 || p.num_blocks < 1 || p.num_sublayers < 0 || p.k < 1 || p.k > CBG_KMAX) {
-    cbg_set_error("cbg_fg_eval_loss_f32: n_bins / num_blocks / num_sublayers / k");
-    return 1;
-  }
+  if (p.n_bins < 2) { cbg_set_error("cbg_fg_eval_loss_f32: n_bins=%d", p.n_bins); return 1; }
   for (int r = 0; r < n_rep; ++r) {
     if (coefs[r].t < 0) { cbg_set_error("cbg_fg_eval_loss_f32: coefs[%d].t=%d", r, coefs[r].t); return 1; }
   }
@@ -273,35 +261,24 @@ extern "C" int32_t cbg_fg_eval_loss_f32(const cbg_fg_plan* plan, const cbg_fg_ev
     cbg_set_error("cbg_fg_eval_loss_f32: NULL batch, draw or output pointer");
     return 1;
   }
-  if (!p.workspace || ((uintptr_t)p.workspace & 255) != 0 ||
-      p.workspace_bytes < cbg_fg_workspace_bytes(p.n_nodes, p.hidden, p.num_classes)) {
-    cbg_set_error("cbg_fg_eval_loss_f32: workspace missing, unaligned or too small");
-    return 1;
-  }
   cudaStream_t st = (cudaStream_t)stream;
   const int N = (int)p.n_nodes, H = p.hidden, K = p.num_classes;
-  char* ws = (char*)p.workspace;
-  size_t off = al256((size_t)cbg_ipa_workspace_bytes(p.n_nodes, H));     // the carve of cbg_fg_step_f32
-  auto take = [&](size_t nbytes) { float* q = (float*)(ws + off); off += al256(nbytes); return q; };
-  float* eps_pos = take((size_t)N * 3 * 4);
-  float* o_pred = take((size_t)N * 3 * 4);
-  float* h_out = take((size_t)N * H * 4);
-  float* r_next = take((size_t)N * 9 * 4);
-  float* logits = take((size_t)N * K * 4);
+  const FgRows rows = fg_rows(p.workspace, p.n_nodes, H, K);
   FgEvalArgs A;
   A.p = p;
   for (int r = 0; r < n_rep; ++r) A.coef.c[r] = coefs[r];
   A.n_rep = n_rep; A.loss_form = loss_form;
   A.x0 = x0; A.v0 = (const long long*)v0; A.o0 = o0;
   A.pos_noise = pos_noise; A.rot_draws = rot_draws; A.type_u = type_u;
-  A.eps_pos = eps_pos; A.r_next = r_next; A.logits = logits;
+  A.eps_pos = rows.eps_pos; A.r_next = rows.r_next; A.logits = rows.logits;
   A.xt = xt; A.ot = ot; A.vt = (long long*)vt; A.pred = pred; A.score = loss_form == CBG_FG_LOSS_SCORE ? score : nullptr;
   A.c_pred = c_pred; A.R_pred = R_pred; A.R0 = R0; A.graph_loss = graph_loss; A.rep_loss = rep_loss;
   CBG_PROF_BEGIN(CBG_K_STEP_INIT, st);
   fg_eval_noise_kernel<<<(p.n_lig + 7) / 8, 256, 0, st>>>(A);
   CBG_LAUNCHED(CBG_K_STEP_INIT, st);
   if (int rc = cbg_ipa_launch(p.blob, H, p.num_sublayers, p.num_blocks, K, p.x, p.o, p.h, p.graph_ptr, p.n_graphs,
-                              p.max_graph_nodes, p.lig_flag, p.gen_flag, N, p.k, eps_pos, h_out, o_pred, r_next, logits, ws, st))
+                              p.max_graph_nodes, p.lig_flag, p.gen_flag, N, p.k, rows.eps_pos, rows.h_out, rows.o_pred,
+                              rows.r_next, rows.logits, (char*)p.workspace, st))
     return rc;
   CBG_PROF_BEGIN(CBG_K_REVERSE, st);
   fg_eval_loss_kernel<<<p.n_graphs, kGraphThreads, 0, st>>>(A);

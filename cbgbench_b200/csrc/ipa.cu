@@ -338,7 +338,7 @@ int ipa_forward_t(const float* blob, int num_sublayers, int num_blocks, int num_
                   float* logits, char* ws, cudaStream_t st) {
   // workspace: x4 [N] | nbr [N,32] | ew [N,32] | scratch [N,32] ints (gate compaction) | planes [N,5H] | q [N,H]
   size_t off = 0;
-  auto take = [&](size_t nbytes) { char* p = ws + off; off += (nbytes + 255) & ~(size_t)255; return p; };
+  auto take = [&](size_t nbytes) { char* p = ws + off; off += align256(nbytes); return p; };
   float4* x4 = (float4*)take((size_t)N * 16);
   int* nbr = (int*)take((size_t)N * CBG_KMAX * 4);
   float* ew = (float*)take((size_t)N * CBG_KMAX * 4);
@@ -400,6 +400,26 @@ int cbg_ipa_launch(const float* blob, int hidden, int num_sublayers, int num_blo
                             lig_flag, gen_flag, N, k, eps_pos, h_out, o_next, R_next, logits, ws, st);
 }
 
+int check_ipa_shape(const char* fn, int hidden, int num_classes, long long n_nodes, int num_blocks, int num_sublayers,
+                    int k, const void* workspace, long long workspace_bytes, long long need_bytes) {
+  if (hidden != 128 && hidden != 256) { cbg_set_error("%s: hidden=%d (128 or 256)", fn, hidden); return 1; }
+  if (num_classes < 1 || num_classes > CBG_IPA_MAXCLS) {
+    cbg_set_error("%s: num_classes=%d outside [1,%d]", fn, num_classes, CBG_IPA_MAXCLS);
+    return 1;
+  }
+  if (n_nodes <= 0 || n_nodes > 0x7fffffffLL / (5 * 256)) { cbg_set_error("%s: n_nodes=%lld out of range", fn, n_nodes); return 1; }
+  if (num_blocks < 1 || num_sublayers < 0) {
+    cbg_set_error("%s: num_blocks=%d num_sublayers=%d", fn, num_blocks, num_sublayers);
+    return 1;
+  }
+  if (k < 1 || k > CBG_KMAX) { cbg_set_error("%s: k=%d outside [1,%d]", fn, k, CBG_KMAX); return 1; }
+  if (!workspace || ((uintptr_t)workspace & 255) != 0 || workspace_bytes < need_bytes) {
+    cbg_set_error("%s: workspace missing, unaligned or too small (%lld of %lld bytes)", fn, workspace_bytes, need_bytes);
+    return 1;
+  }
+  return 0;
+}
+
 extern "C" {
 
 int64_t cbg_ipa_head_floats(int32_t hidden) {
@@ -429,9 +449,8 @@ const char* cbg_ipa_layer_field_name(int32_t f) {
   return (f >= 0 && f < IL_COUNT) ? n[f] : nullptr;
 }
 int64_t cbg_ipa_workspace_bytes(int64_t n_nodes, int32_t hidden) {
-  auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
-  return (int64_t)(al((size_t)n_nodes * 16) + 2 * al((size_t)n_nodes * CBG_KMAX * 4) + al((size_t)n_nodes * 5 * hidden * 4) +
-                   al((size_t)n_nodes * hidden * 4) + 256);
+  return (int64_t)(align256((size_t)n_nodes * 16) + 2 * align256((size_t)n_nodes * CBG_KMAX * 4) +
+                   align256((size_t)n_nodes * 5 * hidden * 4) + align256((size_t)n_nodes * hidden * 4) + 256);
 }
 
 int32_t cbg_ipa_forward_f32(const float* blob, int32_t hidden, int32_t num_sublayers, int32_t num_blocks, int32_t num_classes,
@@ -439,13 +458,9 @@ int32_t cbg_ipa_forward_f32(const float* blob, int32_t hidden, int32_t num_subla
                             int32_t max_graph_nodes, const uint8_t* lig_flag, const uint8_t* gen_flag, int64_t n_nodes,
                             int32_t k, float* eps_pos, float* h_out, float* o_next, float* r_next, float* logits,
                             void* workspace, int64_t workspace_bytes, void* stream) {
-  if (hidden != 128 && hidden != 256) { cbg_set_error("cbg_ipa_forward_f32: hidden=%d (128 or 256)", hidden); return 1; }
-  if (num_classes < 1 || num_classes > CBG_IPA_MAXCLS) { cbg_set_error("num_classes=%d outside [1,%d]", num_classes, CBG_IPA_MAXCLS); return 1; }
-  if (n_nodes <= 0 || n_nodes > 0x7fffffffLL / (5 * 256)) { cbg_set_error("n_nodes=%lld out of range", (long long)n_nodes); return 1; }
-  if (!workspace || workspace_bytes < cbg_ipa_workspace_bytes(n_nodes, hidden)) { cbg_set_error("workspace too small"); return 1; }
-  if (((uintptr_t)workspace & 255) != 0) { cbg_set_error("workspace must be 256-byte aligned"); return 1; }
-  if (num_blocks < 1 || num_sublayers < 0) { cbg_set_error("num_blocks / num_sublayers"); return 1; }
-  if (k < 1 || k > CBG_KMAX) { cbg_set_error("cbg_ipa_forward_f32: k=%d outside [1,%d]", k, CBG_KMAX); return 1; }
+  if (int rc = check_ipa_shape("cbg_ipa_forward_f32", hidden, num_classes, n_nodes, num_blocks, num_sublayers, k, workspace,
+                               workspace_bytes, cbg_ipa_workspace_bytes(n_nodes, hidden)))
+    return rc;
   return cbg_ipa_launch(blob, hidden, num_sublayers, num_blocks, num_classes, x, o, h, graph_ptr, n_graphs, max_graph_nodes,
                         lig_flag, gen_flag, (int)n_nodes, k, eps_pos, h_out, o_next, r_next, logits, (char*)workspace,
                         (cudaStream_t)stream);

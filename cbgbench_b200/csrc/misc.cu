@@ -128,11 +128,6 @@ __global__ void __launch_bounds__(256) step_init_io_kernel(const StepIO* __restr
 //   types:     TypeVPScheduler.backward_remove_noise                diffusion_scheduler.py:367-378
 //              (q_v_posterior :407-418, q_v_pred :420-429, q_v_pred_one_timestep :431-441,
 //               log_sample_categorical / log_add_exp categorical.py:26-37)
-__device__ __forceinline__ float log_add_exp(float a, float b) {
-  const float m = fmaxf(a, b);
-  return m + logf(expf(a - m) + expf(b - m));
-}
-
 __device__ __forceinline__ void reverse_body(const ReverseArgs& p, float logvar, float nonzero) {
   const int a = blockIdx.x * blockDim.x + threadIdx.x;
   if (a >= p.n_lig) return;

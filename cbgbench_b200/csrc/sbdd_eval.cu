@@ -44,7 +44,7 @@ __global__ void __launch_bounds__(kGraphThreads) sbdd_eval_noise_kernel(SbddEval
   const int2 rng = graph_ligand_range(p.b.lig_node, p.b.n_lig, p.b.graph_ptr, g);
   const int lo = rng.x, hi = rng.y, n_g = hi - lo;
   const int lo1 = lo - r * n1, hi1 = hi - r * n1;            // the same atoms in the batch
-  const SbddEvalCoefDev& cf = p.coef.c[j];
+  const cbg_sbdd_eval_coef& cf = p.coef.c[j];
   const float ax = at_zero ? cf.pos_alpha_0 : cf.pos_alpha_t, sx = at_zero ? cf.pos_sigma_0 : cf.pos_sigma_t;
   const float ac = at_zero ? cf.type_alpha_0 : cf.type_alpha_t, sc = at_zero ? cf.type_sigma_0 : cf.type_sigma_t;
   const float* ex = (at_zero ? p.x_0_noise : p.x_t_noise) + (size_t)j * n1 * 3;
@@ -113,7 +113,7 @@ __global__ void __launch_bounds__(kGraphThreads) sbdd_eval_loss_kernel(SbddEvalA
   const int j = blockIdx.x / B1, g = blockIdx.x - j * B1;    // timestep, graph of the batch
   const int2 rng = graph_ligand_range(p.b.lig_node, p.b.n_lig, p.b.graph_ptr, g);     // replica 0's atoms are the batch's
   const int lo = rng.x, hi = rng.y, n_g = hi - lo;
-  const SbddEvalCoefDev& cf = p.coef.c[j];
+  const cbg_sbdd_eval_coef& cf = p.coef.c[j];
   const int K = p.b.num_classes;
   clean_mean(p.b.x0, lo, hi, s_red3, s_mean0);
   const float mean0[3] = {s_mean0[0], s_mean0[1], s_mean0[2]};

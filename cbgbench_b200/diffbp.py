@@ -145,7 +145,7 @@ class DiffBPB200(BaseDiffB200):
                 v0.data_ptr(), pos_noise[r0:r1].data_ptr(), type_uniform[r0:r1].data_ptr(), xt[r0:r1].data_ptr(),
                 vt[r0:r1].data_ptr(), mask[r0:r1].data_ptr(), vec[r0:r1].data_ptr(), c_pred[r0:r1].data_ptr(),
                 rep_loss[r0:r1].data_ptr(), _lib.stream_ptr(dev)))
-        self._eval_loop(b, n_graphs, t_values, _lib.BpEvalCoef, max_nodes, launch)
+        self._eval_plans(b, n_graphs, t_values, _lib.BpEvalCoef, max_nodes, launch)
         loss_dict = self._eval_dict_mean(rep_loss, ('pos', 'atom', 'com', 'inter'))
         vt_onehot = F.one_hot(vt, K).float()
         # the reference's key order: pos_info, then atom_info (its mask_gen, the type mask, replaces gen), then com_info
@@ -191,9 +191,9 @@ class DiffBPB200(BaseDiffB200):
         ``traj_mode='final'`` keeps only traj[0] and traj[-1]; ``eps_out`` (dict) receives eps + eps_com per step."""
         T = self.num_diffusion_timesteps
         state = self.prepare(batch)
-        X, Cc = self._traj_buffers(state['device'], state['x_lig'], state['c_lig'])
+        X, Cc = self._traj_buffers(state['device'], (state['x_lig'], state['c_lig']))
         t_seq = list(reversed(range(T)))
         if num_steps is not None:
             t_seq = t_seq[:num_steps]
         self.run_steps(state, t_seq, X, Cc, pos_noise, type_uniform, eps_out)
-        return self._traj(X, Cc, state['batch_idx_lig'], t_seq[-1], traj_mode)
+        return self._traj((X, Cc), state['batch_idx_lig'], t_seq[-1], traj_mode)

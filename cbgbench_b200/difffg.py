@@ -27,7 +27,7 @@ import torch.nn.functional as F
 from . import _lib
 from .modules import cfg_get, get_e3_gnn, graph_ptr_from_batch, _Workspace
 from .schedulers import CTNVPTables, TypeVPTables, VPTables
-from .targetdiff import BaseDiffB200, eval_t_values, register_model
+from .targetdiff import DiffusionB200, register_model
 
 NUM_AA_TYPES = 21          # repo/utils/protein/constants.py:75: len(AA), the width added to num_fgtype by FGContextEmbedder
 NUM_AA_ONEHOT = 20         # len(aa_name_number): the reference one-hots protein_aa with 20 classes (context_emb.py:119)
@@ -229,11 +229,10 @@ def backbone_dihedrals(pos, chain_nb, res_nb, mask):
 # ---- the model ---------------------------------------------------------------------------------------------------------
 
 @register_model('difffg')
-class D3FGB200(nn.Module):
+class D3FGB200(DiffusionB200):
     """D3FG (difffg.py:32-63, 250-280) with CUDA sampling and validation-loss paths."""
 
     pos_loss_form = _lib.FG_LOSS_SCORE    # difffg: get_score_loss(score_in=False) (difffg.py:145-148)
-    eval_max_nodes = 1 << 20              # composed nodes per validation-loss launch (about 8 GB at ~7.6 KB/node, H = 256)
 
     def __init__(self, cfg):
         super().__init__()
@@ -398,10 +397,7 @@ class D3FGB200(nn.Module):
         rot = self.rot_scheduler.angular_distrib_inv
         rot_std, rot_flag = rot.stddevs.cpu(), rot.approx_flag.cpu()
         dev, n, plan = state['device'], state['n_lig'], state['plan']
-        X = torch.empty(T + 1, n, 3, device=dev)
-        Cc = torch.empty(T + 1, n, K, device=dev)
-        O = torch.empty(T + 1, n, 3, device=dev)
-        X[T], Cc[T], O[T] = state['x0'], state['c0'], state['o0']
+        X, Cc, O = self._traj_buffers(dev, (state['x0'], state['c0'], state['o0']))
         to = lambda a: a.to(dev, torch.float32).contiguous()
         L = _lib.lib()
         st = _lib.stream_ptr(dev)
@@ -421,36 +417,14 @@ class D3FGB200(nn.Module):
                                              O[t + 1].data_ptr(), pn.data_ptr(), rd.data_ptr(), tu.data_ptr(),
                                              X[t].data_ptr(), Cc[t].data_ptr(), O[t].data_ptr(), st))
         self.last_launches = L.cbg_launch_count() - launches0
-        t_last = t_seq[-1]
-        bl, bl_cpu = state['batch_idx_lig'], state['batch_idx_lig'].cpu()
-        traj = {}
-        hi = T if traj_mode == 'full' else t_last + 1
-        Xh, Ch, Oh = X[t_last + 1:hi + 1].cpu(), Cc[t_last + 1:hi + 1].cpu(), O[t_last + 1:hi + 1].cpu()
-        for t in range(t_last, hi):
-            traj[t] = (Xh[t - t_last], Ch[t - t_last], Oh[t - t_last], bl_cpu)
-        traj[t_last - 1] = (X[t_last].clone(), Cc[t_last].clone(), O[t_last].clone(), bl)
-        return traj
+        return self._traj((X, Cc, O), state['batch_idx_lig'], t_seq[-1], traj_mode)
 
     # ---- validation losses (D3FG.forward with self.training == False, difffg.py:65-171 / :283-389) -----------------------
-    def forward(self, batch, pos_noise=None, rot_draws=None, type_uniform=None):
-        """The reference's forward in eval mode: ``(loss_dict, results)`` of ``eval_losses`` for the ``eval_interval``
-        (default 10) timesteps ``np.linspace(0, T-1, eval_interval)`` truncated to integers.  Training mode needs autograd
-        through the encoder and raises, as does a model on the CPU."""
+    def _check_eval_mode(self):
+        """Training mode raises, and so does a model on the CPU: ``eval_losses`` reads the batch's graph ids before its
+        own device check, so ``forward`` checks the device first."""
+        super()._check_eval_mode()
         self._eval_device()
-        t_values = eval_t_values(self.num_diffusion_timesteps, cfg_get(self.cfg, 'eval_interval', 10))
-        return self.eval_losses(batch, t_values, pos_noise=pos_noise, rot_draws=rot_draws, type_uniform=type_uniform)
-
-    def _eval_device(self):
-        name = type(self).__name__
-        if self.training:
-            raise NotImplementedError(f'{name}.forward in training mode needs autograd through the encoder, which the CUDA '
-                                      'path does not provide: training is out of scope (call model.eval() for the '
-                                      'validation losses)')
-        dev = next(self.parameters()).device
-        if dev.type != 'cuda':
-            raise NotImplementedError(f'{name}.forward needs the model on a CUDA device: there is no CPU implementation '
-                                      'of the validation losses')
-        return dev
 
     def eval_coef(self, t):
         """Host scalars of the validation loss at timestep t, with the reference's fp32 torch expressions."""
@@ -488,18 +462,15 @@ class D3FGB200(nn.Module):
         in-bin uniform, Gaussian-branch N(0,1)), ``type_uniform`` [R,n,K] U[0,1).  By default they are drawn with torch on
         the model device in the reference's order (for each t: randn [n,3], randn [n,3], rand [n], rand [n], randn [n],
         rand [n,K]; the bin draw stands for ``torch.multinomial``, see ``multinomial_bin``)."""
-        T, K = self.num_diffusion_timesteps, self.num_classes
-        t_values = [int(t) for t in t_values]
-        if not t_values:
-            raise ValueError('t_values is empty')
-        if any(t < 0 or t > T - 1 for t in t_values):
-            raise ValueError(f't_values must lie in [0, {T - 1}]')
+        K = self.num_classes
+        t_values = self._eval_t_values(t_values)
         if (pos_noise is None) != (rot_draws is None) or (pos_noise is None) != (type_uniform is None):
             raise ValueError('inject pos_noise, rot_draws and type_uniform together, or none of them')
         bl, br = batch['ligand_type_fg_batch'], batch['protein_type_fg_batch']
         if bl.numel() and br.numel() and int(br.max()) > int(bl.max()):
             # the reference sizes t by the last graph with FGs and indexes it with the residues' graph ids (IndexError)
             raise ValueError('D3FGB200.forward: the last graph of the batch has residues but no functional group')
+        self._check_eval_mode()
         dev = self._eval_device()
         ctx = self._context(batch)
         R, n = len(t_values), ctx['n_lig']
@@ -523,31 +494,25 @@ class D3FGB200(nn.Module):
         R0 = torch.empty(n, 3, 3, device=dev)
         rep_loss = torch.empty(R, 3, device=dev)
         x0, v0, o0 = ctx['xc_lig'], ctx['v_lig'].contiguous(), ctx['o_lig']
-        n_nodes = n + ctx['n_rec']
-        budget = self.eval_max_nodes if max_nodes is None else int(max_nodes)
-        per_launch = max(1, min(_lib.EVAL_MAX_REPLICAS, budget // n_nodes))
         fwd, cdf = self.rot_scheduler.angular_distrib_fwd, self.rot_scheduler.fwd_cdf(dev)
         L = _lib.lib()
         st = _lib.stream_ptr(dev)
-        launches0 = L.cbg_launch_count()
         graph_loss = []
-        with torch.cuda.device(dev):
-            for r0 in range(0, R, per_launch):
-                r1 = min(R, r0 + per_launch)
-                state = self._compose(ctx, r1 - r0, fwd, cdf)
-                gl = torch.empty(state['n_graphs'], 4, device=dev)
-                coefs = (_lib.FgEvalCoef * (r1 - r0))(*[self.eval_coef(t) for t in t_values[r0:r1]])
-                _lib.check(L.cbg_fg_eval_loss_f32(
-                    C.byref(state['plan']), coefs, r1 - r0, self.pos_loss_form, x0.data_ptr(), v0.data_ptr(),
-                    o0.data_ptr(), pn[r0:r1].data_ptr(), rd[r0:r1].data_ptr(), tu[r0:r1].data_ptr(), xt[r0:r1].data_ptr(),
-                    ot[r0:r1].data_ptr(), vt[r0:r1].data_ptr(), pred[r0:r1].data_ptr(),
-                    score[r0:r1].data_ptr() if score_form else None, c_pred[r0:r1].data_ptr(), R_pred[r0:r1].data_ptr(),
-                    R0.data_ptr(), gl.data_ptr(), rep_loss[r0:r1].data_ptr(), st))
-                graph_loss.append(gl)
-        self.last_launches = L.cbg_launch_count() - launches0
+
+        def launch(r0, r1, state, coefs):
+            gl = torch.empty(state['n_graphs'], 4, device=dev)
+            _lib.check(L.cbg_fg_eval_loss_f32(
+                C.byref(state['plan']), coefs, r1 - r0, self.pos_loss_form, x0.data_ptr(), v0.data_ptr(),
+                o0.data_ptr(), pn[r0:r1].data_ptr(), rd[r0:r1].data_ptr(), tu[r0:r1].data_ptr(), xt[r0:r1].data_ptr(),
+                ot[r0:r1].data_ptr(), vt[r0:r1].data_ptr(), pred[r0:r1].data_ptr(),
+                score[r0:r1].data_ptr() if score_form else None, c_pred[r0:r1].data_ptr(), R_pred[r0:r1].data_ptr(),
+                R0.data_ptr(), gl.data_ptr(), rep_loss[r0:r1].data_ptr(), st))
+            graph_loss.append(gl)
+        self._eval_loop(n + ctx['n_rec'], t_values, _lib.FgEvalCoef, max_nodes, launch,
+                        lambda n_rep: self._compose(ctx, n_rep, fwd, cdf))
         self.last_ot = ot
         self.last_graph_loss = torch.cat(graph_loss)
-        loss_dict = BaseDiffB200._eval_dict_mean(rep_loss, ('pos', 'rot', 'fg'))
+        loss_dict = self._eval_dict_mean(rep_loss, ('pos', 'rot', 'fg'))
         mask_gen = ctx['gen_lig']
         results = []
         for r in range(R):

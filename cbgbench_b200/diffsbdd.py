@@ -25,7 +25,6 @@ import numpy as np
 import torch
 
 from . import _lib
-from .modules import cfg_get
 from .schedulers import DiffsbddVariationalTables
 from . import targetdiff
 from .targetdiff import BaseDiffB200, register_model
@@ -43,6 +42,7 @@ def eval_t_values(num_timesteps, eval_interval=10):
 @register_model('diffsbdd')
 class DiffSBDDB200(BaseDiffB200):
     allow_rcache = False
+    eval_t_first = 1         # the eval timesteps are np.linspace(1, T, eval_interval) (diffsbdd.py:71-77)
 
     def __init__(self, cfg):
         super().__init__(cfg)
@@ -53,14 +53,6 @@ class DiffSBDDB200(BaseDiffB200):
         self.intersect_reg = cfg.get('intersect_reg', True) if hasattr(cfg, 'get') else True
 
     # ---- validation loss (DiffSBDD.forward with self.training == False, diffsbdd.py:48-191) --------------------------
-    def forward(self, batch, noise=None):
-        """The reference's forward in eval mode: ``(loss_dict, results)`` of ``eval_losses`` for the ``eval_interval``
-        (default 10) timesteps ``np.linspace(1, T, eval_interval)`` truncated to integers, exactly like the reference.
-        Training mode needs autograd through the denoiser and raises."""
-        self._check_eval_mode()
-        t_values = eval_t_values(self.num_diffusion_timesteps, cfg_get(self.cfg, 'eval_interval', 10))
-        return self.eval_losses(batch, t_values, noise=noise)
-
     def eval_coef(self, t):
         """Host scalars of timestep t (integer in [1, T]) with the reference's fp32 torch expressions: s = (t - 1) / T and
         t / T as in get_loss, gamma at 0 (t_zeros) and at 1 (kl_prior's ones)."""
@@ -98,7 +90,7 @@ class DiffSBDDB200(BaseDiffB200):
         ``noise`` = {'x_t', 'c_t', 'x_0', 'c_0'} of [R, n_lig, 3 | K] injects the draws; by default they are drawn with
         torch on the model device in the reference's order (for each t: randn [n_lig,3], [n_lig,K], [n_lig,3],
         [n_lig,K])."""
-        t_values = self._eval_t_values(t_values, first=1)
+        t_values = self._eval_t_values(t_values)
         R, K = len(t_values), self.num_classes
         dev, b, n_graphs, x0, v0, gen = self._eval_batch(batch)
         x_rec = b['protein_pos'].float().contiguous()
@@ -120,8 +112,8 @@ class DiffSBDDB200(BaseDiffB200):
                 C.byref(state['plan']), coefs, r1 - r0, x0.data_ptr(), v0.data_ptr(), x_rec.data_ptr() if x_rec.numel() else None,
                 *[noise[k][r0:r1].data_ptr() for k in EVAL_NOISE_KEYS], vec_pos[r0:r1].data_ptr(),
                 vec_atom[r0:r1].data_ptr(), terms[r0:r1].data_ptr(), t_loss[r0:r1].data_ptr(), _lib.stream_ptr(dev)))
-        self._eval_loop(b, n_graphs, t_values, _lib.SbddEvalCoef, max_nodes, launch, copies=2,
-                        protein_feature_scale=TYPE_NORM)
+        self._eval_plans(b, n_graphs, t_values, _lib.SbddEvalCoef, max_nodes, launch, copies=2,
+                         protein_feature_scale=TYPE_NORM)
         self.last_terms = terms[:, :int(b['ligand_element_batch'].max()) + 1]
         loss_dict = self._eval_dict_mean(t_loss, ('pos', 'atom'))
         # the reference's key order: pos_info, then atom_info (get_score_loss, diffusion_scheduler.py:944-961)
@@ -167,7 +159,7 @@ class DiffSBDDB200(BaseDiffB200):
         x_lig = (x_lig - mean[bl]).contiguous()
         x_rec = x_rec - mean[br]
         state = self.prepare(batch, device=dev, protein_feature_scale=TYPE_NORM, protein_pos=x_rec)
-        state['X'], state['C'] = self._traj_buffers(dev, x_lig, eps_c)
+        state['X'], state['C'] = self._traj_buffers(dev, (x_lig, eps_c))
         return state
 
     @torch.no_grad()
@@ -235,7 +227,7 @@ class DiffSBDDB200(BaseDiffB200):
         if t_last == 0:
             x_fin, c_fin = self.finish(state, noise)
         self.last_launches = launches
-        traj = self._traj(state['X'], state['C'], state['batch_idx_lig'], t_last, traj_mode)
+        traj = self._traj((state['X'], state['C']), state['batch_idx_lig'], t_last, traj_mode)
         if x_fin is not None:
             traj[0] = (x_fin.cpu(), c_fin.cpu(), traj[0][2])
         return traj

@@ -107,13 +107,103 @@ class PLContextEmbedderB200(nn.Module):
         return h_rec, h_lig_bias.contiguous()
 
 
-class BaseDiffB200(nn.Module):
+class DiffusionB200(nn.Module):
+    """What every CUDA diffusion model shares, whatever its network: the trajectory buffers of ``sample`` and the
+    eval-mode ``forward`` (validation losses of replica batches, DESIGN.md section 13).  A subclass provides
+    ``num_diffusion_timesteps``, ``cfg``, ``eval_coef(t)`` and ``eval_losses(batch, t_values, *draws, **kw)``."""
+
+    eval_t_first = 0            # first eval timestep of ``eval_t_values``: 0, or 1 for DiffSBDD
+    # composed nodes per validation-loss launch: about 9 GB of workspace at ~8.5 KB/node for the denoiser, 8 GB at
+    # ~7.6 KB/node for the D3FG encoder at H = 256
+    eval_max_nodes = 1 << 20
+
+    # ---- the trajectory of ``sample`` ----------------------------------------------------------------------------
+    def _traj_buffers(self, dev, init):
+        """One device trajectory [T+1, *v.shape] per initial state tensor v of the tuple ``init`` (x [n_lig,3], c
+        [n_lig,K], ...): slot t+1 is the state entering step t, slot t its result; slot T holds the initial state."""
+        T = self.num_diffusion_timesteps
+        bufs = tuple(torch.empty((T + 1, *v.shape), dtype=torch.float32, device=dev) for v in init)
+        for b, v in zip(bufs, init):
+            b[T].copy_(v)
+        return bufs
+
+    def _traj(self, bufs, bl, t_last, traj_mode):
+        """``traj`` of the reference's sample: {t: (*states, batch_idx_lig)} for t = T-1 ... t_last (on the CPU, one
+        copy; only t_last when ``traj_mode`` is not 'full') and t_last - 1 (on the device)."""
+        T = self.num_diffusion_timesteps
+        hi = T if traj_mode == 'full' else t_last + 1
+        host = [b[t_last + 1:hi + 1].cpu() for b in bufs]
+        bl_cpu = bl.cpu()
+        traj = {t: (*(h[t - t_last] for h in host), bl_cpu) for t in range(t_last, hi)}
+        traj[t_last - 1] = (*(b[t_last].clone() for b in bufs), bl)
+        return traj
+
+    # ---- validation losses: what the eval-mode forwards share (replica batching, DESIGN.md section 13) --------------
+    def forward(self, batch, *draws, **kw):
+        """The reference's forward in eval mode: ``(loss_dict, results)`` of ``eval_losses`` for the ``eval_interval``
+        (default 10) timesteps ``eval_t_values(T, eval_interval, first=eval_t_first)``, exactly like the reference.
+        Training mode needs autograd through the network and raises; ``eval_losses`` refuses a model on the CPU."""
+        self._check_eval_mode()
+        t_values = eval_t_values(self.num_diffusion_timesteps, cfg_get(self.cfg, 'eval_interval', 10),
+                                 first=self.eval_t_first)
+        return self.eval_losses(batch, t_values, *draws, **kw)
+
+    def _check_eval_mode(self):
+        if self.training:
+            raise NotImplementedError(f'{type(self).__name__}.forward in training mode needs autograd through the '
+                                      'network, which the CUDA path does not provide: training is out of scope '
+                                      '(call model.eval() for the validation losses)')
+
+    def _eval_device(self):
+        """The model's device, which must be a CUDA device."""
+        dev = next(self.parameters()).device
+        if dev.type != 'cuda':
+            raise NotImplementedError(f'{type(self).__name__}.forward needs the model on a CUDA device: on the CPU '
+                                      f'{type(self).__name__} is a sampling build without a validation-loss implementation')
+        return dev
+
+    def _eval_t_values(self, t_values):
+        """``t_values`` as ints, each in [eval_t_first, T - 1 + eval_t_first]."""
+        t_values = [int(t) for t in t_values]
+        lo, hi = self.eval_t_first, self.num_diffusion_timesteps - 1 + self.eval_t_first
+        if not t_values:
+            raise ValueError('t_values is empty')
+        if any(t < lo or t > hi for t in t_values):
+            raise ValueError(f't_values must lie in [{lo}, {hi}]')
+        return t_values
+
+    def _eval_loop(self, n_nodes, t_values, coef_type, max_nodes, launch, make_state, copies=1):
+        """Run the timesteps ``t_values`` of a batch of ``n_nodes`` composed nodes in plans of at most 64 replicas and
+        ``max_nodes`` composed nodes (default ``eval_max_nodes``): each plan holds timesteps r0 .. r1-1, ``copies``
+        noised copies each, and is ``make_state(n_rep)`` with n_rep = (r1 - r0) * copies.  ``launch(r0, r1, state,
+        coefs)`` makes the plan's C call, with ``coefs`` the ctypes array of ``eval_coef`` over t_values[r0:r1], on the
+        plan's device.  ``last_launches`` counts the kernels of all plans."""
+        budget = self.eval_max_nodes if max_nodes is None else int(max_nodes)
+        per_launch = max(1, min(_lib.EVAL_MAX_REPLICAS // copies, budget // (copies * n_nodes)))
+        L = _lib.lib()
+        launches0 = L.cbg_launch_count()
+        for r0 in range(0, len(t_values), per_launch):
+            r1 = min(len(t_values), r0 + per_launch)
+            state = make_state((r1 - r0) * copies)
+            coefs = (coef_type * (r1 - r0))(*[self.eval_coef(t) for t in t_values[r0:r1]])
+            with torch.cuda.device(state['device']):
+                launch(r0, r1, state, coefs)
+        self.last_launches = L.cbg_launch_count() - launches0
+
+    @staticmethod
+    def _eval_dict_mean(per_t, keys):
+        """get_dict_mean (common.py:33-42) of the per-t losses [R, len(keys)]: for each key the mean over t of its column,
+        as a CPU float32 0-d tensor."""
+        per_t = per_t.cpu()
+        return {k: torch.mean(torch.tensor(per_t[:, i].tolist())) for i, k in enumerate(keys)}
+
+
+class BaseDiffB200(DiffusionB200):
     """What the samplers built on the denoiser share (mirror of repo/models/diffusion/_base.py:4-11 plus the
     hoisting of everything step-invariant): generator flags, context embedder, denoiser, device workspaces and
     ``prepare`` (batch -> device plan)."""
 
     allow_rcache = True      # samplers whose pocket atoms move between steps (DiffSBDD) turn the R-cache off
-    eval_max_nodes = 1 << 20    # composed nodes per validation-loss launch (about 9 GB of workspace at ~8.5 KB/node)
 
     def __init__(self, cfg):
         super().__init__()
@@ -156,57 +246,7 @@ class BaseDiffB200(nn.Module):
             raise RuntimeError('stale sampling state: prepare() was called again on this model (its device workspace now '
                                'belongs to the newer batch); finish one batch before preparing the next, or use a second model')
 
-    # ---- the trajectory of ``sample`` ----------------------------------------------------------------------------
-    def _traj_buffers(self, dev, x_init, c_init):
-        """Device trajectory X [T+1,n_lig,3] / Cc [T+1,n_lig,K]: slot t+1 is the state entering step t, slot t its
-        result; slot T holds the initial state."""
-        T, n_lig = self.num_diffusion_timesteps, x_init.shape[0]
-        X = torch.empty((T + 1, n_lig, 3), dtype=torch.float32, device=dev)
-        Cc = torch.empty((T + 1, n_lig, self.num_classes), dtype=torch.float32, device=dev)
-        X[T].copy_(x_init)
-        Cc[T].copy_(c_init)
-        return X, Cc
-
-    def _traj(self, X, Cc, bl, t_last, traj_mode):
-        """``traj`` of the reference's sample: {t: (x_lig, c_lig, batch_idx_lig)} for t = T-1 ... t_last (on the CPU,
-        one copy; only t_last when ``traj_mode`` is not 'full') and t_last - 1 (on the device)."""
-        T = self.num_diffusion_timesteps
-        traj = {}
-        bl_cpu = bl.cpu()
-        if traj_mode == 'full':
-            Xh, Ch = X[t_last + 1:].cpu(), Cc[t_last + 1:].cpu()
-            for t in range(t_last, T):
-                traj[t] = (Xh[t - t_last], Ch[t - t_last], bl_cpu)
-        else:
-            traj[t_last] = (X[t_last + 1].cpu(), Cc[t_last + 1].cpu(), bl_cpu)
-        traj[t_last - 1] = (X[t_last].clone(), Cc[t_last].clone(), bl)
-        return traj
-
-    # ---- validation losses: what the eval-mode forwards share (replica batching, DESIGN.md section 13) --------------
-    def forward(self, batch, pos_noise=None, type_uniform=None):
-        """The reference's forward in eval mode: ``(loss_dict, results)`` of ``eval_losses`` for the ``eval_interval``
-        (default 10) timesteps ``np.linspace(0, T-1, eval_interval)`` truncated to integers, exactly like the reference.
-        Training mode needs autograd through the denoiser and raises."""
-        self._check_eval_mode()
-        t_values = eval_t_values(self.num_diffusion_timesteps, cfg_get(self.cfg, 'eval_interval', 10))
-        return self.eval_losses(batch, t_values, pos_noise=pos_noise, type_uniform=type_uniform)
-
-    def _check_eval_mode(self):
-        if self.training:
-            raise NotImplementedError(f'{type(self).__name__}.forward in training mode needs autograd through the '
-                                      'denoiser, which the CUDA path does not provide: training is out of scope '
-                                      '(call model.eval() for the validation losses)')
-
-    def _eval_t_values(self, t_values, first=0):
-        """``t_values`` as ints, each in [first, T - 1 + first]."""
-        t_values = [int(t) for t in t_values]
-        T = self.num_diffusion_timesteps
-        if not t_values:
-            raise ValueError('t_values is empty')
-        if any(t < first or t > T - 1 + first for t in t_values):
-            raise ValueError(f't_values must lie in [{first}, {T - 1 + first}]')
-        return t_values
-
+    # ---- validation losses of the denoiser models ----------------------------------------------------------------
     @staticmethod
     def _eval_noise(R, dev, pos_noise, type_uniform, type_shape):
         """pos_noise [R,n_lig,3] / type_uniform [R,*type_shape] on ``dev``; what is not injected is drawn in the
@@ -228,10 +268,7 @@ class BaseDiffB200(nn.Module):
         """(dev, b, n_graphs, x0, v0, gen): the model's CUDA device, the batch's tensors on it (dict or attribute batch),
         its graph count, the clean ligand positions x0 [n_lig,3] float32 and types v0 [n_lig] int64, and its generation
         flags (ligand_lig_flag when the batch has no ligand_gen_flag)."""
-        dev = next(self.parameters()).device
-        if dev.type != 'cuda':
-            raise NotImplementedError(f'{type(self).__name__}.forward needs the model on a CUDA device: on the CPU '
-                                      f'{type(self).__name__} is a sampling build without a validation-loss implementation')
+        dev = self._eval_device()
         g = lambda k, d=None: batch.get(k, d) if hasattr(batch, 'get') else (batch[k] if k in batch else d)
         b = {k: g(k).to(dev) for k in self._EVAL_KEYS if g(k) is not None}
         if b['ligand_pos'].shape[0] == 0:
@@ -242,31 +279,11 @@ class BaseDiffB200(nn.Module):
         gen = b['ligand_gen_flag'] if 'ligand_gen_flag' in b else b['ligand_lig_flag']
         return dev, b, n_graphs, x0, v0, gen
 
-    def _eval_loop(self, b, n_graphs, t_values, coef_type, max_nodes, launch, copies=1, **prepare_kw):
-        """Run the timesteps ``t_values`` in plans of at most 64 replicas and ``max_nodes`` composed nodes (default
-        ``eval_max_nodes``): each plan holds timesteps r0 .. r1-1, ``copies`` noised copies each, as (r1 - r0) * copies *
-        n_graphs graphs (``prepare_kw`` goes to ``prepare``).  ``launch(r0, r1, state, coefs)`` makes the plan's C call,
-        with ``coefs`` the ctypes array of ``eval_coef`` over t_values[r0:r1], on the plan's device.  ``last_launches``
-        counts the kernels of all plans."""
-        n_nodes = b['ligand_pos'].shape[0] + b['protein_pos'].shape[0]
-        budget = self.eval_max_nodes if max_nodes is None else int(max_nodes)
-        per_launch = max(1, min(_lib.EVAL_MAX_REPLICAS // copies, budget // (copies * n_nodes)))
-        L = _lib.lib()
-        launches0 = L.cbg_launch_count()
-        for r0 in range(0, len(t_values), per_launch):
-            r1 = min(len(t_values), r0 + per_launch)
-            state = self.prepare(replicate_batch(b, (r1 - r0) * copies, n_graphs), **prepare_kw)
-            coefs = (coef_type * (r1 - r0))(*[self.eval_coef(t) for t in t_values[r0:r1]])
-            with torch.cuda.device(state['device']):
-                launch(r0, r1, state, coefs)
-        self.last_launches = L.cbg_launch_count() - launches0
-
-    @staticmethod
-    def _eval_dict_mean(per_t, keys):
-        """get_dict_mean (common.py:33-42) of the per-t losses [R, len(keys)]: for each key the mean over t of its column,
-        as a CPU float32 0-d tensor."""
-        per_t = per_t.cpu()
-        return {k: torch.mean(torch.tensor(per_t[:, i].tolist())) for i, k in enumerate(keys)}
+    def _eval_plans(self, b, n_graphs, t_values, coef_type, max_nodes, launch, copies=1, **prepare_kw):
+        """``_eval_loop`` over plans of ``prepare`` (``prepare_kw`` goes to it) on replicas of the batch ``b`` of
+        ``n_graphs`` graphs."""
+        self._eval_loop(b['ligand_pos'].shape[0] + b['protein_pos'].shape[0], t_values, coef_type, max_nodes, launch,
+                        lambda n_rep: self.prepare(replicate_batch(b, n_rep, n_graphs), **prepare_kw), copies)
 
     # ---- setup of the step-invariant state ------------------------------------------------
     @torch.no_grad()
@@ -434,7 +451,7 @@ class TargetDiffB200(BaseDiffB200):
                 C.byref(state['plan']), coefs, r1 - r0, x0.data_ptr(), v0.data_ptr(), pos_noise[r0:r1].data_ptr(),
                 type_uniform[r0:r1].data_ptr(), xt[r0:r1].data_ptr(), vt[r0:r1].data_ptr(), x_pred[r0:r1].data_ptr(),
                 c_pred[r0:r1].data_ptr(), graph_loss.data_ptr(), rep_loss[r0:r1].data_ptr(), _lib.stream_ptr(dev)))
-        self._eval_loop(b, n_graphs, t_values, _lib.EvalCoef, max_nodes, launch)
+        self._eval_plans(b, n_graphs, t_values, _lib.EvalCoef, max_nodes, launch)
         loss_dict = self._eval_dict_mean(rep_loss, ('pos', 'atom'))
         results = [{'x0': x0, 'xt': xt[r], 'x_pred': x_pred[r], 'mask_gen': mask_gen,
                     'v0': v0, 'vt': vt[r], 'c_pred': c_pred[r]} for r in range(R)]
@@ -499,9 +516,9 @@ class TargetDiffB200(BaseDiffB200):
         ``traj_mode='final'`` keeps only traj[0] and traj[-1]."""
         T = self.num_diffusion_timesteps
         state = self.prepare(batch)
-        X, Cc = self._traj_buffers(state['device'], state['x_lig'], state['c_lig'])
+        X, Cc = self._traj_buffers(state['device'], (state['x_lig'], state['c_lig']))
         t_seq = list(reversed(range(T)))
         if num_steps is not None:
             t_seq = t_seq[:num_steps]
         self.run_steps(state, t_seq, X, Cc, pos_noise=pos_noise, type_uniform=type_uniform)
-        return self._traj(X, Cc, state['batch_idx_lig'], t_seq[-1], traj_mode)
+        return self._traj((X, Cc), state['batch_idx_lig'], t_seq[-1], traj_mode)

@@ -1,4 +1,5 @@
 """Shared test helpers: seeded models/batches and the golden fixtures."""
+import math
 import os
 
 import numpy as np
@@ -89,3 +90,24 @@ def assert_close(a, b, rtol=1e-4, atol=1e-5, what=''):
         i = int(torch.argmax(((a - b).abs() - rtol * b.abs()).flatten()))
         raise AssertionError(f'{what}: {int(bad.sum())} of {bad.numel()} elements outside rtol={rtol} atol={atol}; worst '
                              f'got {float(a.flatten()[i]):.7g} want {float(b.flatten()[i]):.7g}')
+
+
+def loss_close(got, want, rtol, atol=0.0, nan_equal=False):
+    """Two scalar losses agree: |got - want| <= atol + rtol |want|; with ``nan_equal`` a NaN ``want`` asks for a NaN."""
+    if nan_equal and math.isnan(want):
+        return math.isnan(got)
+    return abs(got - want) <= atol + rtol * abs(want)
+
+
+def assert_bitwise(a, b, loss_keys, nan_equal=False):
+    """Two validation-loss outputs (loss_dict, then dicts of tensors or tensors) are bit-identical: the losses of
+    ``loss_keys`` (NaN equal to NaN with ``nan_equal``) and every tensor after them."""
+    for k in loss_keys:
+        assert torch.equal(a[0][k], b[0][k]) or (nan_equal and math.isnan(float(a[0][k])) and
+                                                 math.isnan(float(b[0][k]))), k
+    for x, y in zip(a[1:], b[1:], strict=True):
+        if isinstance(x, dict):
+            for k in x:
+                assert torch.equal(x[k], y[k]), k
+        else:
+            assert torch.equal(x, y)

@@ -6,7 +6,7 @@ import pytest
 import torch
 
 import bp_eval_loss_oracle as BO
-from helpers import assert_close, case_batch, golden, stack, to_dev
+from helpers import assert_bitwise, assert_close, case_batch, golden, loss_close, stack, to_dev
 from cbgbench_b200 import synthetic
 from cbgbench_b200.diffbp import DiffBPB200
 from cbgbench_b200.targetdiff import eval_t_values
@@ -25,12 +25,6 @@ WEIGHT_SEED = 0
 # position loss of a one-atom ligand, whose zero-centred noise and prediction are both exactly 0), so a relative bar
 # alone suffices.
 LOSS_RTOL = 1e-4
-
-
-def loss_close(got, want):
-    if math.isnan(want):
-        return math.isnan(got)
-    return abs(got - want) <= LOSS_RTOL * abs(want)
 
 
 def bp_model(T, device=None, interval=None, **kw):
@@ -141,7 +135,7 @@ def test_gpu_forward_matches_reference_fixtures(case):
     for key in LOSS_KEYS:
         assert loss[key].device.type == 'cpu' and loss[key].dtype == torch.float32 and loss[key].dim() == 0
         want = float(gd[f'{name}/{key}'])
-        assert loss_close(float(loss[key]), want), (key, float(loss[key]), want)
+        assert loss_close(float(loss[key]), want, LOSS_RTOL, nan_equal=True), (key, float(loss[key]), want)
     assert len(res) == R
     assert torch.equal(stack(res, 'vt'), torch.from_numpy(gd[f'{name}/vt']))
     assert torch.equal(stack(res, 'mask_gen'), torch.from_numpy(gd[f'{name}/mask_gen']))
@@ -167,7 +161,8 @@ def check_against_oracle(model, sd, batch, t_values, noise_seed):
     loss, res = model.eval_losses(to_dev(batch), t_values, pos_noise=pn, type_uniform=tu)
     o_loss, o_res, _ = BO.eval_losses(sd, batch, t_values, pn, tu, T)
     for key in LOSS_KEYS:
-        assert loss_close(float(loss[key]), float(o_loss[key])), (key, float(loss[key]), float(o_loss[key]))
+        assert loss_close(float(loss[key]), float(o_loss[key]), LOSS_RTOL, nan_equal=True), \
+            (key, float(loss[key]), float(o_loss[key]))
     for key in ('vt', 'mask_gen', 'mask_gen_com'):
         assert torch.equal(stack(res, key), torch.stack([r[key] for r in o_res])), key
     for key in VEC_KEYS + ('c_pred',):
@@ -215,15 +210,6 @@ def run_eval(model, batch, t_values, pn, tu, **kw):
     return loss, {k: stack(res, k) for k in res[0]}
 
 
-def assert_bitwise(a, b):
-    la, ra = a
-    lb, rb = b
-    for k in LOSS_KEYS:
-        assert torch.equal(la[k], lb[k]) or (math.isnan(float(la[k])) and math.isnan(float(lb[k]))), k
-    for k in ra:
-        assert torch.equal(ra[k], rb[k]), k
-
-
 @pytest.mark.gpu
 def test_gpu_replica_batching_is_exact():
     """R replicas in one launch == R single-timestep calls == a forced split over several launches == a repeat == the
@@ -235,9 +221,10 @@ def test_gpu_replica_batching_is_exact():
     pn, tu = synthetic.make_bp_noise(len(t_values), n, seed=182)
     one = run_eval(model, batch, t_values, pn, tu)
     assert model.last_launches > 0
-    assert_bitwise(one, run_eval(model, batch, t_values, pn, tu))
+    assert_bitwise(one, run_eval(model, batch, t_values, pn, tu), LOSS_KEYS, nan_equal=True)
     n_nodes = n + batch['protein_pos'].shape[0]
-    assert_bitwise(one, run_eval(model, batch, t_values, pn, tu, max_nodes=3 * n_nodes))     # launches of 3, 3, 3, 1
+    # launches of 3, 3, 3, 1
+    assert_bitwise(one, run_eval(model, batch, t_values, pn, tu, max_nodes=3 * n_nodes), LOSS_KEYS, nan_equal=True)
     singles = [run_eval(model, batch, [t], pn[r:r + 1], tu[r:r + 1]) for r, t in enumerate(t_values)]
     for k in one[1]:
         if k in ('v0', 'mask_gen_com'):
@@ -246,7 +233,7 @@ def test_gpu_replica_batching_is_exact():
     for k in LOSS_KEYS:
         assert torch.equal(one[0][k], torch.mean(torch.tensor([float(s[0][k]) for s in singles]))), k
     model.use_prune = model.use_static_lists = False
-    assert_bitwise(one, run_eval(model, batch, t_values, pn, tu))
+    assert_bitwise(one, run_eval(model, batch, t_values, pn, tu), LOSS_KEYS, nan_equal=True)
 
 
 @pytest.mark.gpu

@@ -7,7 +7,7 @@ import pytest
 import torch
 
 import eval_loss_oracle as EO
-from helpers import assert_close, case_batch, golden, stack, to_dev, make_model
+from helpers import assert_bitwise, assert_close, case_batch, golden, loss_close, stack, to_dev, make_model
 from cbgbench_b200 import synthetic
 from cbgbench_b200.targetdiff import eval_t_values
 
@@ -24,10 +24,6 @@ EVAL_CASES = [
 # NLL -log p(v0), with p within ~1e-5 of 1.  That p comes out of a sum of exponentials near 1, so both the reference
 # and this path hold it only to about one ulp of 1 (1.2e-7), which is 1e-3 of a 2.6e-5 loss.
 LOSS_RTOL, LOSS_ATOL = 1e-4, 5e-7
-
-
-def loss_close(got, want):
-    return abs(got - want) <= LOSS_ATOL + LOSS_RTOL * abs(want)
 
 
 def per_graph_means(values, gen, batch_idx, n_graphs):
@@ -127,7 +123,7 @@ def test_gpu_forward_matches_reference_fixtures(case):
     for key in ('pos', 'atom'):
         assert loss[key].device.type == 'cpu' and loss[key].dtype == torch.float32 and loss[key].dim() == 0
         want = float(gd[f'{name}/{key}'])
-        assert loss_close(float(loss[key]), want), (key, float(loss[key]), want)
+        assert loss_close(float(loss[key]), want, LOSS_RTOL, LOSS_ATOL), (key, float(loss[key]), want)
     assert len(res) == R
     assert torch.equal(stack(res, 'vt'), torch.from_numpy(gd[f'{name}/vt']))
     for key in ('xt', 'x_pred', 'c_pred'):
@@ -154,7 +150,7 @@ def check_against_oracle(model, sd, batch, t_values, noise_seed):
         if math.isnan(want):
             assert math.isnan(float(loss[key]))
         else:
-            assert loss_close(float(loss[key]), want), (key, float(loss[key]), want)
+            assert loss_close(float(loss[key]), want, LOSS_RTOL, LOSS_ATOL), (key, float(loss[key]), want)
     assert torch.equal(stack(res, 'vt'), torch.stack([r['vt'] for r in o_res]))
     for key in ('xt', 'x_pred', 'c_pred'):
         assert_close(stack(res, key), torch.stack([r[key] for r in o_res]), what=key)
@@ -189,15 +185,6 @@ def run_eval(model, batch, t_values, pn, tu, **kw):
     return loss, {k: stack(res, k) for k in ('xt', 'vt', 'x_pred', 'c_pred')}
 
 
-def assert_bitwise(a, b):
-    la, ra = a
-    lb, rb = b
-    for k in ('pos', 'atom'):
-        assert torch.equal(la[k], lb[k]), k
-    for k in ra:
-        assert torch.equal(ra[k], rb[k]), k
-
-
 @pytest.mark.gpu
 def test_gpu_replica_batching_is_exact():
     """R replicas in one launch == R single-timestep calls == a forced split over several launches, bit for bit;
@@ -208,9 +195,10 @@ def test_gpu_replica_batching_is_exact():
     n = batch['ligand_pos'].shape[0]
     pn, tu = synthetic.make_noise(len(t_values), n, 13, seed=82)
     one = run_eval(model, batch, t_values, pn, tu)
-    assert_bitwise(one, run_eval(model, batch, t_values, pn, tu))
+    assert_bitwise(one, run_eval(model, batch, t_values, pn, tu), ('pos', 'atom'))
     n_nodes = n + batch['protein_pos'].shape[0]
-    assert_bitwise(one, run_eval(model, batch, t_values, pn, tu, max_nodes=3 * n_nodes))     # launches of 3, 3, 3, 1
+    # launches of 3, 3, 3, 1
+    assert_bitwise(one, run_eval(model, batch, t_values, pn, tu, max_nodes=3 * n_nodes), ('pos', 'atom'))
     singles = [run_eval(model, batch, [t], pn[r:r + 1], tu[r:r + 1]) for r, t in enumerate(t_values)]
     for k in one[1]:
         assert torch.equal(one[1][k], torch.cat([s[1][k] for s in singles])), k

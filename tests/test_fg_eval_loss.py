@@ -11,7 +11,7 @@ import torch
 
 import fg_eval_loss_oracle as OE
 from eval_loss_oracle import auroc as ref_auroc
-from helpers import GOLDEN as GOLDEN_DIR, assert_close
+from helpers import GOLDEN as GOLDEN_DIR, assert_close, loss_close
 from cbgbench_b200 import _lib, synthetic
 from cbgbench_b200.difffg import D3FGB200
 from cbgbench_b200.targetdiff import eval_t_values, get_model
@@ -56,12 +56,6 @@ def _inputs(name):
     batch = MK.case_batch(name)
     t_values = MK.case_t_values(name)
     return batch, t_values, MK.case_draws(name, len(t_values))
-
-
-def _loss_close(got, want):
-    if math.isnan(want):
-        return math.isnan(got)
-    return abs(got - want) <= LOSS_ATOL + LOSS_RTOL * abs(want)
 
 
 # ---- CPU ----------------------------------------------------------------------------------------------------------------
@@ -168,7 +162,8 @@ def test_cuda_matches_fixtures(case, model_name):
     key = f'{case}/{model_name}'
     for k in LOSS_KEYS:
         assert loss[k].dtype == torch.float32 and loss[k].dim() == 0 and loss[k].device.type == 'cpu'
-        assert _loss_close(float(loss[k]), float(g[f'{key}/{k}'])), (k, float(loss[k]), float(g[f'{key}/{k}']))
+        assert loss_close(float(loss[k]), float(g[f'{key}/{k}']), LOSS_RTOL, LOSS_ATOL, nan_equal=True), \
+            (k, float(loss[k]), float(g[f'{key}/{k}']))
     pos_keys = ['eps_0', 'eps_pred', 'score_0', 'score_pred'] if model_name == 'difffg' else ['x0', 'xt', 'x_pred']
     assert len(res) == len(t_values)
     gen = batch.get('ligand_gen_flag', batch['ligand_lig_flag'])

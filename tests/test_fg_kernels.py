@@ -547,6 +547,19 @@ def test_ipa_forward_refuses_k_outside_1_32(k):
     assert rc != 0 and f'k={k}' in L.cbg_last_error().decode()
 
 
+def test_fg_workspace_bytes_cover_the_carve():
+    """cbg_fg_workspace_bytes = the IPATransformer scratch + the five encoder row arrays (eps_pos, o_pred, h, R_next,
+    logits), each rounded up to 256 bytes: the size fg_rows carves for cbg_fg_step_f32 and cbg_fg_eval_loss_f32."""
+    L = _lib.lib()
+    al = lambda b: (b + 255) // 256 * 256
+    for n in (1, 2, 5, 63, 64, 65, 1000, 4097, 100_003, 1 << 20):
+        for H in (128, 256):
+            for K in (1, 28, 32):
+                want = L.cbg_ipa_workspace_bytes(n, H) + 2 * al(n * 3 * 4) + al(n * H * 4) + al(n * 9 * 4) + al(n * K * 4)
+                got = L.cbg_fg_workspace_bytes(n, H, K)
+                assert got == want and got % 256 == 0, (n, H, K, got, want)
+
+
 def test_fg_reverse_refusals():
     L = _lib.lib()
     nil = [None] * 12

@@ -7,7 +7,7 @@ import pytest
 import torch
 
 import sbdd_eval_loss_oracle as SO
-from helpers import assert_close, case_batch, golden, stack, to_dev
+from helpers import assert_bitwise, assert_close, case_batch, golden, loss_close, stack, to_dev
 from cbgbench_b200 import synthetic
 from cbgbench_b200.diffsbdd import DiffSBDDB200, eval_t_values
 
@@ -30,10 +30,6 @@ VEC_KEYS = ('eps_0_pos', 'eps_pred_pos', 'score_0_pos', 'score_pred_pos',
 # values here and in the reference except the fixed-order sum |alpha_T x0|^2, so the two results differ by a few ulps of
 # the summands (ulp(128) = 1.5e-5): the terms get an absolute 5e-5 beside the relative 1e-4.
 LOSS_RTOL, TERM_ATOL = 1e-4, 5e-5
-
-
-def loss_close(got, want):
-    return abs(got - want) <= LOSS_RTOL * abs(want)
 
 
 def sbdd_model(T, device=None, interval=None, **kw):
@@ -118,7 +114,7 @@ def test_gpu_forward_matches_reference_fixtures(case):
     for key in LOSS_KEYS:
         assert loss[key].device.type == 'cpu' and loss[key].dtype == torch.float32 and loss[key].dim() == 0
         want = float(gd[f'{name}/{key}'])
-        assert loss_close(float(loss[key]), want), (key, float(loss[key]), want)
+        assert loss_close(float(loss[key]), want, LOSS_RTOL), (key, float(loss[key]), want)
     assert_close(model.last_terms.cpu(), torch.from_numpy(gd[f'{name}/terms']), rtol=LOSS_RTOL, atol=TERM_ATOL, what='terms')
     assert len(res) == R
     for key in VEC_KEYS:
@@ -140,7 +136,7 @@ def check_against_oracle(model, sd, batch, t_values, noise_seed):
     loss, res = model.eval_losses(to_dev(batch), t_values, noise=noise)
     o_loss, o_res, _, o_terms = SO.eval_losses(sd, batch, t_values, noise, T, K)
     for key in LOSS_KEYS:
-        assert loss_close(float(loss[key]), float(o_loss[key])), (key, float(loss[key]), float(o_loss[key]))
+        assert loss_close(float(loss[key]), float(o_loss[key]), LOSS_RTOL), (key, float(loss[key]), float(o_loss[key]))
     assert_close(model.last_terms.cpu(), o_terms, rtol=LOSS_RTOL, atol=TERM_ATOL, what='terms')
     for key in ('mask_gen_pos', 'mask_gen_atom'):
         assert torch.equal(stack(res, key), torch.stack([r[key] for r in o_res])), key
@@ -181,14 +177,6 @@ def run_eval(model, batch, t_values, noise, **kw):
     return loss, {k: stack(res, k) for k in res[0]}, model.last_terms.cpu()
 
 
-def assert_bitwise(a, b):
-    for k in LOSS_KEYS:
-        assert torch.equal(a[0][k], b[0][k]), k
-    for k in a[1]:
-        assert torch.equal(a[1][k], b[1][k]), k
-    assert torch.equal(a[2], b[2])
-
-
 @pytest.mark.gpu
 def test_gpu_replica_batching_is_exact():
     """2R copies in one launch == R single-timestep calls == a forced split over several launches == a repeat == the
@@ -200,9 +188,9 @@ def test_gpu_replica_batching_is_exact():
     noise = synthetic.make_sbdd_eval_noise(len(t_values), n, K, seed=282)
     one = run_eval(model, batch, t_values, noise)
     assert model.last_launches > 0
-    assert_bitwise(one, run_eval(model, batch, t_values, noise))
+    assert_bitwise(one, run_eval(model, batch, t_values, noise), LOSS_KEYS)
     n_nodes = n + batch['protein_pos'].shape[0]
-    assert_bitwise(one, run_eval(model, batch, t_values, noise, max_nodes=6 * n_nodes))    # 3, 3, 3, 1 timesteps
+    assert_bitwise(one, run_eval(model, batch, t_values, noise, max_nodes=6 * n_nodes), LOSS_KEYS)    # 3, 3, 3, 1 timesteps
     singles = [run_eval(model, batch, [t], {k: v[r:r + 1] for k, v in noise.items()}) for r, t in enumerate(t_values)]
     for k in one[1]:
         if k.startswith('mask_gen'):
@@ -212,7 +200,7 @@ def test_gpu_replica_batching_is_exact():
     for k in LOSS_KEYS:
         assert torch.equal(one[0][k], torch.mean(torch.tensor([float(s[0][k]) for s in singles]))), k
     model.use_prune = False
-    assert_bitwise(one, run_eval(model, batch, t_values, noise))
+    assert_bitwise(one, run_eval(model, batch, t_values, noise), LOSS_KEYS)
 
 
 @pytest.mark.gpu
