@@ -88,10 +88,19 @@ constexpr uint32_t SM_LN = SM_G + 4 * G_IMG;          // gamma * 64 [128] | beta
 constexpr uint32_t SM_B1 = SM_LN + 1024;              // b1v [128]
 constexpr uint32_t SM_RBF = SM_B1 + 512;              // Gaussian offsets [20] + coeff
 constexpr uint32_t SM_EPI = SM_RBF + 128;             // k: [node slot][32 edges][17] logits; v: [slot][warp][128] partial sums; xv: [slot][warp][4]
+// Staged node-plane rows of the tile in flight, per warp: the Pi row of its node, then the Pj rows of its accumulator
+// rows e0 (row r = lane / 4).  The Pj rows are 512 + 32 bytes apart, so that the 64-bit accumulator-layout reads of a
+// half-warp (rows r .. r + 3) fall on 32 different banks.
+constexpr uint32_t P_ROW = CBG_H * 4;                 // one fp32 node-plane row, bytes
+constexpr uint32_t STG_WARP = P_ROW + 8 * (P_ROW + 32);
 constexpr uint32_t SM_BAR = SM_EPI + 4 * 32 * 17 * 4;
-constexpr uint32_t SM_TOTAL = SM_BAR + 64;
-static_assert(SM_TOTAL <= 232448, "shared memory budget");
-enum { B_WFULL = 0 /* Wg images */, B_W1FULL /* W1 images */ };
+constexpr uint32_t SM_STG = SM_BAR + 128;             // [warp][Pi | Pj rows 0 .. 7]
+// STAGE: the whole layout; !STAGE ends before the staging slots, so its shared-memory carve-out (and L1) stays as it was
+constexpr uint32_t sm_total(bool stage) { return stage ? SM_STG + 8 * STG_WARP : SM_STG; }
+static_assert(sm_total(true) <= 232448, "shared memory budget");
+static_assert(SM_STG % 16 == 0 && STG_WARP % 16 == 0, "bulk-copy destinations are 16-byte aligned");
+enum { B_WFULL = 0 /* Wg images */, B_W1FULL /* W1 images */, B_STG /* + warp: staged rows of the warp */ };
+__host__ __device__ constexpr uint32_t stg_pj_row(int r) { return P_ROW + (P_ROW + 32u) * (uint32_t)r; }
 
 __device__ __forceinline__ int list_len(const EdgeArgs& p) {
   int n = p.n_nodes;
@@ -144,7 +153,10 @@ __device__ __forceinline__ float2 ldg2(const float* p) { return __ldg(reinterpre
   } while (0)
 
 // =================================================================================================================
-template <int MODE>
+// STAGE: the Pi row and the Pj rows of accumulator row e0 reach S1 through shared memory (bulk copies issued one tile
+// ahead); the Pj rows of e0 + 8 through registers.  !STAGE (MODE_V, or any mode under CBG_X2H_STAGE=0): Pi + Pj of both
+// rows gathered into registers during the previous epilogue.  Same values, same arithmetic: bit-identical results.
+template <int MODE, bool STAGE>
 __global__ void __launch_bounds__(256, 1) x2h_tc_kernel(EdgeArgs p, TcWeights W) {
   constexpr bool IS_V = MODE == MODE_V, IS_XV = MODE == MODE_XV;
   extern __shared__ __align__(1024) uint8_t smem[];
@@ -163,6 +175,9 @@ __global__ void __launch_bounds__(256, 1) x2h_tc_kernel(EdgeArgs p, TcWeights W)
   if (tid == 32) {
     mbar_init(bar(B_WFULL), 1);
     mbar_init(bar(B_W1FULL), 1);
+    if constexpr (STAGE) {
+      for (int w = 0; w < 8; ++w) mbar_init(bar(B_STG + w), 1);
+    }
     fence_mbar_init();
     // Resident weight images by bulk (TMA) copies.  Wg first on its own barrier: MMA1 of the first tile needs only Wg,
     // W1 is not read before MMA2.  Every CTA of the grid reads the same 112 KB at the same moment, so each image goes
@@ -290,24 +305,50 @@ __global__ void __launch_bounds__(256, 1) x2h_tc_kernel(EdgeArgs p, TcWeights W)
     const float2 b1 = ldg2(pj_plane + (size_t)(tj1 >= 0 ? tj1 : ti) * CBG_H + 2 * qt + 8 * j);
     v[4 * j] = a.x + b0.x; v[4 * j + 1] = a.y + b0.y; v[4 * j + 2] = a.x + b1.x; v[4 * j + 3] = a.y + b1.y;
   };
+  // STAGE: bulk copies of a tile's Pi row and the warp's eight e0 Pj rows into the warp's staging slot, completing on
+  // the warp's barrier (one phase per tile).  The caller guarantees that every lane has read the slot's previous rows.
+  const uint32_t stg = sbase + SM_STG + (uint32_t)warp * STG_WARP;
+  const uint8_t* s_stg = smem + SM_STG + (uint32_t)warp * STG_WARP;
+  auto stage_rows = [&](int sti, int stj0) {
+    __syncwarp();
+    if (lane == 0) mbar_expect_tx(bar(B_STG + warp), 9 * P_ROW);
+    if (qt == 0) bulk_g2s(stg + stg_pj_row(qg), pj_plane + (size_t)(stj0 >= 0 ? stj0 : sti) * CBG_H, P_ROW, bar(B_STG + warp));
+    else if (lane == 1) bulk_g2s(stg, pi_plane + (size_t)sti * CBG_H, P_ROW, bar(B_STG + warp));
+  };
+  // STAGE: Pj of accumulator row e0 + 8 into registers, columns 8 j + 2 qt, + 1 (S1 adds Pi)
+  auto gather_pj1 = [&](float (&b)[32], int sti, int stj1) {
+    const float* r = pj_plane + (size_t)(stj1 >= 0 ? stj1 : sti) * CBG_H + 2 * qt;
+#pragma unroll
+    for (int j = 0; j < 16; ++j) { const float2 t = ldg2(r + 8 * j); b[2 * j] = t.x; b[2 * j + 1] = t.y; }
+  };
 
   // ---- software pipeline over this CTA's tiles.  Per warpgroup, tile k:
   //   wait MMA1(k), S1(k), issue MMA2(k) | load the coordinates of k+1, build G(k+1) while MMA2(k) runs | wait MMA2(k),
   //   issue MMA1(k+1) | epilogue(k) while MMA1(k+1) runs (it issues the Pi + Pj gathers of k+1 as it frees registers)
   // The G buffer is free once every warp of the warpgroup has completed MMA1(k) (MMA2 reads no G), and the s_epi slots once
   // every warp has finished epilogue(k-1): one warpgroup barrier after the MMA2 issue orders both.
-  float d[64], v[64];        // MMA1 accumulator and Pi + Pj of the tile in flight
+  // STAGE: the staged rows of tile k+1 are copied as soon as S1(k) has read those of tile k, and the e0 + 8 Pj row is
+  // loaded behind MMA2(k): each gets most of a tile period to land.
+  float d[64];               // MMA1 accumulator of the tile in flight
+  float v[64];               // Pi + Pj of the tile in flight
+  float pj1[32];             // STAGE: Pj of row e0 + 8 of the tile in flight
   int ti = 0, tj0 = 0, tj1 = 0;                        // node / neighbours of this thread's accumulator rows, tile k
   int ngi = 0, ngjn = 0, nti = 0, ntj0 = 0, ntj1 = 0;  // the same of tile k+1, and its G-row node / neighbour
   if (n_my > 0) {          // prologue: tile 0 up to its MMA1 issue
     int gi, gjn;
     load_idx(0, gi, gjn, ti, tj0, tj1);
+    if constexpr (STAGE) {
+      stage_rows(ti, tj0);
+      gather_pj1(pj1, ti, tj1);
+    }
     build_g(p.x4[gi], p.x4[gjn >= 0 ? gjn : gi]);
     fence_proxy_async();
     warpgroup_sync(wg);
     issue_mma1(d);
+    if constexpr (!STAGE) {
 #pragma unroll
-    for (int j = 0; j < 16; ++j) gather_p(v, j, ti, tj0, tj1);
+      for (int j = 0; j < 16; ++j) gather_p(v, j, ti, tj0, tj1);
+    }
   }
   // one tile; `more` (a compile-time constant: the last tile is peeled) says whether a tile k+1 follows, so the compiler
   // sees exactly where d and v are redefined and keeps neither live across the drain
@@ -327,6 +368,17 @@ __global__ void __launch_bounds__(256, 1) x2h_tc_kernel(EdgeArgs p, TcWeights W)
     uint32_t a_hi[8][4], a_lo[8][4];
     {
       float q0 = 0.f, q1 = 0.f;
+      if constexpr (STAGE) {     // Pi + Pj from the staged rows and pj1, added as gather_p adds them
+        mbar_wait(bar(B_STG + warp), (uint32_t)k & 1u);
+        const float* s_pi = reinterpret_cast<const float*>(s_stg) + 2 * qt;
+        const float* s_pj = reinterpret_cast<const float*>(s_stg + stg_pj_row(qg)) + 2 * qt;
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+          const float2 a = *reinterpret_cast<const float2*>(s_pi + 8 * j);
+          const float2 b0 = *reinterpret_cast<const float2*>(s_pj + 8 * j);
+          v[4 * j] = a.x + b0.x; v[4 * j + 1] = a.y + b0.y; v[4 * j + 2] = a.x + pj1[2 * j]; v[4 * j + 3] = a.y + pj1[2 * j + 1];
+        }
+      }
 #pragma unroll
       for (int j = 0; j < 16; ++j) {
         v[4 * j] = fmaf(d[4 * j], kInvPre, v[4 * j]);
@@ -379,6 +431,10 @@ __global__ void __launch_bounds__(256, 1) x2h_tc_kernel(EdgeArgs p, TcWeights W)
     };
     // ---- while MMA2(k) runs: G(k+1); then MMA2(k) complete, MMA1(k+1) issued
     auto advance = [&](auto& o) {
+      if constexpr (more && STAGE) {
+        stage_rows(nti, ntj0);                         // S1(k) has read the slot: the __syncwarp in stage_rows orders it
+        gather_pj1(pj1, nti, ntj1);
+      }
       if constexpr (more) {
         const float4 xi = p.x4[ngi], xj = p.x4[ngjn >= 0 ? ngjn : ngi];
         warpgroup_sync(wg);                            // MMA1(k) complete and epilogue(k-1) done in every warp
@@ -399,7 +455,7 @@ __global__ void __launch_bounds__(256, 1) x2h_tc_kernel(EdgeArgs p, TcWeights W)
     // ---- epilogue(k) from the MMA2 fragment, while MMA1(k+1) runs.  The Pi + Pj gathers of k+1 are issued column
     // group by column group as the epilogue frees the fragment registers of the same group: they start early, and o and
     // v are never both live in full
-    auto gather_next = [&](int j) { if constexpr (more) gather_p(v, j, nti, ntj0, ntj1); };
+    auto gather_next = [&](int j) { if constexpr (more && !STAGE) gather_p(v, j, nti, ntj0, ntj1); };
     if constexpr (MODE == MODE_K) {
       // attention weights: <q_i, k> per head (a head's 8 columns = one quad's registers), softmax over the node's 32
       // edges through shared memory, w = alpha * e_w
@@ -598,12 +654,20 @@ __global__ void __launch_bounds__(128, 1) wgmma_selftest_kernel(const __half* a,
 }
 
 int g_tc_sms = 0;
+bool g_tc_stage = true;      // CBG_X2H_STAGE=0: the register-gather path in every mode
 long long* g_tc_trace = nullptr;
 int g_tc_trace_tiles = 0;
 
+// MODE_V always gathers into registers: staging measured slower there on H100 (DESIGN §5.2), faster in MODE_K
 template <int MODE>
 void launch_tc(int grid, cudaStream_t st, const EdgeArgs& a, const TcWeights& w) {
-  cbg_launch_pdl(x2h_tc_kernel<MODE>, dim3(grid), dim3(256), SM_TOTAL, st, a, w);
+  if constexpr (MODE != MODE_V) {
+    if (g_tc_stage) {
+      cbg_launch_pdl(x2h_tc_kernel<MODE, true>, dim3(grid), dim3(256), sm_total(true), st, a, w);
+      return;
+    }
+  }
+  cbg_launch_pdl(x2h_tc_kernel<MODE, false>, dim3(grid), dim3(256), sm_total(false), st, a, w);
 }
 
 int tc_init() {
@@ -613,8 +677,10 @@ int tc_init() {
   int dev = 0;
   CBG_CUDA_OK(cudaGetDevice(&dev));
   CBG_CUDA_OK(cudaDeviceGetAttribute(&g_tc_sms, cudaDevAttrMultiProcessorCount, dev));
-#define TC_ATTR(MODE) CBG_CUDA_OK(cudaFuncSetAttribute(x2h_tc_kernel<MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SM_TOTAL))
-  TC_ATTR(MODE_K); TC_ATTR(MODE_V); TC_ATTR(MODE_XV);
+  if (const char* e = getenv("CBG_X2H_STAGE")) g_tc_stage = strcmp(e, "0") != 0;
+#define TC_ATTR(MODE, STAGE) CBG_CUDA_OK(cudaFuncSetAttribute(x2h_tc_kernel<MODE, STAGE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm_total(STAGE)))
+  TC_ATTR(MODE_K, true); TC_ATTR(MODE_XV, true);
+  TC_ATTR(MODE_K, false); TC_ATTR(MODE_V, false); TC_ATTR(MODE_XV, false);
 #undef TC_ATTR
   done = true;
   return 0;
