@@ -110,7 +110,7 @@ class DiffBPB200(BaseDiffB200):
         tensors eps_0, eps_pred, score_0, score_pred, mask_gen (the type mask), v0, vt (one-hot float), c_pred, and
         eps_0_com, eps_pred_com, score_0_com, score_pred_com, mask_gen_com (the generation flag).  A t whose batch has no
         generated atom gets NaN pos / com losses; a t without masked atoms (every t = 0) an atom loss of 0, like the
-        reference.
+        reference.  ``last_rep_loss`` then holds the per-t losses [R, 4] in the order pos, atom, com, inter.
 
         The denoiser is not conditioned on t, so the R = len(t_values) noised copies go through ONE denoiser pass as
         R*B graphs, split over several launches above ``max_nodes`` composed nodes (default ``eval_max_nodes``) or 64
@@ -146,6 +146,7 @@ class DiffBPB200(BaseDiffB200):
                 vt[r0:r1].data_ptr(), mask[r0:r1].data_ptr(), vec[r0:r1].data_ptr(), c_pred[r0:r1].data_ptr(),
                 rep_loss[r0:r1].data_ptr(), _lib.stream_ptr(dev)))
         self._eval_plans(b, n_graphs, t_values, _lib.BpEvalCoef, max_nodes, launch)
+        self.last_rep_loss = rep_loss
         loss_dict = self._eval_dict_mean(rep_loss, ('pos', 'atom', 'com', 'inter'))
         vt_onehot = F.one_hot(vt, K).float()
         # the reference's key order: pos_info, then atom_info (its mask_gen, the type mask, replaces gen), then com_info

@@ -422,7 +422,8 @@ class TargetDiffB200(BaseDiffB200):
         per t).  Returns ``(loss_dict, results)`` like the reference's eval-mode forward: ``loss_dict`` = {'pos', 'atom'}
         as CPU 0-d float32 tensors (mean over t of the per-t losses), ``results`` one dict per t with the device tensors
         x0, xt, x_pred, mask_gen, v0, vt, c_pred.  A t whose batch has no generated atom gets NaN losses, like the
-        reference's mean of an empty tensor.
+        reference's mean of an empty tensor.  ``last_graph_loss`` then holds the per-graph position and type losses
+        [R, B, 2] (means over each graph's generated atoms, 0 for a graph without one).
 
         The denoiser is not conditioned on t, so the R = len(t_values) noised copies of the batch go through ONE
         denoiser pass as R*B graphs.  When R copies would exceed ``max_nodes`` composed nodes (default
@@ -443,15 +444,16 @@ class TargetDiffB200(BaseDiffB200):
         x_pred = torch.empty(R, n_lig, 3, device=dev)
         c_pred = torch.empty(R, n_lig, K, device=dev)
         rep_loss = torch.empty(R, 2, device=dev)
+        graph_loss = torch.empty(R, n_graphs, 2, device=dev)
         L = _lib.lib()
 
         def launch(r0, r1, state, coefs):
-            graph_loss = torch.empty((r1 - r0) * n_graphs, 2, device=dev)
             _lib.check(L.cbg_eval_loss_f32(
                 C.byref(state['plan']), coefs, r1 - r0, x0.data_ptr(), v0.data_ptr(), pos_noise[r0:r1].data_ptr(),
                 type_uniform[r0:r1].data_ptr(), xt[r0:r1].data_ptr(), vt[r0:r1].data_ptr(), x_pred[r0:r1].data_ptr(),
-                c_pred[r0:r1].data_ptr(), graph_loss.data_ptr(), rep_loss[r0:r1].data_ptr(), _lib.stream_ptr(dev)))
+                c_pred[r0:r1].data_ptr(), graph_loss[r0:r1].data_ptr(), rep_loss[r0:r1].data_ptr(), _lib.stream_ptr(dev)))
         self._eval_plans(b, n_graphs, t_values, _lib.EvalCoef, max_nodes, launch)
+        self.last_graph_loss = graph_loss
         loss_dict = self._eval_dict_mean(rep_loss, ('pos', 'atom'))
         results = [{'x0': x0, 'xt': xt[r], 'x_pred': x_pred[r], 'mask_gen': mask_gen,
                     'v0': v0, 'vt': vt[r], 'c_pred': c_pred[r]} for r in range(R)]
